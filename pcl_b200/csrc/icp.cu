@@ -6,14 +6,16 @@
 //       common/impl/eigen.hpp:675-734; or impl/transformation_estimation_point_to_plane_lls.hpp:166-268)
 //   transformCloud (impl/icp.hpp:49-111) ; final = T_k * final (:223) ; convergence (:238)
 //
-// One iteration here = ONE streaming kernel over the Morton-ordered source:
+// One iteration here = a search kernel over the Morton-ordered source:
 //   [apply the previous iteration's T_k to the point, in the reference's fp32 operation order, and
-//    write it back]  ->  exact 1-NN in the LBVH with the gate as the initial bound  ->  fp64 accumulation of
-//   the 17 (Umeyama) or 29 (point-to-plane) sums  ->  warp/block/grid reduction with a FIXED order
-//   (deterministic), last block folds the per-block partials
-// followed (after the cross-GPU all-reduce, if any) by a one-warp solve kernel that leaves T_k in
-// device memory for the next iteration.  The host only reads back ~200 bytes per iteration to run
-// DefaultConvergenceCriteria (default_convergence_criteria.hpp:49-140) in the caller's Scalar.
+//    write it back]  ->  exact 1-NN in the LBVH with the gate as the initial bound
+// then an accumulation kernel: fp64 sums of the 17 (Umeyama) or 29 (point-to-plane) terms, warp/block/grid
+// reduction with a FIXED order (deterministic), last block folds the per-block partials; then (after the
+// cross-GPU all-reduce, if any) a one-warp solve kernel that leaves T_k in device memory for the next
+// iteration and does the loop's bookkeeping in its tail: final = T_k * final, the iteration count and
+// DefaultConvergenceCriteria (default_convergence_criteria.hpp:49-140) in the caller's Scalar, on a LoopCtrl in
+// device memory.  icp_iterate enqueues the iterations and synchronises once per call, or once per iteration
+// when a stage between search and solve needs the host.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -155,18 +157,6 @@ float gate_from_max_dist(double max_dist)
   return g;
 }
 
-// C = A*B row-major, Eigen coefficient order, in Scalar S (final = T_k * final, icp.hpp:223)
-template <typename S>
-static void mat4_mul(const S* A, const S* B, S* C)
-{
-  S R[16];
-  for (int r = 0; r < 4; ++r)
-    for (int c = 0; c < 4; ++c)
-      R[4 * r + c] = ((A[4 * r] * B[c] + A[4 * r + 1] * B[4 + c]) + A[4 * r + 2] * B[8 + c]) + A[4 * r + 3] * B[12 + c];
-  for (int i = 0; i < 16; ++i)
-    C[i] = R[i];
-}
-
 struct Reducer {  // scratch for block_reduce_and_publish
   DevBuf<double> partials;
   DevBuf<double> partials2;  // max_blocks * 128 (k_accum_dmma)
@@ -206,34 +196,23 @@ struct Icp {
   DevBuf<float4> cur;           // Morton order, w = slot
   DevBuf<float4> cur_normals;   // source normals in the order of `cur` (symmetric objective only)
   DevBuf<Match> match;          // Morton order: this iteration's matches = next iteration's seeds
-  DevBuf<LoopCtrl> ctrl;        // device-side loop state of the enqueue-ahead path (icp_iterate)
+  DevBuf<LoopCtrl> ctrl;        // device copy of `loop` for one icp_iterate call: k_solve advances it every iteration
   DevBuf<float> lb;             // per query: lower bound on the distance to every OTHER target point (TRACK searches)
-  bool lb_valid = false;        // lb was written by the previous search
   DevBuf<int32_t> cur_label;    // Morton order: original source index of cur[i] (labels of the reciprocal tree)
   bool have_src_normals = false;
   DevBuf<unsigned char> src_raw; // the caller's records verbatim (kept when stride != 16) for output = *input_
   size_t src_stride = 0;
   ptrdiff_t src_normal_off = -1; // byte offset of nx inside a record, when the normals live in the same records
-  int64_t total_corr = 0;
   // device state
   DevBuf<Pending> pending;
   DevBuf<SolveOut> solve_out;
   DevBuf<unsigned long long> skip_count;
   int64_t total_skipped = 0;
-  int searches = 0;             // search launches since set_source (the first one has no seeds)
   std::vector<pclb200_rejector> rejectors;  // applied in order after every search (icp.hpp:187-201)
-  bool track_next = false;      // run the next search with lower-bound tracking / skip test (set per iteration)
   Reducer red;
-  // host state (Scalar-typed values are kept in double; float mode rounds after every operation)
-  double final_T[16], last_T[16];
-  int iterations = 0;
-  int state = PCLB200_CONV_NOT_CONVERGED;
-  bool converged = false;
-  int64_t n_corr = 0;
-  double mse = 0.0;
-  // DefaultConvergenceCriteria state
-  double prev_mse = std::numeric_limits<double>::max();
-  int iterations_similar = 0;
+  // the loop state between icp_iterate calls (Scalar-typed values are kept in double; float mode rounds after every
+  // operation): counters, DefaultConvergenceCriteria state, final / last transform, tracking decision
+  LoopCtrl loop;
 };
 
 static void set_identity(double* T)
@@ -262,6 +241,23 @@ static void upload_pending(Icp& s, const double* T, int apply)
   PCLB_CUDA(cudaStreamSynchronize(s.ctx->stream));  // h is a stack object
 }
 
+void icp_reset_state(Icp& s, const double* guess)
+{
+  LoopCtrl& L = s.loop;
+  memset(&L, 0, sizeof(L));
+  L.state = PCLB200_CONV_NOT_CONVERGED;
+  L.prev_mse = std::numeric_limits<double>::max();
+  set_identity(L.last_T);
+  if (guess) {
+    for (int i = 0; i < 16; ++i)
+      L.final_T[i] = s.P.scalar_is_double ? guess[i] : (double)(float)guess[i];
+  }
+  else
+    set_identity(L.final_T);
+  s.total_skipped = 0;
+  PCLB_CUDA(cudaMemsetAsync(s.skip_count.p, 0, sizeof(unsigned long long), s.ctx->stream));
+}
+
 Icp* icp_create(Ctx& c, const pclb200_icp_params& P)
 {
   std::unique_ptr<Icp> s(new Icp());
@@ -271,11 +267,9 @@ Icp* icp_create(Ctx& c, const pclb200_icp_params& P)
   s->solve_out.alloc(1, c.stream);
   s->ctrl.alloc(1, c.stream);
   s->skip_count.alloc(1, c.stream);
-  PCLB_CUDA(cudaMemsetAsync(s->skip_count.p, 0, sizeof(unsigned long long), c.stream));
   s->red.init(c, (unsigned)c.sm_count * 16);
-  set_identity(s->final_T);
-  set_identity(s->last_T);
-  upload_pending(*s, s->final_T, 0);
+  icp_reset_state(*s, nullptr);
+  upload_pending(*s, s->loop.final_T, 0);
   return s.release();
 }
 
@@ -397,30 +391,6 @@ __global__ void k_gather_subset(const float4* __restrict__ all, const int32_t* _
     out[i] = all[sub[i]];
 }
 
-void icp_reset_state(Icp& s, const double* guess)
-{
-  set_identity(s.last_T);
-  if (guess) {
-    for (int i = 0; i < 16; ++i)
-      s.final_T[i] = s.P.scalar_is_double ? guess[i] : (double)(float)guess[i];
-  }
-  else
-    set_identity(s.final_T);
-  s.iterations = 0;
-  s.state = PCLB200_CONV_NOT_CONVERGED;
-  s.converged = false;
-  s.n_corr = 0;
-  s.track_next = false;
-  s.lb_valid = false;
-  s.total_skipped = 0;
-  s.searches = 0;
-  PCLB_CUDA(cudaMemsetAsync(s.skip_count.p, 0, sizeof(unsigned long long), s.ctx->stream));
-  s.total_corr = 0;
-  s.mse = 0.0;
-  s.prev_mse = std::numeric_limits<double>::max();
-  s.iterations_similar = 0;
-}
-
 void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
                     const int32_t* indices, size_t n_idx, const double* guess)
 {
@@ -495,7 +465,6 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   s.match.alloc(s.n_q, st);
   PCLB_CUDA(cudaMemsetAsync(s.match.p, 0xff, s.n_q * sizeof(Match), st));  // pos = -1: no seed yet
   s.lb.alloc(s.n_q, st);
-  s.lb_valid = false;
   s.cur_label.alloc(s.n_q, st);
   if (s.n_q) {
     k_cur_labels<<<grid_for(s.n_q, 256), 256, 0, st>>>(s.cur.p, s.src_orig.p, s.n_q, s.cur_label.p);
@@ -506,14 +475,14 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   bool guess_identity = true;
   if (guess)
     for (int i = 0; i < 16; ++i)
-      if (s.final_T[i] != ((i % 5 == 0) ? 1.0 : 0.0))
+      if (s.loop.final_T[i] != ((i % 5 == 0) ? 1.0 : 0.0))
         guess_identity = false;
   if (!guess_identity) {
-    upload_pending(s, s.final_T, 1);
+    upload_pending(s, s.loop.final_T, 1);
     k_apply_pending<<<persistent_grid(c, s.n_q, 256, 8), 256, 0, st>>>(s.cur.p, s.n_q, s.pending.p, s.cur_normals.p);
     ++c.launches;
   }
-  upload_pending(s, s.last_T, 0);
+  upload_pending(s, s.loop.last_T, 0);
   PCLB_CUDA(cudaGetLastError());
 }
 
@@ -528,81 +497,29 @@ static void check_device_error(Ctx& c)
   }
 }
 
-// DefaultConvergenceCriteria::hasConverged — impl/default_convergence_criteria.hpp:49-140.
-// T is the current T_k in Scalar (stored as doubles; float mode: exactly representable floats).
-template <typename S>
-static bool has_converged(Icp& s, const double* Td)
-{
-  const pclb200_icp_params& P = s.P;
-  if (s.state != PCLB200_CONV_NOT_CONVERGED) {
-    s.iterations_similar = 0;
-    s.state = PCLB200_CONV_NOT_CONVERGED;
-  }
-  bool is_similar = false;
-  if (s.iterations >= P.max_iterations) {
-    if (!P.failure_after_max_iter) {
-      s.state = PCLB200_CONV_ITERATIONS;
-      return true;
-    }
-    s.state = PCLB200_CONV_FAILURE_AFTER_MAX_ITERATIONS;
-  }
-  S T[16];
-  for (int i = 0; i < 16; ++i)
-    T[i] = static_cast<S>(Td[i]);
-  const double rotation_threshold = P.transformation_rotation_epsilon > 0 ? P.transformation_rotation_epsilon : 0.99999;
-  const double translation_threshold = P.transformation_epsilon;
-  const double mse_threshold_relative = P.euclidean_fitness_epsilon;
-  const double mse_threshold_absolute = P.mse_threshold_absolute;
-  double cos_angle = 0.5 * (T[0] + T[5] + T[10] - 1);
-  double translation_sqr = T[3] * T[3] + T[7] * T[7] + T[11] * T[11];
-  if (cos_angle >= rotation_threshold && translation_sqr <= translation_threshold) {
-    if (s.iterations_similar >= P.max_iterations_similar_transforms) {
-      s.state = PCLB200_CONV_TRANSFORM;
-      return true;
-    }
-    is_similar = true;
-  }
-  const double cur_mse = s.mse;
-  if (std::abs(cur_mse - s.prev_mse) < mse_threshold_absolute) {
-    if (s.iterations_similar >= P.max_iterations_similar_transforms) {
-      s.state = PCLB200_CONV_ABS_MSE;
-      return true;
-    }
-    is_similar = true;
-  }
-  if (std::abs(cur_mse - s.prev_mse) / s.prev_mse < mse_threshold_relative) {
-    if (s.iterations_similar >= P.max_iterations_similar_transforms) {
-      s.state = PCLB200_CONV_REL_MSE;
-      return true;
-    }
-    is_similar = true;
-  }
-  if (is_similar)
-    ++s.iterations_similar;
-  else
-    s.iterations_similar = 0;
-  s.prev_mse = cur_mse;
-  return false;
-}
-
 static void fill_stats(const Icp& s, pclb200_icp_stats* st)
 {
   if (!st)
     return;
-  st->converged = s.converged ? 1 : 0;
-  st->state = s.state;
-  st->iterations = s.iterations;
+  const LoopCtrl& L = s.loop;
+  st->converged = L.converged ? 1 : 0;
+  st->state = L.state;
+  st->iterations = L.iterations;
   st->reserved = 0;
-  st->n_correspondences = s.n_corr;
-  st->total_correspondences = s.total_corr;
+  st->n_correspondences = (int64_t)L.n_corr;
+  st->total_correspondences = L.total_corr;
   st->total_skipped_walks = s.total_skipped;
-  st->mse = s.mse;
+  st->mse = L.mse;
   for (int i = 0; i < 16; ++i) {
-    st->final_transformation[i] = s.final_T[i];
-    st->last_transformation[i] = s.last_T[i];
+    st->final_transformation[i] = L.final_T[i];
+    st->last_transformation[i] = L.last_T[i];
   }
 }
 
+// The do-while of icp.hpp:164-241.  Every iteration enqueues correspondence estimation -> rejector chain -> accumulation
+// -> (NCCL all-reduce) -> k_solve, and k_solve's tail does the loop's bookkeeping on the device copy of the loop state:
+// final = T_k * final, the iteration count, DefaultConvergenceCriteria, the tracking decision and the correspondence
+// totals.  Once a criterion fires `done` turns the kernels still queued into no-ops.
 void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
 {
   Ctx& c = *s.ctx;
@@ -615,10 +532,74 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
   // a sharded source sees only its own shard in the reciprocal tree: a different answer, not a smaller one
   PCLB_REQUIRE(!(comm_active(c) && s.P.use_reciprocal), PCLB200_ERR_INVALID,
                "icp: reciprocal correspondences are not available with a sharded source (multi-GPU communicator)");
-  const Index& T = *s.tgt;
-  SolveOut* h_out = reinterpret_cast<SolveOut*>(c.pinned);
-  int steps = 0;
-  auto base_args = [&]() {
+  // the reference's do-while runs at least once per align(); a caller stepping one iteration at a time resumes a
+  // NOT_CONVERGED session, and a fresh session (iterations == 0) always enters
+  if (s.loop.state == PCLB200_CONV_NOT_CONVERGED && max_steps > 0) {
+    const Index& T = *s.tgt;
+    const int kind = s.P.correspondence_kind;
+    const bool normal_based = kind != PCLB200_CORR_NEAREST;  // setCorrespondenceEstimation(NormalShooting / BackProjection)
+    int keff = 0;
+    if (normal_based) {
+      PCLB_REQUIRE(kind == PCLB200_CORR_NORMAL_SHOOTING || kind == PCLB200_CORR_BACK_PROJECTION, PCLB200_ERR_INVALID,
+                   "icp: unknown correspondence_kind");
+      PCLB_REQUIRE(!s.P.use_reciprocal, PCLB200_ERR_INVALID,
+                   "icp: reciprocal correspondences are only built for the nearest-neighbour estimator");
+      PCLB_REQUIRE(s.cur_normals.p, PCLB200_ERR_INVALID, "icp: the normal-based estimators need source normals");
+      PCLB_REQUIRE(kind != PCLB200_CORR_BACK_PROJECTION || s.tgt_normals.p, PCLB200_ERR_INVALID,
+                   "icp: back projection needs target normals");
+      keff = (int)std::min<size_t>((size_t)std::max(s.P.correspondence_k, 0), T.n_valid);
+      PCLB_REQUIRE(keff > 0, PCLB200_ERR_INVALID, "icp: correspondence_k must be positive");
+    }
+    PCLB_REQUIRE(s.rejectors.empty() || !comm_active(c), PCLB200_ERR_INVALID,
+                 "correspondence rejectors need the whole correspondence set: not available with a sharded source");
+    const bool host_reduce = comm_active(c) && !comm_peer_fused(c);  // a collective launched by NCCL
+    // The normal-based estimators' k-NN rows, rejector chains (their sorts synchronise), the reciprocal tree rebuilt
+    // every iteration, the symmetric objective and an NCCL collective: the loop state is read back after every
+    // iteration and the loop stops once k_solve sets `done`.  Otherwise every iteration this call may run is enqueued
+    // at once and the stream is synchronised once.
+    const bool needs_host_between = normal_based || !s.rejectors.empty() || s.P.use_reciprocal ||
+                                    s.P.estimator == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS || host_reduce;
+    // Temporal coherence (still_nearest) pays once the cloud has almost stopped moving: tracking the lower bounds makes a
+    // walk look at a wider ball, so AUTO switches it on when the last increment displaced no point by more than half the
+    // RMS correspondence distance (k_solve), and the skip test fires from the following iteration on.  Only the plain
+    // nearest-neighbour search keeps the bounds.
+    const int track_mode = (normal_based || s.P.use_reciprocal) ? (int)PCLB200_TRACK_OFF : s.P.track_mode;
+    CritParams crit;
+    crit.max_iterations = s.P.max_iterations;
+    crit.failure_after_max_iter = s.P.failure_after_max_iter;
+    crit.max_iterations_similar = s.P.max_iterations_similar_transforms;
+    crit.scalar_is_double = s.P.scalar_is_double;
+    crit.track_mode = track_mode;
+    crit.rot_eps = s.P.transformation_rotation_epsilon;
+    crit.trans_eps = s.P.transformation_epsilon;
+    crit.rel_mse = s.P.euclidean_fitness_epsilon;
+    crit.abs_mse = s.P.mse_threshold_absolute;
+    {
+      double rmax = 0.0;
+      for (int r = 0; r < 3; ++r) {
+        const double m = std::max(std::fabs((double)T.lo[r]), std::fabs((double)T.hi[r]));
+        rmax += m * m;
+      }
+      crit.rmax = std::sqrt(rmax);
+    }
+    if (track_mode != PCLB200_TRACK_AUTO)  // AUTO carries the last decision over from the previous call
+      s.loop.track_next = track_mode == PCLB200_TRACK_ON ? 1 : 0;
+    LoopCtrl* h_ctrl = static_cast<LoopCtrl*>(c.pinned);
+    int* h_err = reinterpret_cast<int*>(h_ctrl + 1);
+    *h_ctrl = s.loop;
+    PCLB_CUDA(cudaMemcpyAsync(s.ctrl.p, h_ctrl, sizeof(LoopCtrl), cudaMemcpyHostToDevice, st));
+    auto read_back = [&]() {
+      PCLB_CUDA(cudaMemcpyAsync(h_ctrl, s.ctrl.p, sizeof(LoopCtrl), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaMemcpyAsync(h_err, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaStreamSynchronize(st));
+      if (*h_err) {
+        PCLB_CUDA(cudaMemsetAsync(c.d_error, 0, sizeof(int), st));
+        if (*h_err == 2)
+          throw Error(PCLB200_ERR_NCCL, "fused cross-GPU reduce timed out waiting for a peer rank");
+        throw Error(PCLB200_ERR_INTERNAL, "LBVH traversal stack overflow (tree deeper than the per-query stack)");
+      }
+      s.loop = *h_ctrl;
+    };
     IterArgs a;
     memset(&a, 0, sizeof(a));
     a.nodes = T.nodes.p;
@@ -642,92 +623,78 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     a.cur_normals = s.cur_normals.p;
     a.enforce_same_dir = s.P.enforce_same_direction_normals;
     a.cells = tree_view(T).cells;
-    a.peer.nranks = 0;
-    a.seq = 0;
-    return a;
-  };
-  auto raise_device_error = [&](int h_err) {
-    if (!h_err)
-      return;
-    PCLB_CUDA(cudaMemsetAsync(c.d_error, 0, sizeof(int), st));
-    if (h_err == 2)
-      throw Error(PCLB200_ERR_NCCL, "fused cross-GPU reduce timed out waiting for a peer rank");
-    throw Error(PCLB200_ERR_INTERNAL, "LBVH traversal stack overflow (tree deeper than the per-query stack)");
-  };
-  // ---- enqueue-ahead path ------------------------------------------------------------------------------------------
-  // The plain loop (nearest-neighbour correspondences, no rejector chain, no reciprocal tree) needs the host for nothing
-  // between iterations: k_solve leaves T_k in device memory for the next search, composes the final transform, counts
-  // the iteration and evaluates the convergence criteria (LoopCtrl).  So every iteration this call may run is enqueued
-  // at once and the stream is synchronised ONCE; when a criterion fires early the kernels still queued find `done` set
-  // and return.  With AUTO tracking both flavours of the search kernel are queued and the device picks one.
-  const bool needs_host_between = s.P.correspondence_kind != PCLB200_CORR_NEAREST || !s.rejectors.empty() ||
-                                  s.P.use_reciprocal || s.P.estimator == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS ||
-                                  (comm_active(c) && !comm_peer_fused(c));
-  if (!needs_host_between && s.state == PCLB200_CONV_NOT_CONVERGED && max_steps > 0) {
-    const int left = std::max(1, s.P.max_iterations - s.iterations);  // the do-while always runs once
-    const int n_enq = std::min(max_steps, left);
-    LoopCtrl* h_ctrl = reinterpret_cast<LoopCtrl*>(static_cast<unsigned char*>(c.pinned) + 1024);
-    int* h_err = reinterpret_cast<int*>(static_cast<unsigned char*>(c.pinned) + 1024 + sizeof(LoopCtrl));
-    memset(h_ctrl, 0, sizeof(LoopCtrl));
-    h_ctrl->iterations = s.iterations;
-    h_ctrl->state = s.state;
-    h_ctrl->iterations_similar = s.iterations_similar;
-    h_ctrl->track_next = s.P.track_mode == PCLB200_TRACK_ON ? 1 : (s.P.track_mode == PCLB200_TRACK_OFF ? 0 : (s.track_next ? 1 : 0));
-    h_ctrl->lb_valid = s.lb_valid ? 1 : 0;
-    h_ctrl->prev_mse = s.prev_mse;
-    h_ctrl->total_corr = s.total_corr;
-    for (int i = 0; i < 16; ++i) {
-      h_ctrl->final_T[i] = s.final_T[i];
-      h_ctrl->last_T[i] = s.last_T[i];
-    }
-    PCLB_CUDA(cudaMemcpyAsync(s.ctrl.p, h_ctrl, sizeof(LoopCtrl), cudaMemcpyHostToDevice, st));
-    CritParams crit;
-    crit.max_iterations = s.P.max_iterations;
-    crit.failure_after_max_iter = s.P.failure_after_max_iter;
-    crit.max_iterations_similar = s.P.max_iterations_similar_transforms;
-    crit.scalar_is_double = s.P.scalar_is_double;
-    crit.track_mode = s.P.track_mode;
-    crit.rot_eps = s.P.transformation_rotation_epsilon;
-    crit.trans_eps = s.P.transformation_epsilon;
-    crit.rel_mse = s.P.euclidean_fitness_epsilon;
-    crit.abs_mse = s.P.mse_threshold_absolute;
-    {
-      double rmax = 0.0;
-      for (int r = 0; r < 3; ++r) {
-        const double m = std::max(std::fabs((double)T.lo[r]), std::fabs((double)T.hi[r]));
-        rmax += m * m;
-      }
-      crit.rmax = std::sqrt(rmax);
-    }
+    a.ctrl = s.ctrl.p;
+    a.track_sel = track_mode == PCLB200_TRACK_AUTO;  // the search runs only in the flavour of the device's decision
+    const unsigned grid = persistent_grid(c, s.n_q, 256, 8);
     const unsigned wgrid = persistent_grid(c, s.n_q, 256, 18);
     const unsigned agrid = std::min(persistent_grid(c, s.n_q, 256, kAccumBlocksPerSM), s.red.max_blocks);
+    const int n_enq = std::min(max_steps, std::max(1, s.P.max_iterations - s.loop.iterations));
     for (int k = 0; k < n_enq; ++k) {
-      IterArgs a = base_args();
-      a.ctrl = s.ctrl.p;
       comm_peer_view(c, &a.peer, &a.seq);
+      std::unique_ptr<Index> src_index;
       {
         ProfScope ps(c, "icp_search");
-        if (s.P.track_mode == PCLB200_TRACK_AUTO) {
-          a.track_sel = 1;
-          k_search<false, false><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
-          k_search<false, true><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
+        if (normal_based || s.P.use_reciprocal) {
+          k_apply_pending<<<grid, 256, 0, st>>>(s.cur.p, s.n_q, s.pending.p, s.cur_normals.p);
+          k_clear_apply<<<1, 1, 0, st>>>(s.pending.p);
           c.launches += 2;
         }
-        else {
-          if (s.P.track_mode == PCLB200_TRACK_ON)
-            k_search<false, true><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
-          else
-            k_search<false, false><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
+        if (normal_based) {
+          // k-NN candidates, then the normal-based choice
+          DevBuf<int32_t> nn_idx;
+          DevBuf<float> nn_d2;
+          nn_idx.alloc(s.n_q * (size_t)keff, st);
+          nn_d2.alloc(s.n_q * (size_t)keff, st);
+          launch_knn(c, T, s.cur.p, s.n_q, keff, std::numeric_limits<float>::infinity(), nn_idx.p, nn_d2.p);
+          ensure_pos_of_orig(c, const_cast<Index&>(T));
+          k_select_match<<<grid_for(s.n_q, 128), 128, 0, st>>>(s.cur.p, s.cur_normals.p, s.n_q, kind, keff, nn_idx.p,
+                                                              nn_d2.p, T.pts.p, T.pos_of_orig.p, s.tgt_normals.p,
+                                                              s.P.max_correspondence_distance, s.match.p);
           ++c.launches;
         }
+        else if (s.P.use_reciprocal) {
+          // tree_reciprocal_ is rebuilt over the transformed source every iteration
+          // (correspondence_estimation.hpp:117-135 via setInputSource at icp.hpp:175)
+          src_index.reset(build_index_from_device(c, s.cur.p, s.n_q, s.cur_label.p));
+          a.s_nodes = src_index->nodes.p;
+          a.s_pts = src_index->pts.p;
+          a.s_root = src_index->root;
+          k_search<true, false><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
+          ++c.launches;
+        }
+        else {
+          bool plain = track_mode != PCLB200_TRACK_ON, track = track_mode != PCLB200_TRACK_OFF;
+          if (track_mode == PCLB200_TRACK_AUTO && needs_host_between) {  // the host has read this iteration's decision
+            track = s.loop.track_next != 0;
+            plain = !track;
+          }
+          if (plain) {
+            k_search<false, false><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
+            ++c.launches;
+          }
+          if (track) {
+            k_search<false, true><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
+            ++c.launches;
+          }
+        }
+      }
+      if (!s.rejectors.empty()) {
+        ProfScope ps(c, "icp_reject");
+        run_rejectors(s);
       }
       {
         ProfScope ps(c, "icp_accum");
         if (s.P.estimator == PCLB200_EST_SVD)
           k_accum_dmma<PCLB200_EST_SVD><<<agrid, 256, 0, st>>>(a, s.match.p);
-        else
+        else if (s.P.estimator == PCLB200_EST_POINT_TO_PLANE_LLS)
           k_accum_dmma<PCLB200_EST_POINT_TO_PLANE_LLS><<<agrid, 256, 0, st>>>(a, s.match.p);
+        else
+          k_accum<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS><<<grid, 256, 0, st>>>(a, s.match.p);
         ++c.launches;
+      }
+      if (host_reduce) {
+        ProfScope ps(c, "allreduce");
+        comm_allreduce_sum(c, s.red.accum.p, kAccum);
       }
       {
         ProfScope ps(c, "solve");
@@ -736,175 +703,15 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
                                   crit);
         ++c.launches;
       }
-    }
-    PCLB_CUDA(cudaGetLastError());
-    PCLB_CUDA(cudaMemcpyAsync(h_ctrl, s.ctrl.p, sizeof(LoopCtrl), cudaMemcpyDeviceToHost, st));
-    PCLB_CUDA(cudaMemcpyAsync(h_err, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
-    PCLB_CUDA(cudaStreamSynchronize(st));
-    raise_device_error(*h_err);
-    steps = h_ctrl->n_run;
-    s.iterations = h_ctrl->iterations;
-    s.state = h_ctrl->state;
-    s.converged = h_ctrl->converged != 0;
-    s.iterations_similar = h_ctrl->iterations_similar;
-    s.prev_mse = h_ctrl->prev_mse;
-    s.track_next = h_ctrl->track_next != 0;
-    s.lb_valid = h_ctrl->lb_valid != 0;
-    if (steps > 0) {
-      s.n_corr = (int64_t)h_ctrl->n_corr;
-      s.mse = h_ctrl->mse;
-    }
-    s.total_corr = h_ctrl->total_corr;
-    for (int i = 0; i < 16; ++i) {
-      s.final_T[i] = h_ctrl->final_T[i];
-      s.last_T[i] = h_ctrl->last_T[i];
-    }
-    s.searches += steps;
-  }
-  // ---- stage-by-stage path: something between search and solve needs the host (rejector chain with its sorts, the
-  // reciprocal tree rebuilt every iteration, the normal-based estimators' k-NN rows, a collective launched by NCCL) ----
-  // the reference's do-while runs at least once per align(); a caller stepping one iteration at a time
-  // resumes a NOT_CONVERGED session, and a fresh session (iterations == 0) always enters.
-  while (needs_host_between && steps < max_steps && (s.state == PCLB200_CONV_NOT_CONVERGED)) {
-    IterArgs a = base_args();
-    const bool fused_reduce = comm_peer_view(c, &a.peer, &a.seq);
-    const unsigned grid = persistent_grid(c, s.n_q, 256, 8);
-    std::unique_ptr<Index> src_index;
-    if (s.P.use_reciprocal) {
-      // tree_reciprocal_ is rebuilt over the transformed source every iteration
-      // (correspondence_estimation.hpp:117-135 via setInputSource at icp.hpp:175)
-      k_apply_pending<<<grid, 256, 0, st>>>(s.cur.p, s.n_q, s.pending.p, s.cur_normals.p);
-      k_clear_apply<<<1, 1, 0, st>>>(s.pending.p);
-      c.launches += 2;
-      src_index.reset(build_index_from_device(c, s.cur.p, s.n_q, s.cur_label.p));
-      a.s_nodes = src_index->nodes.p;
-      a.s_pts = src_index->pts.p;
-      a.s_root = src_index->root;
-    }
-    if (s.P.correspondence_kind != PCLB200_CORR_NEAREST) {
-      // setCorrespondenceEstimation(NormalShooting / BackProjection): k-NN candidates, then the normal-based choice
-      ProfScope ps(c, "icp_search");
-      const int kind = s.P.correspondence_kind;
-      PCLB_REQUIRE(kind == PCLB200_CORR_NORMAL_SHOOTING || kind == PCLB200_CORR_BACK_PROJECTION, PCLB200_ERR_INVALID,
-                   "icp: unknown correspondence_kind");
-      PCLB_REQUIRE(!s.P.use_reciprocal, PCLB200_ERR_INVALID,
-                   "icp: reciprocal correspondences are only built for the nearest-neighbour estimator");
-      PCLB_REQUIRE(s.cur_normals.p, PCLB200_ERR_INVALID, "icp: the normal-based estimators need source normals");
-      PCLB_REQUIRE(kind != PCLB200_CORR_BACK_PROJECTION || s.tgt_normals.p, PCLB200_ERR_INVALID,
-                   "icp: back projection needs target normals");
-      const int keff = (int)std::min<size_t>((size_t)std::max(s.P.correspondence_k, 0), T.n_valid);
-      PCLB_REQUIRE(keff > 0, PCLB200_ERR_INVALID, "icp: correspondence_k must be positive");
-      k_apply_pending<<<grid, 256, 0, st>>>(s.cur.p, s.n_q, s.pending.p, s.cur_normals.p);
-      k_clear_apply<<<1, 1, 0, st>>>(s.pending.p);
-      c.launches += 2;
-      DevBuf<int32_t> nn_idx;
-      DevBuf<float> nn_d2;
-      nn_idx.alloc(s.n_q * (size_t)keff, st);
-      nn_d2.alloc(s.n_q * (size_t)keff, st);
-      launch_knn(c, T, s.cur.p, s.n_q, keff, std::numeric_limits<float>::infinity(), nn_idx.p, nn_d2.p);
-      ensure_pos_of_orig(c, const_cast<Index&>(T));
-      k_select_match<<<grid_for(s.n_q, 128), 128, 0, st>>>(s.cur.p, s.cur_normals.p, s.n_q, kind, keff, nn_idx.p, nn_d2.p,
-                                                          T.pts.p, T.pos_of_orig.p, s.tgt_normals.p,
-                                                          s.P.max_correspondence_distance, s.match.p);
-      ++c.launches;
       PCLB_CUDA(cudaGetLastError());
-    }
-    else {
-      ProfScope ps(c, "icp_search");
-      ++s.searches;
-      // Temporal coherence (still_nearest) pays once the cloud has almost stopped moving: tracking the lower bounds makes
-      // a walk look at a wider ball, so it is switched on when the last increment displaced no point by more than half
-      // the RMS correspondence distance (or always / never: pclb200_icp_params::track_mode), and the skip test then
-      // fires from the following iteration on.
-      bool track = s.P.track_mode == PCLB200_TRACK_ON || (s.P.track_mode == PCLB200_TRACK_AUTO && s.track_next);
-      if (s.P.use_reciprocal)
-        track = false;
-      if (track && !s.lb_valid)  // bounds left by an earlier TRACK phase say nothing about the current matches
-        PCLB_CUDA(cudaMemsetAsync(s.lb.p, 0, s.n_q * sizeof(float), st));
-      s.lb_valid = track;
-      const unsigned wgrid = persistent_grid(c, s.n_q, 256, 18);
-      if (s.P.use_reciprocal)
-        k_search<true, false><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
-      else if (track)
-        k_search<false, true><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
-      else
-        k_search<false, false><<<wgrid, 256, 0, st>>>(a, s.match.p, s.lb.p);
-      ++c.launches;
-    }
-    if (!s.rejectors.empty()) {
-      PCLB_REQUIRE(!comm_active(c), PCLB200_ERR_INVALID,
-                   "correspondence rejectors need the whole correspondence set: not available with a sharded source");
-      ProfScope ps(c, "icp_reject");
-      run_rejectors(s);
-    }
-    {
-      ProfScope ps(c, "icp_accum");
-      const unsigned agrid = std::min(persistent_grid(c, s.n_q, 256, kAccumBlocksPerSM), s.red.max_blocks);
-      if (s.P.estimator == PCLB200_EST_SVD)
-        k_accum_dmma<PCLB200_EST_SVD><<<agrid, 256, 0, st>>>(a, s.match.p);
-      else if (s.P.estimator == PCLB200_EST_POINT_TO_PLANE_LLS)
-        k_accum_dmma<PCLB200_EST_POINT_TO_PLANE_LLS><<<agrid, 256, 0, st>>>(a, s.match.p);
-      else
-        k_accum<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS><<<grid, 256, 0, st>>>(a, s.match.p);
-      ++c.launches;
-    }
-    PCLB_CUDA(cudaGetLastError());
-    if (!fused_reduce) {
-      ProfScope ps(c, "allreduce");
-      comm_allreduce_sum(c, s.red.accum.p, kAccum);
-    }
-    {
-      ProfScope ps(c, "solve");
-      k_solve<<<1, 32, 0, st>>>(s.red.accum.p, s.P.estimator, s.P.scalar_is_double, transform_mode(s.P), (double)a.ox,
-                                (double)a.oy, (double)a.oz, 3, s.pending.p, s.solve_out.p, s.P.svd_no_umeyama, nullptr,
-                                CritParams{});
-    }
-    ++c.launches;
-    PCLB_CUDA(cudaMemcpyAsync(h_out, s.solve_out.p, sizeof(SolveOut), cudaMemcpyDeviceToHost, st));
-    int h_err = 0;
-    PCLB_CUDA(cudaMemcpyAsync(&h_err, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
-    PCLB_CUDA(cudaStreamSynchronize(st));
-    raise_device_error(h_err);
-    ++steps;
-    s.n_corr = (int64_t)h_out->n;
-    s.total_corr += s.n_corr;
-    s.mse = h_out->n > 0 ? h_out->sum_d / h_out->n : 0.0;
-    if (!h_out->ok) {  // icp.hpp:204-213
-      s.state = PCLB200_CONV_NO_CORRESPONDENCES;
-      s.converged = false;
-      break;
-    }
-    for (int i = 0; i < 16; ++i)
-      s.last_T[i] = h_out->T[i];
-    if (s.P.scalar_is_double)
-      mat4_mul<double>(s.last_T, s.final_T, s.final_T);
-    else {
-      float A[16], B[16], C[16];
-      for (int i = 0; i < 16; ++i) {
-        A[i] = (float)s.last_T[i];
-        B[i] = (float)s.final_T[i];
+      if (needs_host_between) {
+        read_back();
+        if (s.loop.done)
+          break;
       }
-      mat4_mul<float>(A, B, C);
-      for (int i = 0; i < 16; ++i)
-        s.final_T[i] = C[i];
     }
-    ++s.iterations;
-    s.converged = s.P.scalar_is_double ? has_converged<double>(s, s.last_T) : has_converged<float>(s, s.last_T);
-    {
-      // upper bound of the displacement T_k causes anywhere near the target: |R - I|_F * r_max + |t|
-      double rf = 0.0, tn = 0.0, rmax = 0.0;
-      for (int r = 0; r < 3; ++r) {
-        for (int cc = 0; cc < 3; ++cc) {
-          const double d = s.last_T[4 * r + cc] - (r == cc ? 1.0 : 0.0);
-          rf += d * d;
-        }
-        tn += s.last_T[4 * r + 3] * s.last_T[4 * r + 3];
-        const double m = std::max(std::fabs((double)T.lo[r]), std::fabs((double)T.hi[r]));
-        rmax += m * m;
-      }
-      const double disp = std::sqrt(rf) * std::sqrt(rmax) + std::sqrt(tn);
-      s.track_next = disp < 0.5 * std::sqrt(std::max(s.mse, 0.0));
-    }
+    if (!needs_host_between)
+      read_back();
   }
   if (stats) {
     unsigned long long h = 0;
@@ -943,7 +750,7 @@ size_t icp_get_correspondences(Icp& s, pclb200_corr* out)
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
   PCLB_REQUIRE(s.tgt && s.cur.p && s.match.p, PCLB200_ERR_INVALID, "icp: no iteration has run");
-  if (!s.n_q || s.iterations == 0)
+  if (!s.n_q || s.loop.iterations == 0)
     return 0;
   DevBuf<pclb200_corr> by_slot, compact;
   DevBuf<size_t> d_count;
@@ -986,8 +793,8 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
   pend.alloc(1, st);
   Pending h;
   for (int i = 0; i < 12; ++i) {
-    h.f[i] = (float)s.final_T[i];
-    h.d[i] = s.final_T[i];
+    h.f[i] = (float)s.loop.final_T[i];
+    h.d[i] = s.loop.final_T[i];
   }
   h.apply = 1;
   h.mode = transform_mode(s.P);

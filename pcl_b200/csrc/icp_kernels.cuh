@@ -129,7 +129,7 @@ struct IterArgs {
   float4* cur_normals;             // source normals, same order as cur (symmetric objective), rotated with T_k
   int enforce_same_dir;
   CellTable cells;                 // cell table of the target index (walks start at the candidate ball)
-  LoopCtrl* ctrl;                  // device-side loop state (nullptr: the host decides everything, one iteration per sync)
+  LoopCtrl* ctrl;                  // device-side loop state: a finished loop (`done`) turns the kernel into a no-op
   int track_sel;                   // 1: the search kernel runs only if ctrl->track_next matches its TRACK flavour
   // fused cross-GPU reduce (optional): peer-mapped exchange buffers + this iteration's sequence number
   PeerView peer;

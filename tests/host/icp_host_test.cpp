@@ -1,7 +1,7 @@
 // icp_host_test.cpp — whole ICP iterations of the DEVICE code (pcl_b200/csrc/icp_kernels.cuh: k_search, k_accum_dmma on the
 // emulated fp64 tensor-core fragments, k_solve with the convergence criteria in its tail) compiled for the HOST, run on a
-// lock-step emulation of a 256-thread block (tests/host/warp_emu.h) and driven exactly like icp.cu's enqueue-ahead path
-// drives them — against the CPU oracle's IterativeClosestPoint (oracle/libpcl_oracle.so, linked: test infrastructure).
+// lock-step emulation of a 256-thread block (tests/host/warp_emu.h) and driven exactly like icp.cu's icp_iterate drives
+// them — against the CPU oracle's IterativeClosestPoint (oracle/libpcl_oracle.so, linked: test infrastructure).
 // CPU only.  Checked: every iteration-0 correspondence against brute force, the accumulated normal equations against
 // plain fp64 sums, and iterations / convergence state / final transform of the whole align against the oracle for
 // Scalar = float and double, point-to-point (SVD, both formulas) and point-to-plane (LLS), gates, temporal tracking on.
@@ -161,7 +161,7 @@ static void run_align(const char* name, const Scene& S, int estimator, bool scal
   blockDim.x = 256;
   long skipped_total = 0;
   for (int it = 0; it < max_iterations; ++it) {
-    HostIndex SI;   // reciprocal: tree over the re-transformed source of THIS iteration (icp.cu: stage-by-stage path)
+    HostIndex SI;   // reciprocal: tree over the re-transformed source of THIS iteration (icp.cu: icp_iterate)
     if (X.reciprocal) {
       if (pending.apply) {
         for (std::size_t i = 0; i < ns; ++i) {

@@ -595,6 +595,34 @@ def test_icp_with_rejector_chain_vs_oracle(gpu, orc):
     assert s.iterate(1)["n_correspondences"] == S.shape[0]   # no rejectors, no gate: every source point pairs up
 
 
+@pytest.mark.parametrize("dbl", [False, True], ids=["float", "double"])
+@pytest.mark.parametrize("track", ["on", "off", "auto"])
+def test_icp_per_iteration_sync_matches_single_sync(gpu, track, dbl):
+    """icp_iterate synchronises once per call, or after every iteration when a stage between search and solve needs the
+    host (here a rejector chain).  A distance rejector far above the gate keeps every pair, so its only effect is the
+    per-iteration synchronisation: stepped one iteration at a time and then run to the end, both modes go through the
+    same states, counts and transforms, bit for bit, in every tracking mode."""
+    P, ctx = gpu
+    src, tgt = _synthetic_pair(np.random.default_rng(44), 30000)
+    src, tgt = P.xyz1(src), P.xyz1(tgt)
+    tidx = P.Index(ctx, tgt)
+    gate = 0.05
+    mode = {"on": P.TRACK_ON, "off": P.TRACK_OFF, "auto": P.TRACK_AUTO}[track]
+    runs = []
+    for chain in ([], [(P.REJ_DISTANCE, 100 * gate, 0)]):
+        s = P.Icp(ctx, max_iterations=40, transformation_epsilon=1e-10, max_correspondence_distance=gate,
+                  scalar_is_double=int(dbl), track_mode=mode)
+        s.set_rejectors(chain)
+        s.set_target(tidx)
+        s.set_source(src)
+        runs.append([s.iterate(1) for _ in range(3)] + [s.iterate()])
+    keys = ("iterations", "state", "converged", "n_correspondences", "total_correspondences", "total_skipped_walks")
+    for k, (a, b) in enumerate(zip(*runs)):
+        assert [a[x] for x in keys] == [b[x] for x in keys], (k, a, b)
+        assert np.array_equal(a["final"], b["final"]) and np.array_equal(a["last"], b["last"]), k
+    assert runs[0][-1]["state"] != 0 and runs[0][-1]["iterations"] > 3
+
+
 def test_symmetric_point_to_plane(gpu, orc):
     """TransformationEstimationSymmetricPointToPlaneLLS (SURVEY.md §8f #2): the reference's paraboloid test
     (test_registration_api.cpp:663-713), oracle parity, and ICP with setUseSymmetricObjective(true)."""

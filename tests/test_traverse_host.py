@@ -72,7 +72,7 @@ def test_warp_knn_kernel_on_an_emulated_warp(tmp_path, device_built):
 @pytest.mark.parametrize("device_built", [False, True], ids=["reference-index", "device-built-index"])
 def test_whole_icp_iterations_on_an_emulated_block(tmp_path, device_built):
     """icp_kernels.cuh — k_search, k_accum_dmma (the m8n8k4 fp64 MMA emulated fragment by fragment), k_accum, k_solve with the
-    convergence criteria in its tail — on an emulated 256-thread block, driven like icp.cu's enqueue-ahead path: every
+    convergence criteria in its tail — on an emulated 256-thread block, driven like icp.cu's icp_iterate: every
     iteration's correspondences equal brute force, the accumulated normal equations equal plain fp64 sums, and iterations /
     state / counts / final transform of twelve aligns (SVD, point-to-plane, the symmetric objective, ICPWithNormals,
     reciprocal correspondences; float and double; gates; tracking off / on / automatic; rejector chains inside the loop —
