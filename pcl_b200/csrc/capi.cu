@@ -74,15 +74,21 @@ static int guarded(F&& f)
   }
 }
 
-static void raise_if_device_error(Ctx& c)
+void raise_device_error(Ctx& c, int code)
+{
+  PCLB_CUDA(cudaMemsetAsync(c.d_error, 0, sizeof(int), c.stream));
+  if (code == kErrPeerTimeout)
+    throw Error(PCLB200_ERR_NCCL, "fused cross-GPU reduce timed out waiting for a peer rank");
+  throw Error(PCLB200_ERR_INTERNAL, "LBVH traversal stack overflow (tree deeper than the per-query stack)");
+}
+
+void check_device_error(Ctx& c)
 {
   int h = 0;
   PCLB_CUDA(cudaMemcpyAsync(&h, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
   PCLB_CUDA(cudaStreamSynchronize(c.stream));
-  if (h) {
-    PCLB_CUDA(cudaMemsetAsync(c.d_error, 0, sizeof(int), c.stream));
-    throw Error(PCLB200_ERR_INTERNAL, "LBVH traversal stack overflow (tree deeper than the per-query stack)");
-  }
+  if (h)
+    raise_device_error(c, h);
 }
 
 static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
@@ -267,7 +273,7 @@ static void radius_impl(Ctx& c, const Index& idx, const void* queries, size_t nq
         deliver(o, di.p, dd.p, kept);
         PCLB_CUDA(cudaStreamSynchronize(st));
       }
-      raise_if_device_error(c);
+      check_device_error(c);
       return;
     }
     {
@@ -318,7 +324,7 @@ static void radius_impl(Ctx& c, const Index& idx, const void* queries, size_t nq
       }
       PCLB_CUDA(cudaStreamSynchronize(st));
     }
-    raise_if_device_error(c);
+    check_device_error(c);
 }
 
 
@@ -571,7 +577,7 @@ int pclb200_knn(pclb200_ctx* ctx, const pclb200_index* h, const void* queries, s
       PCLB_CUDA(cudaMemcpyAsync(out_idx, pi, nq * (size_t)k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       PCLB_CUDA(cudaMemcpyAsync(out_d2, pd, nq * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, st));
     }
-    raise_if_device_error(c);
+    check_device_error(c);
   });
 }
 
@@ -613,7 +619,7 @@ int pclb200_knn_stats(pclb200_ctx* ctx, const pclb200_index* h, const void* pts,
       PCLB_CUDA(cudaMemcpyAsync(out_mean, pm, nq * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (out_kth && !k_dev)
       PCLB_CUDA(cudaMemcpyAsync(out_kth, pk, nq * sizeof(float), cudaMemcpyDeviceToHost, st));
-    raise_if_device_error(c);
+    check_device_error(c);
   });
 }
 
@@ -706,7 +712,7 @@ int pclb200_correspondences_normals(pclb200_ctx* ctx, const pclb200_index* idx_t
     PCLB_CUDA(cudaSetDevice(ctx->c.device));
     *n_out = correspondences_by_normals(ctx->c, *idx_tgt->idx, kind, src, n, stride, src_normals, stride_sn, tgt_normals,
                                         stride_tn, src_indices, n_idx, k, max_dist, out);
-    raise_if_device_error(ctx->c);
+    check_device_error(ctx->c);
   });
 }
 
@@ -1029,7 +1035,7 @@ int pclb200_normals_knn(pclb200_ctx* ctx, const pclb200_index* h, const void* pt
     PCLB_CUDA(cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     if (!dev_out)
       PCLB_CUDA(cudaMemcpyAsync(out, po, nq * sizeof(float4), cudaMemcpyDeviceToHost, st));
-    raise_if_device_error(c);
+    check_device_error(c);
     if (is_dense_out)
       *is_dense_out = flag ? 0 : 1;
   });
@@ -1075,7 +1081,7 @@ int pclb200_normals_radius(pclb200_ctx* ctx, const pclb200_index* h, const void*
     PCLB_CUDA(cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     if (!dev_out)
       PCLB_CUDA(cudaMemcpyAsync(out, po, nq * sizeof(float4), cudaMemcpyDeviceToHost, st));
-    raise_if_device_error(c);
+    check_device_error(c);
     if (is_dense_out)
       *is_dense_out = flag ? 0 : 1;
   });
@@ -1104,7 +1110,7 @@ int pclb200_cluster_labels(pclb200_ctx* ctx, const pclb200_index* h, double tole
     cluster_labels(c, idx, tolerance, pl);
     if (!dev_out)
       PCLB_CUDA(cudaMemcpyAsync(out_labels, pl, n_labels * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    raise_if_device_error(c);
+    check_device_error(c);
   });
 }
 

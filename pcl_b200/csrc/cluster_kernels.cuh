@@ -75,7 +75,7 @@ k_cc_union(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, in
     return;  // padding slot
   UnionVisitor v{q.x, q.y, q.z, r2, r2_below, (int)j, parent};
   if (!traverse(nodes, pts, root, q.x, q.y, q.z, v))
-    atomicExch(d_error, 1);
+    atomicExch(d_error, kErrStackOverflow);
 }
 
 // smallest original index of every component, kept at the component's root

@@ -1,10 +1,12 @@
-// comm.cu — cross-GPU reduction of the per-iteration accumulators.
+// comm.cu — cross-GPU exchanges of a sharded source.
 //
 // The reference has no multi-GPU path.  Here the source cloud is sharded across ranks (one process per
-// GPU, target index replicated); the only exchange per ICP iteration is a sum of kAccum (= 40) doubles,
-// issued on the same stream as the iteration kernel so the solve kernel that follows sees the global sums.
-// NCCL is bound at run time (dlopen of libnccl.so.2 — the copy torch already loaded, if any) so the library
-// has no link-time dependency and single-GPU users never touch it.
+// GPU, target index replicated); every ICP iteration sums kAccum (= 40) doubles, issued on the same stream as the
+// iteration kernel so the solve kernel that follows sees the global sums, and a rejector chain adds u64 sums, minima
+// and barriers (reject.cu).  Both run on every rank's IPC-mapped exchange block with one device protocol
+// (peer_exchange.cuh): the accumulators inside the accumulate kernels, the u64 collectives in k_peer_u64.  Without the
+// mappings they fall back to ncclAllReduce.  NCCL is bound at run time (dlopen of libnccl.so.2 — the copy torch
+// already loaded, if any) so the library has no link-time dependency and single-GPU users never touch it.
 #include <dlfcn.h>
 
 #include <algorithm>
@@ -12,6 +14,7 @@
 #include <vector>
 
 #include "internal.cuh"
+#include "peer_exchange.cuh"
 
 namespace pclb200 {
 
@@ -98,8 +101,7 @@ struct Comm {
   void* peer_block[kMaxRanks] = {};
   PeerView view;
   bool peer_ok = false;
-  unsigned long long seq = 0;
-  PeerU64View uview;                  // the u64 region of the same blocks (sharded rejectors)
+  unsigned long long seq = 0;         // the last sequence number drawn (next_seq)
   unsigned long long id = 0;          // distinct per communicator made in this process
   std::vector<std::weak_ptr<OneToOneEntry>> o2o;  // the sessions' one-to-one tables made for this communicator
   Comm();
@@ -108,22 +110,44 @@ struct Comm {
 static unsigned long long g_comm_ids = 0;
 Comm::Comm() : id(++g_comm_ids) {}
 
-void comm_destroy(Ctx& c);
+// The sequence number of the next peer exchange.  Every rank must draw them in the same order (peer_exchange.cuh): an
+// iteration's rejector chain first, its accumulator exchange last.
+static unsigned long long next_seq(Comm& cm) { return ++cm.seq; }
 
-static size_t peer_u64_offset() { return kMaxRanks * sizeof(unsigned long long) + 2ull * kMaxRanks * kAccum * sizeof(double); }
-static size_t peer_block_bytes() { return peer_u64_offset() + 2ull * kMaxRanks * kU64Words * sizeof(unsigned long long); }
-
-static void set_u64_view(Comm& cm)
+// Opens the IPC handles of the other ranks' allocations: ptr[p] = rank p's (ptr[rank] = mine).  Returns the first rank
+// whose handle does not open (its CUDA error cleared, *err = the error, ptr[p] = nullptr), or -1 once all are open.
+static int open_peers(const cudaIpcMemHandle_t* handles, int rank, int nranks, void* mine, void** ptr,
+                      cudaError_t* err = nullptr)
 {
-  cm.uview.rank = cm.rank;
-  cm.uview.nranks = cm.nranks;
-  for (int p = 0; p < cm.nranks; ++p) {
-    unsigned char* b = static_cast<unsigned char*>(cm.peer_block[p]);
-    cm.uview.flags[p] = reinterpret_cast<unsigned long long*>(b);
-    cm.uview.words[p] = reinterpret_cast<unsigned long long*>(b + peer_u64_offset());
+  for (int p = 0; p < nranks; ++p) {
+    if (p == rank) {
+      ptr[p] = mine;
+      continue;
+    }
+    const cudaError_t e = cudaIpcOpenMemHandle(&ptr[p], handles[p], cudaIpcMemLazyEnablePeerAccess);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      ptr[p] = nullptr;
+      if (err)
+        *err = e;
+      return p;
+    }
   }
+  return -1;
 }
 
+// every rank's block is mapped: switch to the peer exchange
+static void use_peer_blocks(Comm& cm)
+{
+  cm.view.rank = cm.rank;
+  cm.view.nranks = cm.nranks;
+  for (int p = 0; p < cm.nranks; ++p) {
+    unsigned char* b = static_cast<unsigned char*>(cm.peer_block[p]);
+    cm.view.flags[p] = reinterpret_cast<unsigned long long*>(b);
+    cm.view.slots[p] = reinterpret_cast<double*>(b + kPeerSlotsOffset);
+  }
+  cm.peer_ok = true;
+}
 
 // Maps every rank's exchange block into this process (CUDA IPC over NVLink / NVSwitch).  Any failure leaves
 // peer_ok = false and the per-iteration reduce falls back to ncclAllReduce.
@@ -132,11 +156,11 @@ static void setup_peer_reduce(Ctx& c, Comm& cm)
   if (cm.nranks > kMaxRanks || !nccl().AllGather)
     return;
   cudaStream_t st = c.stream;
-  if (cudaMalloc(reinterpret_cast<void**>(&cm.local_block), peer_block_bytes()) != cudaSuccess) {
+  if (cudaMalloc(reinterpret_cast<void**>(&cm.local_block), kPeerBlockBytes) != cudaSuccess) {
     cudaGetLastError();
     return;
   }
-  cudaMemsetAsync(cm.local_block, 0, peer_block_bytes(), st);
+  cudaMemsetAsync(cm.local_block, 0, kPeerBlockBytes, st);
   cudaIpcMemHandle_t mine;
   bool ok = cudaIpcGetMemHandle(&mine, cm.local_block) == cudaSuccess;
   // exchange handles (+ an "ok" byte) through the communicator we already have
@@ -155,21 +179,12 @@ static void setup_peer_reduce(Ctx& c, Comm& cm)
   PCLB_CUDA(cudaMemcpyAsync(all.data(), d_recv.p, sizeof(Rec) * cm.nranks, cudaMemcpyDeviceToHost, st));
   PCLB_CUDA(cudaStreamSynchronize(st));
   bool all_ok = true;
-  for (int p = 0; p < cm.nranks; ++p)
+  cudaIpcMemHandle_t handles[kMaxRanks];
+  for (int p = 0; p < cm.nranks; ++p) {
     all_ok = all_ok && all[p].ok;
-  if (all_ok) {
-    for (int p = 0; p < cm.nranks && all_ok; ++p) {
-      if (p == cm.rank) {
-        cm.peer_block[p] = cm.local_block;
-        continue;
-      }
-      if (cudaIpcOpenMemHandle(&cm.peer_block[p], all[p].h, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
-        cudaGetLastError();
-        cm.peer_block[p] = nullptr;
-        all_ok = false;
-      }
-    }
+    handles[p] = all[p].h;
   }
+  all_ok = all_ok && open_peers(handles, cm.rank, cm.nranks, cm.local_block, cm.peer_block) < 0;
   // every rank must take the same decision: agree through one more tiny all-reduce
   DevBuf<double> d_flag;
   d_flag.alloc(1, st);
@@ -178,17 +193,8 @@ static void setup_peer_reduce(Ctx& c, Comm& cm)
   PCLB_NCCL(nccl().AllReduce(d_flag.p, d_flag.p, 1, ncclFloat64, ncclSum, cm.comm, st));
   PCLB_CUDA(cudaMemcpyAsync(&hv, d_flag.p, sizeof(double), cudaMemcpyDeviceToHost, st));
   PCLB_CUDA(cudaStreamSynchronize(st));
-  if (hv != 0.0)
-    return;
-  cm.view.rank = cm.rank;
-  cm.view.nranks = cm.nranks;
-  for (int p = 0; p < cm.nranks; ++p) {
-    unsigned char* b = static_cast<unsigned char*>(cm.peer_block[p]);
-    cm.view.flags[p] = reinterpret_cast<unsigned long long*>(b);
-    cm.view.slots[p] = reinterpret_cast<double*>(b + kMaxRanks * sizeof(unsigned long long));
-  }
-  set_u64_view(cm);
-  cm.peer_ok = true;
+  if (hv == 0.0)
+    use_peer_blocks(cm);
 }
 
 static void teardown_peer_reduce(Comm& cm)
@@ -213,9 +219,8 @@ void comm_unique_id(void* out128)
   memcpy(out128, &id, sizeof(id));
 }
 
-void comm_init(Ctx& c, int rank, int nranks, const void* unique_id)
+void comm_destroy(Ctx& c)
 {
-  PCLB_REQUIRE(nranks >= 1 && rank >= 0 && rank < nranks, PCLB200_ERR_INVALID, "bad rank / nranks");
   if (c.comm) {
     teardown_peer_reduce(*c.comm);
     if (c.comm->comm)
@@ -223,6 +228,12 @@ void comm_init(Ctx& c, int rank, int nranks, const void* unique_id)
     delete c.comm;
     c.comm = nullptr;
   }
+}
+
+void comm_init(Ctx& c, int rank, int nranks, const void* unique_id)
+{
+  PCLB_REQUIRE(nranks >= 1 && rank >= 0 && rank < nranks, PCLB200_ERR_INVALID, "bad rank / nranks");
+  comm_destroy(c);
   if (nranks == 1)
     return;
   ncclUniqueId id;
@@ -245,17 +256,6 @@ void comm_init(Ctx& c, int rank, int nranks, const void* unique_id)
   }
 }
 
-void comm_destroy(Ctx& c)
-{
-  if (c.comm) {
-    teardown_peer_reduce(*c.comm);
-    if (c.comm->comm)
-      nccl().CommDestroy(c.comm->comm);
-    delete c.comm;
-    c.comm = nullptr;
-  }
-}
-
 // ---- caller-bootstrapped peer exchange (no NCCL): export the local block's IPC handle, import everybody's ----------------
 // For deployments whose launcher already has a way to all-gather 64 bytes per rank (MPI, gloo, a file), and for
 // ranks that share one GPU (NCCL refuses duplicate devices; CUDA IPC does not).
@@ -267,8 +267,8 @@ void comm_export(Ctx& c, void* out64)
   Comm* cm = new Comm();
   c.comm = cm;
   PCLB_CUDA(cudaSetDevice(c.device));
-  PCLB_CUDA(cudaMalloc(reinterpret_cast<void**>(&cm->local_block), peer_block_bytes()));
-  PCLB_CUDA(cudaMemsetAsync(cm->local_block, 0, peer_block_bytes(), c.stream));
+  PCLB_CUDA(cudaMalloc(reinterpret_cast<void**>(&cm->local_block), kPeerBlockBytes));
+  PCLB_CUDA(cudaMemsetAsync(cm->local_block, 0, kPeerBlockBytes, c.stream));
   PCLB_CUDA(cudaStreamSynchronize(c.stream));
   cudaIpcMemHandle_t h;
   PCLB_CUDA(cudaIpcGetMemHandle(&h, cm->local_block));
@@ -282,29 +282,12 @@ void comm_import(Ctx& c, int rank, int nranks, const void* handles)
   Comm& cm = *c.comm;
   cm.rank = rank;
   cm.nranks = nranks;
-  const cudaIpcMemHandle_t* all = static_cast<const cudaIpcMemHandle_t*>(handles);
-  for (int p = 0; p < nranks; ++p) {
-    if (p == rank) {
-      cm.peer_block[p] = cm.local_block;
-      continue;
-    }
-    cudaError_t e = cudaIpcOpenMemHandle(&cm.peer_block[p], all[p], cudaIpcMemLazyEnablePeerAccess);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      cm.peer_block[p] = nullptr;
-      throw Error(PCLB200_ERR_CUDA, std::string("comm_import: cudaIpcOpenMemHandle failed for rank ") + std::to_string(p) +
-                                        ": " + cudaGetErrorString(e));
-    }
-  }
-  cm.view.rank = rank;
-  cm.view.nranks = nranks;
-  for (int p = 0; p < nranks; ++p) {
-    unsigned char* b = static_cast<unsigned char*>(cm.peer_block[p]);
-    cm.view.flags[p] = reinterpret_cast<unsigned long long*>(b);
-    cm.view.slots[p] = reinterpret_cast<double*>(b + kMaxRanks * sizeof(unsigned long long));
-  }
-  set_u64_view(cm);
-  cm.peer_ok = true;
+  cudaError_t e = cudaSuccess;
+  const int p = open_peers(static_cast<const cudaIpcMemHandle_t*>(handles), rank, nranks, cm.local_block, cm.peer_block, &e);
+  if (p >= 0)
+    throw Error(PCLB200_ERR_CUDA, std::string("comm_import: cudaIpcOpenMemHandle failed for rank ") + std::to_string(p) +
+                                      ": " + cudaGetErrorString(e));
+  use_peer_blocks(cm);
 }
 
 void comm_set_mode(Ctx& c, int mode)
@@ -323,10 +306,10 @@ bool comm_peer_fused(const Ctx& c) { return comm_active(c) && c.comm->peer_ok &&
 // view + next sequence number for a fused in-kernel exchange; returns false when the NCCL path must be used
 bool comm_peer_view(Ctx& c, PeerView* view, unsigned long long* seq)
 {
-  if (!comm_active(c) || !c.comm->peer_ok || c.comm->mode != PCLB200_REDUCE_FUSED)
+  if (!comm_peer_fused(c))
     return false;
   *view = c.comm->view;
-  *seq = ++c.comm->seq;
+  *seq = next_seq(*c.comm);
   return true;
 }
 
@@ -340,60 +323,20 @@ void comm_allreduce_sum(Ctx& c, double* d_buf, int count)
 }
 
 // ---- u64 collectives of the sharded rejectors ---------------------------------------------------------------------------
-// One block; the protocol of peer_exchange (icp_kernels.cuh) on the u64 region: store this rank's words into every rank's
-// words[seq & 1][rank][.], fence, publish seq in every rank's flags[rank], wait (10 s, then d_error = 2) until every peer
-// has published >= seq in ours, fold in rank order.  The sequence numbers come from the same counter as the accumulator
-// exchange and every rank draws them in the same order, so a peer is at most one exchange ahead and the parity pair of
-// the region is never overwritten while it is read.  count == 0 is a barrier.
-__global__ void __launch_bounds__(256)
-k_peer_u64(const PeerU64View v, unsigned long long seq, const unsigned long long* __restrict__ send,
-           unsigned long long* __restrict__ recv, int count, int op, int* __restrict__ d_error)
+// One block of kU64Words threads runs peer_exchange on the u64 region: element-wise sum or min (identity ~0) of count
+// <= kU64Words words; count == 0 is a barrier.
+__global__ void __launch_bounds__(kU64Words)
+k_peer_u64(const PeerView v, unsigned long long seq, const unsigned long long* send, unsigned long long* recv, int count,
+           int op, int* d_error)
 {
-  const int buf = (int)(seq & 1ull);
-  for (int i = threadIdx.x; i < count; i += blockDim.x) {
-    const unsigned long long x = send[i];
-    for (int p = 0; p < v.nranks; ++p)
-      v.words[p][((size_t)buf * kMaxRanks + v.rank) * kU64Words + i] = x;
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x < v.nranks)
-    *reinterpret_cast<volatile unsigned long long*>(&v.flags[threadIdx.x][v.rank]) = seq;
-  __shared__ int timed_out;
-  if (threadIdx.x == 0)
-    timed_out = 0;
-  __syncthreads();
-  if (threadIdx.x < v.nranks) {
-    const volatile unsigned long long* f = v.flags[v.rank] + threadIdx.x;
-    const long long t0 = clock64();
-    while (*f < seq) {
-      if (clock64() - t0 > 20000000000LL) {  // ~10 s: a peer died — fail loudly instead of hanging the GPU
-        timed_out = 1;
-        break;
-      }
-    }
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (timed_out) {
-    if (threadIdx.x == 0)
-      atomicExch(d_error, 2);
-    return;
-  }
-  const volatile unsigned long long* mine = v.words[v.rank] + (size_t)buf * kMaxRanks * kU64Words;
-  for (int i = threadIdx.x; i < count; i += blockDim.x) {
-    unsigned long long a = op == kU64Min ? ~0ull : 0ull;
-    for (int r = 0; r < v.nranks; ++r) {
-      const unsigned long long x = mine[(size_t)r * kU64Words + i];
-      a = op == kU64Min ? (x < a ? x : a) : a + x;
-    }
-    recv[i] = a;
-  }
+  const bool min = op == kU64Min;
+  peer_exchange(v, seq, send, recv, count, min ? ~0ull : 0ull,
+                [min](unsigned long long a, unsigned long long x) { return min ? (x < a ? x : a) : a + x; }, d_error);
 }
 
 static void peer_u64(Ctx& c, const unsigned long long* d_send, unsigned long long* d_recv, int count, int op)
 {
-  k_peer_u64<<<1, 256, 0, c.stream>>>(c.comm->uview, ++c.comm->seq, d_send, d_recv, count, op, c.d_error);
+  k_peer_u64<<<1, kU64Words, 0, c.stream>>>(c.comm->view, next_seq(*c.comm), d_send, d_recv, count, op, c.d_error);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
 }
@@ -430,7 +373,7 @@ unsigned long long comm_shard_offset(Ctx& c, unsigned long long n_q, unsigned lo
   PCLB_CUDA(cudaMemcpyAsync(d.p, v.data(), kMaxRanks * sizeof(unsigned long long), cudaMemcpyHostToDevice, c.stream));
   comm_allreduce_u64(c, d.p, d.p, kMaxRanks, kU64Sum);
   PCLB_CUDA(cudaMemcpyAsync(v.data(), d.p, kMaxRanks * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c.stream));
-  PCLB_CUDA(cudaStreamSynchronize(c.stream));
+  check_device_error(c);
   unsigned long long off = 0, tot = 0;
   for (int p = 0; p < c.comm->nranks; ++p) {
     if (p < c.comm->rank)
@@ -442,44 +385,28 @@ unsigned long long comm_shard_offset(Ctx& c, unsigned long long n_q, unsigned lo
 }
 
 // Maps every rank's table into this process: the IPC handles travel through the u64 region (one exchange), then every
-// rank reports whether it could open all of them (a second one) so that all ranks take the same decision.
+// rank reports whether it could open all of them (a second one) so that all ranks take the same decision.  The caller
+// releases the table when this throws.
 static void map_one_to_one(Ctx& c, OneToOneEntry& e)
 {
   Comm& cm = *c.comm;
   cudaStream_t st = c.stream;
-  static_assert(kMaxRanks * 8 <= kU64Words, "IPC handles must fit the u64 region");
-  std::vector<unsigned long long> h(kMaxRanks * 8, 0ull);
-  cudaIpcMemHandle_t mine;
-  PCLB_CUDA(cudaIpcGetMemHandle(&mine, e.local));
-  memcpy(&h[(size_t)cm.rank * 8], &mine, sizeof(mine));
+  constexpr int kWords = sizeof(cudaIpcMemHandle_t) / sizeof(unsigned long long);
+  static_assert(kMaxRanks * kWords <= kU64Words, "IPC handles must fit the u64 region");
+  std::vector<cudaIpcMemHandle_t> h(kMaxRanks);  // zero but for this rank's: the sum is every rank's handle
+  PCLB_CUDA(cudaIpcGetMemHandle(&h[cm.rank], e.local));
   DevBuf<unsigned long long> d;
-  d.alloc(h.size(), st);
-  PCLB_CUDA(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
-  comm_allreduce_u64(c, d.p, d.p, (size_t)cm.nranks * 8, kU64Sum);
-  PCLB_CUDA(cudaMemcpyAsync(h.data(), d.p, (size_t)cm.nranks * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  unsigned long long bad = 0;
-  for (int p = 0; p < cm.nranks; ++p) {
-    if (p == cm.rank) {
-      e.peer[p] = e.local;
-      continue;
-    }
-    cudaIpcMemHandle_t hp;
-    memcpy(&hp, &h[(size_t)p * 8], sizeof(hp));
-    if (cudaIpcOpenMemHandle(&e.peer[p], hp, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
-      cudaGetLastError();
-      e.peer[p] = nullptr;
-      bad = 1;
-    }
-  }
+  d.alloc((size_t)kMaxRanks * kWords, st);
+  PCLB_CUDA(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(cudaIpcMemHandle_t), cudaMemcpyHostToDevice, st));
+  comm_allreduce_u64(c, d.p, d.p, (size_t)cm.nranks * kWords, kU64Sum);
+  PCLB_CUDA(cudaMemcpyAsync(h.data(), d.p, cm.nranks * sizeof(cudaIpcMemHandle_t), cudaMemcpyDeviceToHost, st));
+  check_device_error(c);
+  unsigned long long bad = open_peers(h.data(), cm.rank, cm.nranks, e.local, e.peer) >= 0 ? 1 : 0;
   PCLB_CUDA(cudaMemcpyAsync(d.p, &bad, sizeof(bad), cudaMemcpyHostToDevice, st));
   comm_allreduce_u64(c, d.p, d.p, 1, kU64Sum);
   PCLB_CUDA(cudaMemcpyAsync(&bad, d.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  if (bad) {
-    e.release();
-    throw Error(PCLB200_ERR_CUDA, "one-to-one rejector: a rank could not map the peers' tables (CUDA IPC)");
-  }
+  check_device_error(c);
+  PCLB_REQUIRE(!bad, PCLB200_ERR_CUDA, "one-to-one rejector: a rank could not map the peers' tables (CUDA IPC)");
   e.mapped = true;
 }
 
@@ -507,8 +434,15 @@ OneToOneTables comm_one_to_one_tables(Ctx& c, std::shared_ptr<OneToOneEntry>& ow
   OneToOneTables t;
   t.local = e->local;
   if (comm_peer_fused(c)) {
-    if (!e->mapped)
-      map_one_to_one(c, *e);
+    if (!e->mapped) {
+      try {
+        map_one_to_one(c, *e);
+      }
+      catch (const Error&) {
+        e->release();
+        throw;
+      }
+    }
     t.peer = true;
     t.n_read = cm.nranks;
     for (int p = 0; p < cm.nranks; ++p)

@@ -79,7 +79,6 @@ __global__ void k_scatter_xyz(const float4* __restrict__ src, size_t n, unsigned
 // =============================================================================================================
 // host side
 // =============================================================================================================
-static void check_device_error(Ctx& c);
 
 // ---- GICP covariances -----------------------------------------------------------------------------------------------
 // GeneralizedIterativeClosestPoint::computeCovariances (registration/impl/gicp.hpp:69-147): per point, the covariance
@@ -534,17 +533,6 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   PCLB_CUDA(cudaGetLastError());
 }
 
-static void check_device_error(Ctx& c)
-{
-  int h = 0;
-  PCLB_CUDA(cudaMemcpyAsync(&h, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-  PCLB_CUDA(cudaStreamSynchronize(c.stream));
-  if (h) {
-    PCLB_CUDA(cudaMemsetAsync(c.d_error, 0, sizeof(int), c.stream));
-    throw Error(PCLB200_ERR_INTERNAL, "LBVH traversal stack overflow (tree deeper than the per-query stack)");
-  }
-}
-
 static void fill_stats(const Icp& s, pclb200_icp_stats* st)
 {
   if (!st)
@@ -640,12 +628,8 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
       PCLB_CUDA(cudaMemcpyAsync(h_ctrl, s.ctrl.p, sizeof(LoopCtrl), cudaMemcpyDeviceToHost, st));
       PCLB_CUDA(cudaMemcpyAsync(h_err, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
       PCLB_CUDA(cudaStreamSynchronize(st));
-      if (*h_err) {
-        PCLB_CUDA(cudaMemsetAsync(c.d_error, 0, sizeof(int), st));
-        if (*h_err == 2)
-          throw Error(PCLB200_ERR_NCCL, "fused cross-GPU reduce timed out waiting for a peer rank");
-        throw Error(PCLB200_ERR_INTERNAL, "LBVH traversal stack overflow (tree deeper than the per-query stack)");
-      }
+      if (*h_err)
+        raise_device_error(c, *h_err);
       s.loop = *h_ctrl;
     };
     IterArgs a;

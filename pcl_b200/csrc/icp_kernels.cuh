@@ -6,6 +6,7 @@
 #pragma once
 #include "internal.cuh"
 #include "corr_select.cuh"
+#include "peer_exchange.cuh"
 #include "traverse.cuh"
 
 namespace pclb200 {
@@ -138,54 +139,9 @@ struct IterArgs {
 
 // Fused all-reduce over NVLink peer memory (replaces a separate ncclAllReduce launch); called by every thread of the
 // LAST block of an accumulating kernel once a.accum[0..kAccum) holds this rank's totals.
-//   1. store this rank's totals into EVERY rank's slots[seq&1][rank][.]   (remote stores)
-//   2. fence, then publish the sequence number into every rank's flags[rank]
-//   3. wait until all peers have published >= seq in OUR flags, then fold the slots in rank order:
-//      every rank adds the same numbers in the same order => bitwise identical sums everywhere.
-// Two slot sets alternate by sequence parity: a peer can be at most one iteration ahead (it needs our flag for
-// seq+1 before it can finish seq+1), so it never overwrites what we are still reading.
 __device__ __forceinline__ void peer_exchange(const IterArgs& a)
 {
-  if (a.peer.nranks <= 1)
-    return;
-  __syncthreads();
-  const int buf = (int)(a.seq & 1ull);
-  if (threadIdx.x < kAccum) {
-    const double v = a.accum[threadIdx.x];
-    for (int p = 0; p < a.peer.nranks; ++p)
-      a.peer.slots[p][((size_t)buf * kMaxRanks + a.peer.rank) * kAccum + threadIdx.x] = v;
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x < a.peer.nranks)
-    *reinterpret_cast<volatile unsigned long long*>(&a.peer.flags[threadIdx.x][a.peer.rank]) = a.seq;
-  __shared__ int timed_out;
-  if (threadIdx.x == 0)
-    timed_out = 0;
-  __syncthreads();
-  if (threadIdx.x < a.peer.nranks) {
-    const volatile unsigned long long* f = a.peer.flags[a.peer.rank] + threadIdx.x;
-    const long long t0 = clock64();
-    while (*f < a.seq) {
-      if (clock64() - t0 > 20000000000LL) {  // ~10 s: a peer died — fail loudly instead of hanging the GPU
-        timed_out = 1;
-        break;
-      }
-    }
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (timed_out) {
-    if (threadIdx.x == 0)
-      atomicExch(a.d_error, 2);
-  }
-  else if (threadIdx.x < kAccum) {
-    double v = 0.0;
-    const volatile double* mine = a.peer.slots[a.peer.rank] + (size_t)buf * kMaxRanks * kAccum;
-    for (int r = 0; r < a.peer.nranks; ++r)
-      v += mine[(size_t)r * kAccum + threadIdx.x];
-    a.accum[threadIdx.x] = v;
-  }
+  peer_exchange(a.peer, a.seq, a.accum, a.accum, kAccum, 0.0, [](double s, double x) { return s + x; }, a.d_error);
 }
 
 template <int NACC>
@@ -571,7 +527,7 @@ k_search(const IterArgs a, Match* __restrict__ match, float* __restrict__ lbs)
       atomicAdd(a.skip_count, (unsigned long long)skipped);
   }
   if (overflow)
-    atomicExch(a.d_error, 1);
+    atomicExch(a.d_error, kErrStackOverflow);
 }
 
 // Streaming accumulation on the fp64 tensor cores: one pass over (source point, match) pairs, the normal equations
@@ -1210,14 +1166,14 @@ k_corr(const TreeView T, const float4* __restrict__ q,
     Nearest1 v{p.x, p.y, p.z, gate, kSentinelIndex, -1};
     WalkStats ws{};
     if (!nearest1<false>(T, p.x, p.y, p.z, v, -1, 1.00001f, ws))
-      atomicExch(d_error, 1);
+      atomicExch(d_error, kErrStackOverflow);
     if (v.best_pos >= 0) {
       bool keep = true;
       if (RECIP) {
         const float4 t = ldg4(T.pts + v.best_pos);
         Nearest1 b{t.x, t.y, t.z, gate, kSentinelIndex, -1};
         if (!traverse(s_nodes, s_pts, s_root, t.x, t.y, t.z, b))
-          atomicExch(d_error, 1);
+          atomicExch(d_error, kErrStackOverflow);
         keep = b.best_pos >= 0 && b.best_idx == my_orig;
       }
       if (keep) {
@@ -1250,7 +1206,7 @@ k_fitness(const TreeView T, const float4* __restrict__ q, size_t nq, double max_
     }
   }
   if (overflow)
-    atomicExch(pub.d_error, 1);
+    atomicExch(pub.d_error, kErrStackOverflow);
   block_reduce_and_publish<2>(acc, pub);
 }
 

@@ -59,9 +59,16 @@ struct Ctx {
   uint64_t launches = 0;  // kernels launched by this library (incl. CUB passes, counted per call)
   void* pinned = nullptr; // small pinned staging block for per-iteration read-backs
   size_t pinned_bytes = 0;
-  int* d_error = nullptr; // device-side invariant flag (traversal stack overflow)
+  int* d_error = nullptr; // device-side error flag: 0 or one of kErr*
   Comm* comm = nullptr;
 };
+
+// values a kernel stores into *Ctx::d_error
+enum { kErrStackOverflow = 1, kErrPeerTimeout = 2 };
+// the Error a non-zero device error flag stands for; clears the flag (on the ctx stream) and throws it
+[[noreturn]] void raise_device_error(Ctx& c, int code);
+// synchronises the ctx stream, then raise_device_error if a kernel set the flag
+void check_device_error(Ctx& c);
 
 // records a CUDA-event pair around a region of the ctx stream when profiling is on
 struct ProfScope {
@@ -254,28 +261,25 @@ void apply_rejector(Ctx& c, const pclb200_rejector& r, const RejectArrays& a, in
 // accumulators of one ICP iteration (all fp64), see icp.cu
 constexpr int kAccum = 40;
 
-// Cross-GPU exchange buffers of the fused reduce (comm.cu): every rank owns one block
-//   flags[kMaxRanks] (u64, latest sequence number published by each peer) | slots[2][kMaxRanks][kAccum] (fp64)
-// mapped into every peer through CUDA IPC, so a kernel on rank r can store its partial sums straight into
-// rank p's slots[.][r][.] over NVLink.
+// Cross-GPU exchange block of the fused reduce (comm.cu): every rank owns one, mapped into every peer through CUDA IPC
+//   flags[kMaxRanks]                  u64, the latest sequence number published by each peer
+//   slots[2][kMaxRanks][kAccum]       fp64: the accumulators of one ICP iteration (accumulate kernels, icp_kernels.cuh)
+//   words[2][kMaxRanks][kU64Words]    u64: sums, minima and barriers of the rejector chain on a sharded source (reject.cu)
+// so a kernel on rank r stores its values straight into rank p's region[.][r][.] over NVLink.  Both regions follow one
+// protocol (peer_exchange.cuh) with the same flags and one sequence counter.
 constexpr int kMaxRanks = 8;
+constexpr int kU64Words = 256;  // one histogram of 8-bit digits; also holds kMaxRanks IPC handles (8 words each)
+constexpr size_t kPeerSlotsOffset = kMaxRanks * sizeof(unsigned long long);
+constexpr size_t kPeerWordsOffset = kPeerSlotsOffset + 2ull * kMaxRanks * kAccum * sizeof(double);
+constexpr size_t kPeerBlockBytes = kPeerWordsOffset + 2ull * kMaxRanks * kU64Words * sizeof(unsigned long long);
 struct PeerView {
   int rank = 0;
   int nranks = 0;                       // 0 / 1 = no exchange
-  unsigned long long* flags[kMaxRanks]; // flags[p] = base of rank p's flag array (peer-mapped, [rank] = self)
+  unsigned long long* flags[kMaxRanks]; // flags[p] = base of rank p's block (its flag array; peer-mapped, [rank] = self)
   double* slots[kMaxRanks];             // slots[p] = base of rank p's slot array
 };
 
 // ---- cross-rank u64 collectives (comm.cu) for the rejector chain on a sharded source (reject.cu) ----------------------
-// The peer block continues after the fp64 slots with words[2][kMaxRanks][kU64Words] (u64): the same flags and sequence
-// numbers as the accumulator exchange, a separate region, so the kernels of that exchange are untouched.
-constexpr int kU64Words = 256;  // one histogram of 8-bit digits; also holds kMaxRanks IPC handles (8 words each)
-struct PeerU64View {
-  int rank = 0;
-  int nranks = 0;
-  unsigned long long* flags[kMaxRanks];  // = PeerView::flags
-  unsigned long long* words[kMaxRanks];  // words[p] = base of rank p's u64 region
-};
 enum { kU64Sum = 0, kU64Min = 1 };
 // element-wise sum / min over the ranks, enqueued on the ctx stream; send == recv is allowed.  The peer-mapped path moves
 // at most kU64Words words; NCCL any count.

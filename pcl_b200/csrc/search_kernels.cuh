@@ -76,7 +76,7 @@ k_knn(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, int roo
   // a non-finite query has no neighbours (every comparison with NaN fails; rows stay (-1, +inf)) — without the guard
   // it would walk the whole tree, because a NaN box bound never prunes
   if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, 1);
+    atomicExch(d_error, kErrStackOverflow);
 #pragma unroll
   for (int j = 0; j < K; ++j)
     if (j < k_out) {
@@ -140,7 +140,7 @@ k_knn_any(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, int
     v.pos[j] = -1;
   }
   if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, 1);
+    atomicExch(d_error, kErrStackOverflow);
   for (int j = 0; j < k; ++j) {
     int p = v.pos[j];
     v.pos[j] = p >= 0 ? v.orig(p) : -1;
@@ -170,7 +170,7 @@ k_knn_stats(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, i
     v.pts = pts;
     v.init(__int_as_float(0x7f800000));
     if (!traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-      atomicExch(d_error, 1);
+      atomicExch(d_error, kErrStackOverflow);
     double sum = 0.0;
     int cnt = 0;
 #pragma unroll
@@ -269,7 +269,7 @@ k_radius_count(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts
   RadiusCount v{qq.x, qq.y, qq.z, r2, r2_below, 0ULL};
   // a non-finite query has no neighbour (every comparison with NaN fails) — and would otherwise walk the whole tree
   if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, 1);
+    atomicExch(d_error, kErrStackOverflow);
   counts[(size_t)(unsigned)__float_as_int(qq.w)] = v.n;
 }
 
@@ -285,7 +285,7 @@ k_radius_fill(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts,
   const float4 qq = __ldg(q + i);
   RadiusFill v{qq.x, qq.y, qq.z, r2, r2_below, keys + offsets[(size_t)(unsigned)__float_as_int(qq.w)]};
   if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, 1);
+    atomicExch(d_error, kErrStackOverflow);
 }
 
 // k-NN -> shifted single-pass covariance in the neighbour order the search returns
@@ -315,7 +315,7 @@ k_normals(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, int
   v.pts = pts;
   v.init(__int_as_float(0x7f800000));
   if (!traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, 1);
+    atomicExch(d_error, kErrStackOverflow);
   int cnt = 0;
 #pragma unroll
   for (int j = 0; j < K; ++j)

@@ -3,7 +3,7 @@
 Two PROCESSES, both on cuda:0 (NCCL refuses duplicate devices; the library's fused exchange only needs CUDA IPC, which
 the caller bootstraps with pclb200_comm_export / _import over gloo).  Each rank holds a replica of the target index and
 one half of the source; every iteration's 40 accumulators cross between the two processes through the peer-mapped
-exchange block inside the iteration kernel (comm.cu + icp.cu: peer_exchange).  The sharded result must equal the
+exchange block inside the iteration kernel (comm.cu + peer_exchange.cuh).  The sharded result must equal the
 single-process result on the whole cloud: same correspondence counts, same iterations, transform within 1e-6."""
 import os
 import sys
