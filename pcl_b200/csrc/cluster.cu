@@ -15,8 +15,6 @@
 
 namespace pclb200 {
 
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 // labels: idx.n_cloud entries on the device; -1 for points the index does not hold (non-finite, outside the subset)
 void cluster_labels(Ctx& c, const Index& idx, double tolerance, int32_t* d_labels)
 {

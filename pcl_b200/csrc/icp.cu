@@ -35,8 +35,6 @@ bool comm_active(const Ctx& c);
 bool comm_peer_view(Ctx& c, PeerView* view, unsigned long long* seq);
 bool comm_peer_fused(const Ctx& c);  // the per-iteration exchange happens inside the accumulate kernel
 
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 // ---- misc streaming kernels ------------------------------------------------------------------------------
 __global__ void k_apply_pending(float4* __restrict__ pts, size_t n, const Pending* __restrict__ pending,
                                 float4* __restrict__ normals /* nullable */)
@@ -94,28 +92,19 @@ void gicp_covariances(Ctx& c, Index& idx, const void* pts, size_t n, size_t stri
   PCLB_REQUIRE(k >= 1, PCLB200_ERR_INVALID, "k must be positive");
   const int keff = (int)std::min<size_t>((size_t)k, idx.n_valid);
   DevBuf<float4> dense;
-  dense.alloc(n, st);
-  load_xyz_as_float4(c, pts, n, stride, nullptr, 0, dense.p, st);
-  QueryBatch qb;
-  make_query_batch(c, idx, dense.p, n, qb);
+  QueryBatch qb = load_queries(c, idx, pts, n, stride, nullptr, 0, dense);
   DevBuf<int32_t> rows;
   DevBuf<float> rows_d2;
   rows.alloc(n * (size_t)keff, st);
   rows_d2.alloc(n * (size_t)keff, st);
   launch_knn(c, idx, qb.q.p, n, keff, std::numeric_limits<float>::infinity(), rows.p, rows_d2.p);
   ensure_pos_of_orig(c, idx);
-  DevBuf<double> d_out;
-  const bool on_dev = is_device_ptr(out);
-  double* d_o = out;
-  if (!on_dev) {
-    d_out.alloc(n * 9, st);
-    d_o = d_out.p;
-  }
+  DevBuf<double> tmp;
+  double* d_o = out_on_device(c, out, n * 9, tmp);
   k_gicp_cov<<<grid_for(n, 128), 128, 0, st>>>(dense.p, n, rows.p, keff, k, idx.pts.p, idx.pos_of_orig.p, gicp_epsilon, d_o);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
-  if (!on_dev)
-    PCLB_CUDA(cudaMemcpyAsync(out, d_out.p, n * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  copy_out(c, out, tmp, n * 9);
   check_device_error(c);
 }
 
@@ -460,8 +449,7 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
     // one contiguous H2D of the records; every field other than xyz/normals is carried through to the output
     PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
     s.src_raw.alloc(n * stride, st);
-    PCLB_CUDA(cudaMemcpyAsync(s.src_raw.p, src, n * stride,
-                              is_device_ptr(src) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    PCLB_CUDA(cudaMemcpyAsync(s.src_raw.p, src, n * stride, cudaMemcpyDefault, st));
     src_dev = s.src_raw.p;
   }
   load_xyz_as_float4(c, src_dev, n, stride, nullptr, 0, s.src_all.p, st);
@@ -482,8 +470,7 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   if (indices) {
     s.n_q = n_idx;
     s.src_orig.alloc(n_idx, st);
-    PCLB_CUDA(cudaMemcpyAsync(s.src_orig.p, indices, n_idx * sizeof(int32_t),
-                              is_device_ptr(indices) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    PCLB_CUDA(cudaMemcpyAsync(s.src_orig.p, indices, n_idx * sizeof(int32_t), cudaMemcpyDefault, st));
     sub.alloc(n_idx, st);
     if (n_idx) {
       k_gather_subset<<<grid_for(n_idx, 256), 256, 0, st>>>(s.src_all.p, s.src_orig.p, n_idx, sub.p);
@@ -755,10 +742,6 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
   fill_stats(s, stats);
 }
 
-struct CorrValid {
-  __host__ __device__ bool operator()(const pclb200_corr& c) const { return c.index_match >= 0; }
-};
-
 // correspondences of the last evaluated iteration (Registration::correspondences_, what PCL hands to the
 // visualisation callback at icp.hpp:228-236), ordered by position in the source index list
 __global__ void k_matches_to_corr(const float4* __restrict__ cur, const Match* __restrict__ match, size_t n,
@@ -785,25 +768,11 @@ size_t icp_get_correspondences(Icp& s, pclb200_corr* out)
   PCLB_REQUIRE(s.tgt && s.cur.p && s.match.p, PCLB200_ERR_INVALID, "icp: no iteration has run");
   if (!s.n_q || s.loop.iterations == 0)
     return 0;
-  DevBuf<pclb200_corr> by_slot, compact;
-  DevBuf<size_t> d_count;
+  DevBuf<pclb200_corr> by_slot;
   by_slot.alloc(s.n_q, st);
-  compact.alloc(s.n_q, st);
-  d_count.alloc(1, st);
   k_matches_to_corr<<<grid_for(s.n_q, 256), 256, 0, st>>>(s.cur.p, s.match.p, s.n_q, s.tgt->pts.p, s.src_orig.p, by_slot.p);
   ++c.launches;
-  size_t tmp_bytes = 0;
-  PCLB_CUDA(cub::DeviceSelect::If(nullptr, tmp_bytes, by_slot.p, compact.p, d_count.p, (int)s.n_q, CorrValid(), st));
-  DevBuf<unsigned char> tmp;
-  tmp.alloc(tmp_bytes, st);
-  PCLB_CUDA(cub::DeviceSelect::If(tmp.p, tmp_bytes, by_slot.p, compact.p, d_count.p, (int)s.n_q, CorrValid(), st));
-  c.launches += 2;
-  size_t m = 0;
-  PCLB_CUDA(cudaMemcpyAsync(&m, d_count.p, sizeof(size_t), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  if (m)
-    PCLB_CUDA(cudaMemcpyAsync(out, compact.p, m * sizeof(pclb200_corr),
-                              is_device_ptr(out) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  const size_t m = compact_corr_to(c, by_slot.p, s.n_q, out);
   PCLB_CUDA(cudaStreamSynchronize(st));
   return m;
 }
@@ -843,14 +812,7 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
   if (s.src_raw.p && stride_out == s.src_stride && (!do_n || normals_inside)) {
     // output = *input_ (all fields), then xyz / normals overwritten: assembled on the device, one contiguous copy out
     DevBuf<unsigned char> rec;
-    unsigned char* d_rec = nullptr;
-    const bool out_dev = is_device_ptr(out_pts);
-    if (out_dev)
-      d_rec = static_cast<unsigned char*>(out_pts);
-    else {
-      rec.alloc(s.n_all * stride_out, st);
-      d_rec = rec.p;
-    }
+    unsigned char* d_rec = out_on_device(c, static_cast<unsigned char*>(out_pts), s.n_all * stride_out, rec);
     PCLB_CUDA(cudaMemcpyAsync(d_rec, s.src_raw.p, s.n_all * stride_out, cudaMemcpyDeviceToDevice, st));
     k_scatter_xyz<<<grid_for(s.n_all, 256), 256, 0, st>>>(tmp.p, s.n_all, d_rec, stride_out, 0, 0.f);
     ++c.launches;
@@ -858,8 +820,7 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
       k_scatter_xyz<<<grid_for(s.n_all, 256), 256, 0, st>>>(tmpn.p, s.n_all, d_rec + s.src_normal_off, stride_out, 0, 0.f);
       ++c.launches;
     }
-    if (!out_dev)
-      PCLB_CUDA(cudaMemcpyAsync(out_pts, d_rec, s.n_all * stride_out, cudaMemcpyDeviceToHost, st));
+    copy_out(c, static_cast<unsigned char*>(out_pts), rec, s.n_all * stride_out);
     PCLB_CUDA(cudaStreamSynchronize(st));
     return;
   }
@@ -902,11 +863,12 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
   PCLB_REQUIRE(src && tgt && n > 0, PCLB200_ERR_INVALID, "estimate: empty input");
   // the caller's arrays are indexed by corr[].index_*; without their sizes we need the max index
   size_t n_src = n, n_tgt = n;
-  DevBuf<pclb200_corr> d_corr;
+  DevBuf<pclb200_corr> staged_corr;
+  const pclb200_corr* d_corr = on_device(c, corr, n, staged_corr);
   if (corr) {
     std::vector<pclb200_corr> hc;
     const pclb200_corr* hcorr = corr;
-    if (is_device_ptr(corr)) {
+    if (d_corr == corr) {  // the caller's list is in device memory: scan a host copy
       hc.resize(n);
       PCLB_CUDA(cudaMemcpy(hc.data(), corr, n * sizeof(pclb200_corr), cudaMemcpyDeviceToHost));
       hcorr = hc.data();
@@ -919,8 +881,6 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
     }
     n_src = (size_t)mq + 1;
     n_tgt = (size_t)mm + 1;
-    d_corr.alloc(n, st);
-    PCLB_CUDA(cudaMemcpyAsync(d_corr.p, hcorr, n * sizeof(pclb200_corr), cudaMemcpyHostToDevice, st));
     PCLB_CUDA(cudaStreamSynchronize(st));
   }
   DevBuf<float4> ds, dt, dn;
@@ -951,7 +911,7 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
   a.tgt_normals = dn.p;
   a.src_normals = dsn.p;
   a.enforce_same_dir = enforce_same_dir;
-  a.corr = d_corr.p;
+  a.corr = d_corr;
   a.n = n;
   a.ox = a.oy = a.oz = 0.f;
   a.pub.partials = red.partials.p;
@@ -1009,41 +969,23 @@ size_t correspondences(Ctx& c, const Index& tgt, const Index* src_index, const v
     k_apply_pending<<<persistent_grid(c, nq, 256, 8), 256, 0, st>>>(dense.p, nq, pend.p, nullptr);
     ++c.launches;
   }
-  DevBuf<int32_t> d_ind;
-  if (indices) {
-    d_ind.alloc(n_idx, st);
-    PCLB_CUDA(cudaMemcpyAsync(d_ind.p, indices, n_idx * sizeof(int32_t),
-                              is_device_ptr(indices) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-  }
+  DevBuf<int32_t> staged_ind;
+  const int32_t* d_ind = on_device(c, indices, n_idx, staged_ind);
   QueryBatch qb;
   make_query_batch(c, tgt, dense.p, nq, qb);
-  DevBuf<pclb200_corr> by_slot, compact;
-  DevBuf<size_t> d_count;
+  DevBuf<pclb200_corr> by_slot;
   by_slot.alloc(nq, st);
-  compact.alloc(nq, st);
-  d_count.alloc(1, st);
   const float gate = gate_override ? *gate_override : gate_from_max_dist(max_dist);
   if (src_index)
     k_corr<true><<<grid_for(nq, 128), 128, 0, st>>>(tree_view(tgt), qb.q.p, nq, gate,
-                                                   src_index->nodes.p, src_index->pts.p, src_index->root, d_ind.p,
+                                                   src_index->nodes.p, src_index->pts.p, src_index->root, d_ind,
                                                    by_slot.p, c.d_error);
   else
     k_corr<false><<<grid_for(nq, 128), 128, 0, st>>>(tree_view(tgt), qb.q.p, nq, gate, nullptr,
-                                                    nullptr, 0, d_ind.p, by_slot.p, c.d_error);
+                                                    nullptr, 0, d_ind, by_slot.p, c.d_error);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
-  size_t tmp_bytes = 0;
-  PCLB_CUDA(cub::DeviceSelect::If(nullptr, tmp_bytes, by_slot.p, compact.p, d_count.p, (int)nq, CorrValid(), st));
-  DevBuf<unsigned char> tmp;
-  tmp.alloc(tmp_bytes, st);
-  PCLB_CUDA(cub::DeviceSelect::If(tmp.p, tmp_bytes, by_slot.p, compact.p, d_count.p, (int)nq, CorrValid(), st));
-  c.launches += 2;
-  size_t m = 0;
-  PCLB_CUDA(cudaMemcpyAsync(&m, d_count.p, sizeof(size_t), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  if (m)
-    PCLB_CUDA(cudaMemcpyAsync(out, compact.p, m * sizeof(pclb200_corr),
-                              is_device_ptr(out) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  const size_t m = compact_corr_to(c, by_slot.p, nq, out);
   check_device_error(c);
   return m;
 }

@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <stdexcept>
@@ -141,6 +142,47 @@ struct DevBuf {
 
 bool is_device_ptr(const void* p);
 
+#ifdef __CUDACC__
+// blocks of a 1-D launch over n items.  Only the .cu drivers launch; the kernel headers compiled by g++ for the host
+// tests (tests/host) bring their own launcher and grid size.
+inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
+#endif
+
+// Any caller array may live in host or device memory (DESIGN.md §1).  The kernels read an input through on_device: the
+// caller's pointer when it is device memory (or null / empty), else `staging` after an upload of its first n elements
+// enqueued on the ctx stream.  A strided array passes T = unsigned char and the byte count up to its last needed byte.
+template <typename T>
+const T* on_device(Ctx& c, const T* p, size_t n, DevBuf<T>& staging)
+{
+  if (!p || n == 0 || is_device_ptr(p))
+    return p;
+  staging.alloc(n, c.stream);
+  PCLB_CUDA(cudaMemcpyAsync(staging.p, p, n * sizeof(T), cudaMemcpyHostToDevice, c.stream));
+  return staging.p;
+}
+// The kernels write an output of n elements through out_on_device: the caller's pointer when it is device memory (or
+// null), else the temporary `tmp`.  copy_out then moves the first n elements of the temporary to the caller; it does
+// nothing when the kernel wrote in place.
+template <typename T>
+T* out_on_device(Ctx& c, T* p, size_t n, DevBuf<T>& tmp)
+{
+  if (!p || is_device_ptr(p))
+    return p;
+  tmp.alloc(n, c.stream);
+  return tmp.p;
+}
+template <typename T>
+void copy_out(Ctx& c, T* p, const DevBuf<T>& tmp, size_t n)
+{
+  if (tmp.p && n)
+    PCLB_CUDA(cudaMemcpyAsync(p, tmp.p, n * sizeof(T), cudaMemcpyDeviceToHost, c.stream));
+}
+// Keeps the entries of a device correspondence list with index_match >= 0 (or those whose flag is set), in order, and
+// writes them to the caller's host or device array.  Returns their number; the ctx stream has synchronised once to read
+// it, and the copy to the caller is enqueued after that.
+size_t compact_corr_to(Ctx& c, const pclb200_corr* d_in, size_t n, pclb200_corr* caller_out);
+size_t compact_corr_to(Ctx& c, const pclb200_corr* d_in, const unsigned char* d_flags, size_t n, pclb200_corr* caller_out);
+
 // Copies `count` records of `rec_bytes` (<= stride) from a strided host-or-device array into a
 // dense device array of float4 {x,y,z,w_fill}: the layout every kernel reads with 128-bit loads.
 // If `subset` != NULL, record i is src[subset[i]].
@@ -212,6 +254,10 @@ struct QueryBatch {
 };
 void make_query_batch(Ctx& c, const Index& ref_frame, const float4* d_q /*n, w ignored*/, size_t n,
                       QueryBatch& out);
+// load_xyz_as_float4 of a caller's query points into `dense` (kept alive: some kernels read it in input order), then
+// make_query_batch over it
+QueryBatch load_queries(Ctx& c, const Index& ref_frame, const void* pts, size_t n, size_t stride, const int32_t* subset,
+                        size_t n_subset, DevBuf<float4>& dense);
 
 // ---------------------------------------------------------------------------------------------
 // search / registration kernels (search.cu, icp.cu, voxel.cu)
@@ -234,8 +280,20 @@ void radius_fill_sorted(Ctx& c, const Index& idx, const float4* d_q, size_t nq, 
                         DevBuf<unsigned long long>& keys_sorted);
 void radius_csr(Ctx& c, const Index& idx, const float4* d_q, size_t nq, float r2, DevBuf<unsigned long long>& counts,
                 DevBuf<unsigned long long>& offsets, DevBuf<unsigned long long>& keys_sorted, unsigned long long& total);
+// radiusSearch of a caller's query batch (pclb200_radius / pclb200_radius_into).  `sink(total)` returns where the packed
+// lists go (host or device pointers; {nullptr, nullptr} = do not deliver, e.g. the caller's buffers are too small);
+// offsets are written to out_offsets (host or device, nq + 1 entries).
+struct RadiusSinkBuffers {
+  int32_t* idx;
+  float* d2;
+};
+void radius_search(Ctx& c, const Index& idx, const void* queries, size_t nq, size_t stride, double radius, unsigned max_nn,
+                   int64_t* out_offsets, const std::function<RadiusSinkBuffers(unsigned long long)>& sink);
+void launch_normals(Ctx& c, Index& idx, const float4* d_q, size_t nq, int k, const float vp[3], float4* d_out,
+                    int* d_not_dense);
 void launch_normals_radius(Ctx& c, Index& idx, const float4* d_q, size_t nq, float r2, const float vp[3], float4* d_out,
                            int* d_not_dense);
+void launch_knn_stats(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_mean, float* d_kth);
 // correspondences chosen among the k nearest with the help of normals; surface-normal rejector (normals_corr.cu)
 size_t correspondences_by_normals(Ctx& c, Index& tgt, int kind, const void* src, size_t n, size_t stride,
                                   const void* src_normals, size_t stride_sn, const void* tgt_normals, size_t stride_tn,

@@ -61,29 +61,18 @@ static void strided_to_float4(Ctx& c, const void* src, size_t n_records, size_t 
     return;
   PCLB_REQUIRE(src != nullptr, PCLB200_ERR_INVALID, "null point array");
   PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
-  const bool on_device = is_device_ptr(src);
   if (!subset && stride == 16) {
     // pcl::PointXYZ records already are float4: one straight copy (w is never read by the kernels)
-    PCLB_CUDA(cudaMemcpyAsync(d_out, src, n * 16, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+    PCLB_CUDA(cudaMemcpyAsync(d_out, src, n * 16, is_device_ptr(src) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                              s));
     return;
   }
+  // only up to the last byte a record's xyz can occupy: `src` may point INSIDE the caller's records (normals at offset 16
+  // of a PointNormal), so n_records * stride bytes would run past the end of the caller's array
   DevBuf<unsigned char> staged;
   DevBuf<int32_t> staged_sub;
-  const unsigned char* d_src = static_cast<const unsigned char*>(src);
-  if (!on_device) {
-    // only up to the last byte a record's xyz can occupy: `src` may point INSIDE the caller's records (normals at
-    // offset 16 of a PointNormal), so n_records * stride bytes would run past the end of the caller's array
-    const size_t bytes = (n_records - 1) * stride + 12;
-    staged.alloc(bytes, s);
-    PCLB_CUDA(cudaMemcpyAsync(staged.p, src, bytes, cudaMemcpyHostToDevice, s));
-    d_src = staged.p;
-  }
-  const int32_t* d_sub = subset;
-  if (subset && !is_device_ptr(subset)) {
-    staged_sub.alloc(n_subset, s);
-    PCLB_CUDA(cudaMemcpyAsync(staged_sub.p, subset, n_subset * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    d_sub = staged_sub.p;
-  }
+  const unsigned char* d_src = on_device(c, static_cast<const unsigned char*>(src), (n_records - 1) * stride + 12, staged);
+  const int32_t* d_sub = on_device(c, subset, n_subset, staged_sub);
   k_strided_to_float4<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_src, stride, d_sub, n, w_fill, d_out);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
@@ -99,8 +88,6 @@ void load_vec3_as_float4(Ctx& c, const void* src, size_t n_records, size_t strid
 {
   strided_to_float4(c, src, n_records, stride, nullptr, 0, 0.f, d_out, s);
 }
-
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
 
 struct SortedCloud {
   DevBuf<unsigned long long> keys;  // sorted
@@ -334,17 +321,7 @@ Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32
   dense.alloc(cnt, s);
   load_xyz_as_float4(c, pts, n, stride, subset, n_subset, dense.p, s);
   DevBuf<int32_t> d_sub;
-  const int32_t* d_orig = nullptr;
-  if (subset) {
-    if (is_device_ptr(subset))
-      d_orig = subset;
-    else {
-      d_sub.alloc(n_subset, s);
-      PCLB_CUDA(cudaMemcpyAsync(d_sub.p, subset, n_subset * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-      d_orig = d_sub.p;
-    }
-  }
-  return build_from_dense(c, dense.p, cnt, d_orig, n, true);
+  return build_from_dense(c, dense.p, cnt, on_device(c, subset, n_subset, d_sub), n, true);
 }
 
 Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig)
@@ -399,6 +376,58 @@ void make_query_batch(Ctx& c, const Index& frame, const float4* d_q, size_t n, Q
   k_gather_queries<<<grid_for(n, 256), 256, 0, s>>>(d_q, sc.vals.p, n, out.q.p);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
+}
+
+QueryBatch load_queries(Ctx& c, const Index& frame, const void* pts, size_t n, size_t stride, const int32_t* subset,
+                        size_t n_subset, DevBuf<float4>& dense)
+{
+  const size_t nq = subset ? n_subset : n;
+  dense.alloc(nq, c.stream);
+  load_xyz_as_float4(c, pts, n, stride, subset, n_subset, dense.p, c.stream);
+  QueryBatch qb;
+  make_query_batch(c, frame, dense.p, nq, qb);
+  return qb;
+}
+
+// ---- correspondence lists to the caller ---------------------------------------------------------------------------
+struct CorrValid {
+  __host__ __device__ bool operator()(const pclb200_corr& c) const { return c.index_match >= 0; }
+};
+
+// select(temp, temp_bytes, d_out, d_count): one cub::DeviceSelect call of the two-phase protocol
+template <typename Select>
+static size_t compact_with(Ctx& c, size_t n, pclb200_corr* out, Select&& select)
+{
+  cudaStream_t st = c.stream;
+  DevBuf<pclb200_corr> staged;
+  DevBuf<size_t> d_count;
+  pclb200_corr* d_out = out_on_device(c, out, n, staged);
+  d_count.alloc(1, st);
+  size_t tmp_bytes = 0;
+  PCLB_CUDA(select(nullptr, tmp_bytes, d_out, d_count.p));
+  DevBuf<unsigned char> tmp;
+  tmp.alloc(tmp_bytes, st);
+  PCLB_CUDA(select(tmp.p, tmp_bytes, d_out, d_count.p));
+  c.launches += 2;
+  size_t m = 0;
+  PCLB_CUDA(cudaMemcpyAsync(&m, d_count.p, sizeof(size_t), cudaMemcpyDeviceToHost, st));
+  PCLB_CUDA(cudaStreamSynchronize(st));
+  copy_out(c, out, staged, m);
+  return m;
+}
+
+size_t compact_corr_to(Ctx& c, const pclb200_corr* d_in, size_t n, pclb200_corr* out)
+{
+  return compact_with(c, n, out, [&](void* tmp, size_t& tb, pclb200_corr* d_out, size_t* d_count) {
+    return cub::DeviceSelect::If(tmp, tb, d_in, d_out, d_count, (int)n, CorrValid(), c.stream);
+  });
+}
+
+size_t compact_corr_to(Ctx& c, const pclb200_corr* d_in, const unsigned char* d_flags, size_t n, pclb200_corr* out)
+{
+  return compact_with(c, n, out, [&](void* tmp, size_t& tb, pclb200_corr* d_out, size_t* d_count) {
+    return cub::DeviceSelect::Flagged(tmp, tb, d_in, d_flags, d_out, d_count, (int)n, c.stream);
+  });
 }
 
 }  // namespace pclb200

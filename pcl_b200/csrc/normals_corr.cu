@@ -16,12 +16,6 @@
 
 namespace pclb200 {
 
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
-struct CorrHasMatch {
-  __host__ __device__ bool operator()(const pclb200_corr& c) const { return c.index_match >= 0; }
-};
-
 size_t correspondences_by_normals(Ctx& c, Index& tgt, int kind, const void* src, size_t n, size_t stride,
                                   const void* src_normals, size_t stride_sn, const void* tgt_normals, size_t stride_tn,
                                   const int32_t* indices, size_t n_idx, int k, double max_dist, pclb200_corr* out)
@@ -32,22 +26,15 @@ size_t correspondences_by_normals(Ctx& c, Index& tgt, int kind, const void* src,
   if (nq == 0 || keff <= 0)
     return 0;
   DevBuf<float4> dense, sn, tn;
-  dense.alloc(nq, st);
-  load_xyz_as_float4(c, src, n, stride, indices, n_idx, dense.p, st);
+  QueryBatch qb = load_queries(c, tgt, src, n, stride, indices, n_idx, dense);
   sn.alloc(n, st);
   load_vec3_as_float4(c, src_normals, n, stride_sn, sn.p, st);
   if (kind == PCLB200_CORR_BACK_PROJECTION) {
     tn.alloc(tgt.n_cloud, st);
     load_vec3_as_float4(c, tgt_normals, tgt.n_cloud, stride_tn, tn.p, st);
   }
-  DevBuf<int32_t> d_ind;
-  if (indices) {
-    d_ind.alloc(n_idx, st);
-    PCLB_CUDA(cudaMemcpyAsync(d_ind.p, indices, n_idx * sizeof(int32_t),
-                              is_device_ptr(indices) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-  }
-  QueryBatch qb;
-  make_query_batch(c, tgt, dense.p, nq, qb);
+  DevBuf<int32_t> staged_ind;
+  const int32_t* d_ind = on_device(c, indices, n_idx, staged_ind);
   DevBuf<int32_t> nn_idx;
   DevBuf<float> nn_d2;
   nn_idx.alloc(nq * (size_t)keff, st);
@@ -57,27 +44,13 @@ size_t correspondences_by_normals(Ctx& c, Index& tgt, int kind, const void* src,
     launch_knn(c, tgt, qb.q.p, nq, keff, std::numeric_limits<float>::infinity(), nn_idx.p, nn_d2.p);
   }
   ensure_pos_of_orig(c, tgt);
-  DevBuf<pclb200_corr> by_slot, compact;
-  DevBuf<size_t> d_count;
+  DevBuf<pclb200_corr> by_slot;
   by_slot.alloc(nq, st);
-  compact.alloc(nq, st);
-  d_count.alloc(1, st);
-  k_corr_by_normals<<<grid_for(nq, 128), 128, 0, st>>>(dense.p, nq, d_ind.p, sn.p, kind, keff, nn_idx.p, nn_d2.p,
+  k_corr_by_normals<<<grid_for(nq, 128), 128, 0, st>>>(dense.p, nq, d_ind, sn.p, kind, keff, nn_idx.p, nn_d2.p,
                                                       tgt.pts.p, tgt.pos_of_orig.p, tn.p, max_dist, by_slot.p);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
-  size_t tmp_bytes = 0;
-  PCLB_CUDA(cub::DeviceSelect::If(nullptr, tmp_bytes, by_slot.p, compact.p, d_count.p, (int)nq, CorrHasMatch(), st));
-  DevBuf<unsigned char> tmp;
-  tmp.alloc(tmp_bytes, st);
-  PCLB_CUDA(cub::DeviceSelect::If(tmp.p, tmp_bytes, by_slot.p, compact.p, d_count.p, (int)nq, CorrHasMatch(), st));
-  c.launches += 2;
-  size_t m = 0;
-  PCLB_CUDA(cudaMemcpyAsync(&m, d_count.p, sizeof(size_t), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  if (m)
-    PCLB_CUDA(cudaMemcpyAsync(out, compact.p, m * sizeof(pclb200_corr),
-                              is_device_ptr(out) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  const size_t m = compact_corr_to(c, by_slot.p, nq, out);
   PCLB_CUDA(cudaStreamSynchronize(st));
   return m;
 }
@@ -95,32 +68,13 @@ size_t reject_surface_normal(Ctx& c, const pclb200_corr* in, size_t n, const voi
   tn.alloc(n_tgt, st);
   load_vec3_as_float4(c, src_normals, n_src, stride_sn, sn.p, st);
   load_vec3_as_float4(c, tgt_normals, n_tgt, stride_tn, tn.p, st);
-  DevBuf<pclb200_corr> d_in, marked, compact;
-  const pclb200_corr* pin = in;
-  if (!is_device_ptr(in)) {
-    d_in.alloc(n, st);
-    PCLB_CUDA(cudaMemcpyAsync(d_in.p, in, n * sizeof(pclb200_corr), cudaMemcpyHostToDevice, st));
-    pin = d_in.p;
-  }
+  DevBuf<pclb200_corr> staged, marked;
+  const pclb200_corr* pin = on_device(c, in, n, staged);
   marked.alloc(n, st);
-  compact.alloc(n, st);
-  DevBuf<size_t> d_count;
-  d_count.alloc(1, st);
   k_mark_surface_normal<<<grid_for(n, 256), 256, 0, st>>>(pin, n, sn.p, n_src, tn.p, n_tgt, threshold, marked.p);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
-  size_t tmp_bytes = 0;
-  PCLB_CUDA(cub::DeviceSelect::If(nullptr, tmp_bytes, marked.p, compact.p, d_count.p, (int)n, CorrHasMatch(), st));
-  DevBuf<unsigned char> tmp;
-  tmp.alloc(tmp_bytes, st);
-  PCLB_CUDA(cub::DeviceSelect::If(tmp.p, tmp_bytes, marked.p, compact.p, d_count.p, (int)n, CorrHasMatch(), st));
-  c.launches += 2;
-  size_t m = 0;
-  PCLB_CUDA(cudaMemcpyAsync(&m, d_count.p, sizeof(size_t), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  if (m)
-    PCLB_CUDA(cudaMemcpyAsync(out, compact.p, m * sizeof(pclb200_corr),
-                              is_device_ptr(out) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  const size_t m = compact_corr_to(c, marked.p, n, out);
   PCLB_CUDA(cudaStreamSynchronize(st));
   return m;
 }

@@ -26,8 +26,6 @@
 
 namespace pclb200 {
 
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 // Applies one rejector to the arrays.  perm / keep_sorted (nullable, n entries): for ONE_TO_ONE and TRIMMED the sorted
 // order of the input positions and which of them survive, so a caller can emit the output in the reference's order.
 // d_info (nullable, 2 doubles): [0] median distance.  trimmed_flag (nullable): 1 if TRIMMED actually cut the list.
@@ -180,13 +178,8 @@ size_t reject_standalone(Ctx& c, const pclb200_rejector& r, const pclb200_corr* 
     *median_out = 0.0;
   if (n == 0)
     return 0;
-  DevBuf<pclb200_corr> d_in, staged, d_out;
-  const pclb200_corr* din = in;
-  if (!is_device_ptr(in)) {
-    d_in.alloc(n, st);
-    PCLB_CUDA(cudaMemcpyAsync(d_in.p, in, n * sizeof(pclb200_corr), cudaMemcpyHostToDevice, st));
-    din = d_in.p;
-  }
+  DevBuf<pclb200_corr> d_in, staged;
+  const pclb200_corr* din = on_device(c, in, n, d_in);
   DevBuf<float> d2;
   DevBuf<int> match, acc, perm, keep_sorted, trimmed;
   DevBuf<unsigned> tie;
@@ -221,24 +214,11 @@ size_t reject_standalone(Ctx& c, const pclb200_rejector& r, const pclb200_corr* 
   // output order: input order for DISTANCE / MEDIAN (and an un-trimmed TRIMMED), sorted order otherwise
   const int use_perm = (r.kind == PCLB200_REJ_ONE_TO_ONE) || (r.kind == PCLB200_REJ_TRIMMED && h_trim);
   staged.alloc(n, st);
-  d_out.alloc(n, st);
   DevBuf<unsigned char> flag;
-  DevBuf<size_t> d_count;
   flag.alloc(n, st);
-  d_count.alloc(1, st);
   k_rej_flag_in_order<<<grid_for(n, 256), 256, 0, st>>>(acc.p, perm.p, keep_sorted.p, n, use_perm, din, staged.p, flag.p);
-  size_t tb = 0;
-  PCLB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, staged.p, flag.p, d_out.p, d_count.p, (int)n, st));
-  DevBuf<unsigned char> tmp;
-  tmp.alloc(tb, st);
-  PCLB_CUDA(cub::DeviceSelect::Flagged(tmp.p, tb, staged.p, flag.p, d_out.p, d_count.p, (int)n, st));
-  c.launches += 3;
-  size_t m = 0;
-  PCLB_CUDA(cudaMemcpyAsync(&m, d_count.p, sizeof(size_t), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
-  if (m)
-    PCLB_CUDA(cudaMemcpyAsync(out, d_out.p, m * sizeof(pclb200_corr),
-                              is_device_ptr(out) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+  ++c.launches;
+  const size_t m = compact_corr_to(c, staged.p, flag.p, n, out);
   PCLB_CUDA(cudaStreamSynchronize(st));
   return m;
 }

@@ -20,8 +20,6 @@
 
 namespace pclb200 {
 
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 // warp-cooperative path (defined below): returns the per-query "redo" flags of the queries it handed back, or an empty
 // buffer when it does not apply (no cell table, k outside 8..32)
 static bool warp_knn_lists(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, int32_t* d_out_idx,
@@ -165,6 +163,193 @@ void radius_csr(Ctx& c, const Index& idx, const float4* d_q, size_t nq, float r2
 {
   radius_count(c, idx, d_q, nq, r2, counts, offsets, total);
   radius_fill_sorted(c, idx, d_q, nq, r2, offsets, total, keys_sorted);
+}
+
+// ---- radius search of a caller's queries ------------------------------------------------------------------------------
+__global__ void k_unpack_keys(const unsigned long long* __restrict__ keys, size_t n, int32_t* __restrict__ idx,
+                              float* __restrict__ d2)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i < n) {
+    unsigned long long k = keys[i];
+    idx[i] = (int32_t)(unsigned)(k & 0xffffffffULL);
+    d2[i] = __uint_as_float((unsigned)(k >> 32));
+  }
+}
+
+// keep only the first max_nn entries of every (sorted) segment
+__global__ void k_truncate_segments(const unsigned long long* __restrict__ keys,
+                                    const unsigned long long* __restrict__ off_in,
+                                    const unsigned long long* __restrict__ off_out, size_t nq,
+                                    unsigned long long* __restrict__ out)
+{
+  size_t q = blockIdx.x;
+  if (q >= nq)
+    return;
+  const unsigned long long b = off_in[q], bo = off_out[q], len = off_out[q + 1] - off_out[q];
+  for (unsigned long long j = threadIdx.x; j < len; j += blockDim.x)
+    out[bo + j] = keys[b + j];
+}
+
+// max_nn <= 32 radius search = "the max_nn nearest inside the ball": k-NN rows (-1 padded) -> CSR
+__global__ void k_count_row_entries(const int32_t* __restrict__ rows, size_t nq, int k, unsigned long long* __restrict__ counts)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= nq)
+    return;
+  unsigned long long c = 0;
+  for (int j = 0; j < k; ++j)
+    if (rows[i * (size_t)k + j] >= 0)
+      ++c;
+  counts[i] = c;
+}
+
+__global__ void k_pack_rows(const int32_t* __restrict__ rows, const float* __restrict__ rows_d2, size_t nq, int k,
+                            const unsigned long long* __restrict__ offsets, int32_t* __restrict__ idx,
+                            float* __restrict__ d2)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= nq)
+    return;
+  unsigned long long o = offsets[i];
+  for (int j = 0; j < k; ++j) {
+    const int32_t v = rows[i * (size_t)k + j];
+    if (v < 0)
+      break;  // rows are filled from the front
+    idx[o] = v;
+    d2[o] = rows_d2[i * (size_t)k + j];
+    ++o;
+  }
+}
+
+__global__ void k_clamp_counts(const unsigned long long* __restrict__ in, size_t n, unsigned long long cap,
+                               unsigned long long* __restrict__ out)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i < n)
+    out[i] = in[i] < cap ? in[i] : cap;
+}
+
+__global__ void k_offsets_to_i64(const unsigned long long* __restrict__ in, size_t n, int64_t* __restrict__ out)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i < n)
+    out[i] = (int64_t)in[i];
+}
+
+void radius_search(Ctx& c, const Index& idx, const void* queries, size_t nq, size_t stride, double radius, unsigned max_nn,
+                 int64_t* out_offsets, const std::function<RadiusSinkBuffers(unsigned long long)>& sink)
+{
+  cudaStream_t st = c.stream;
+  auto write_offsets = [&](const unsigned long long* d_off) {
+    if (is_device_ptr(out_offsets)) {
+      k_offsets_to_i64<<<grid_for(nq + 1, 256), 256, 0, st>>>(d_off, nq + 1, out_offsets);
+      ++c.launches;
+    }
+    else {
+      static_assert(sizeof(unsigned long long) == sizeof(int64_t), "offset width");
+      PCLB_CUDA(cudaMemcpyAsync(out_offsets, d_off, (nq + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    }
+  };
+  const float r2 = (float)(radius * radius);  // kdtree_flann.hpp:398
+  if (max_nn == 0 || (size_t)max_nn > idx.n_valid)
+    max_nn = (unsigned)idx.n_valid;            // :382-383
+  DevBuf<float4> dense;
+  QueryBatch qb = load_queries(c, idx, queries, nq, stride, nullptr, 0, dense);
+  DevBuf<unsigned long long> counts, offsets, keys_sorted;
+  unsigned long long total = 0;
+  {
+    ProfScope ps(c, "radius_count");
+    radius_count(c, idx, qb.q.p, nq, r2, counts, offsets, total);
+  }
+  // KNNRadiusResultSet semantics (kdtree_flann.hpp:382-391): the max_nn nearest among those with d2 < r2.  Normally
+  // the whole ball is materialised, sorted and cut (the passes below: ~3 ms per million queries at ~30 neighbours).
+  // When the balls hold far more than max_nn points that would move (or overflow on) data that is thrown away, so
+  // for max_nn <= 32 the register k-NN kernel runs instead, started with the pruning bound just below r2 (every
+  // d2 < r2 is <= that bound; a candidate AT the bound still enters through the index tie rule).
+  if ((size_t)max_nn < idx.n_valid && max_nn <= 32 && total > 16ULL * (unsigned long long)nq * max_nn) {
+    const int k = (int)max_nn;
+    DevBuf<int32_t> rows;
+    DevBuf<float> rows_d2;
+    rows.alloc(nq * (size_t)k, st);
+    rows_d2.alloc(nq * (size_t)k, st);
+    {
+      ProfScope ps(c, "radius_knn");
+      launch_knn(c, idx, qb.q.p, nq, k, std::nextafter(r2, -std::numeric_limits<float>::infinity()), rows.p, rows_d2.p);
+    }
+    DevBuf<unsigned long long> cnt, off;
+    cnt.alloc(nq + 1, st);
+    off.alloc(nq + 1, st);
+    PCLB_CUDA(cudaMemsetAsync(cnt.p, 0, (nq + 1) * sizeof(unsigned long long), st));
+    k_count_row_entries<<<grid_for(nq, 256), 256, 0, st>>>(rows.p, nq, k, cnt.p);
+    size_t tb = 0;
+    PCLB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.p, off.p, (int)(nq + 1), st));
+    DevBuf<unsigned char> tmp;
+    tmp.alloc(tb, st);
+    PCLB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, cnt.p, off.p, (int)(nq + 1), st));
+    c.launches += 2;
+    unsigned long long kept = 0;
+    PCLB_CUDA(cudaMemcpyAsync(&kept, off.p + nq, sizeof(kept), cudaMemcpyDeviceToHost, st));
+    write_offsets(off.p);
+    PCLB_CUDA(cudaStreamSynchronize(st));
+    const RadiusSinkBuffers o = sink(kept);
+    if (kept > 0 && o.idx && o.d2) {
+      DevBuf<int32_t> di;
+      DevBuf<float> dd;
+      k_pack_rows<<<grid_for(nq, 256), 256, 0, st>>>(rows.p, rows_d2.p, nq, k, off.p, out_on_device(c, o.idx, kept, di),
+                                                     out_on_device(c, o.d2, kept, dd));
+      ++c.launches;
+      copy_out(c, o.idx, di, kept);
+      copy_out(c, o.d2, dd, kept);
+      PCLB_CUDA(cudaStreamSynchronize(st));
+    }
+    check_device_error(c);
+    return;
+  }
+  {
+    ProfScope ps(c, "radius");
+    radius_fill_sorted(c, idx, qb.q.p, nq, r2, offsets, total, keys_sorted);
+  }
+  const unsigned long long* d_final_keys = nullptr;
+  const unsigned long long* d_final_off = offsets.p;
+  unsigned long long final_total = total;
+  DevBuf<unsigned long long> counts2, offsets2, keys_trunc;
+  if (total > 0) {
+    d_final_keys = keys_sorted.p;
+    if ((size_t)max_nn < idx.n_valid) {  // KNNRadius semantics: the max_nn nearest inside the ball
+      counts2.alloc(nq + 1, st);
+      offsets2.alloc(nq + 1, st);
+      PCLB_CUDA(cudaMemsetAsync(counts2.p, 0, (nq + 1) * sizeof(unsigned long long), st));
+      k_clamp_counts<<<grid_for(nq, 256), 256, 0, st>>>(counts.p, nq, (unsigned long long)max_nn, counts2.p);
+      size_t tb = 0;
+      PCLB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, counts2.p, offsets2.p, (int)(nq + 1), st));
+      DevBuf<unsigned char> tmp;
+      tmp.alloc(tb, st);
+      PCLB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, counts2.p, offsets2.p, (int)(nq + 1), st));
+      PCLB_CUDA(cudaMemcpyAsync(&final_total, offsets2.p + nq, sizeof(final_total), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaStreamSynchronize(st));
+      keys_trunc.alloc(std::max<unsigned long long>(final_total, 1), st);
+      k_truncate_segments<<<(unsigned)nq, 64, 0, st>>>(keys_sorted.p, offsets.p, offsets2.p, nq, keys_trunc.p);
+      c.launches += 3;
+      d_final_keys = keys_trunc.p;
+      d_final_off = offsets2.p;
+    }
+  }
+  write_offsets(d_final_off);
+  PCLB_CUDA(cudaStreamSynchronize(st));
+  const RadiusSinkBuffers o = sink(final_total);
+  if (final_total > 0 && o.idx && o.d2) {
+    DevBuf<int32_t> di;
+    DevBuf<float> dd;
+    k_unpack_keys<<<grid_for(final_total, 256), 256, 0, st>>>(d_final_keys, final_total,
+                                                              out_on_device(c, o.idx, final_total, di),
+                                                              out_on_device(c, o.d2, final_total, dd));
+    ++c.launches;
+    copy_out(c, o.idx, di, final_total);
+    copy_out(c, o.d2, dd, final_total);
+    PCLB_CUDA(cudaStreamSynchronize(st));
+  }
+  check_device_error(c);
 }
 
 // ---- normals: eigen33 / moments (knn_warp.cuh) ------------------------------------------------------------------

@@ -19,8 +19,6 @@
 
 namespace pclb200 {
 
-static inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 struct IsSet {
   __host__ __device__ bool operator()(unsigned char v) const { return v != 0; }
 };
@@ -151,51 +149,28 @@ size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t
     return 0;
   // pass 5: centroids
   DevBuf<float4> out;
-  float4* d_out = nullptr;
-  const bool out_on_device = is_device_ptr(out_xyz1);
-  if (out_on_device)
-    d_out = reinterpret_cast<float4*>(out_xyz1);
-  else {
-    out.alloc(n_out, st);
-    d_out = out.p;
-  }
-  k_vg_centroids<<<grid_for(n_out, 128), 128, 0, st>>>(dense.p, vals.p, d_runs, n_out, d_out);
+  float4* const caller_out = reinterpret_cast<float4*>(out_xyz1);
+  k_vg_centroids<<<grid_for(n_out, 128), 128, 0, st>>>(dense.p, vals.p, d_runs, n_out, out_on_device(c, caller_out, n_out, out));
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
-  if (!out_on_device)
-    PCLB_CUDA(cudaMemcpyAsync(out_xyz1, out.p, n_out * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  copy_out(c, caller_out, out, n_out);
   if (normals && out_normal_curv) {
     // the remaining fields of a PointNormal / Normal record, averaged over the same runs in the same order
     PCLB_REQUIRE(stride_n >= 20 && stride_n % 4 == 0, PCLB200_ERR_INVALID, "normal stride must be a multiple of 4 and >= 20");
+    // the upload stops at the last byte of the last record's fields (as in strided_to_float4)
     DevBuf<unsigned char> staged;
     DevBuf<int32_t> staged_sub;
-    const unsigned char* d_src = static_cast<const unsigned char*>(normals);
-    if (!is_device_ptr(normals)) {
-      const size_t bytes = (n - 1) * stride_n + 20;
-      staged.alloc(bytes, st);
-      PCLB_CUDA(cudaMemcpyAsync(staged.p, normals, bytes, cudaMemcpyHostToDevice, st));
-      d_src = staged.p;
-    }
-    const int32_t* d_sub = indices;
-    if (indices && !is_device_ptr(indices)) {
-      staged_sub.alloc(n_idx, st);
-      PCLB_CUDA(cudaMemcpyAsync(staged_sub.p, indices, n_idx * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-      d_sub = staged_sub.p;
-    }
+    const unsigned char* d_src = on_device(c, static_cast<const unsigned char*>(normals), (n - 1) * stride_n + 20, staged);
+    const int32_t* d_sub = on_device(c, indices, n_idx, staged_sub);
     DevBuf<float4> nc, nout;
     nc.alloc(2 * cnt, st);
     k_vg_load_nc<<<grid_for(cnt, 256), 256, 0, st>>>(d_src, stride_n, d_sub, cnt, nc.p);
-    const bool nc_on_device = is_device_ptr(out_normal_curv);
-    float4* d_nout = reinterpret_cast<float4*>(out_normal_curv);
-    if (!nc_on_device) {
-      nout.alloc(2 * n_out, st);
-      d_nout = nout.p;
-    }
-    k_vg_normals<<<grid_for(n_out, 128), 128, 0, st>>>(nc.p, vals.p, d_runs, n_out, d_nout);
+    float4* const caller_nout = reinterpret_cast<float4*>(out_normal_curv);
+    k_vg_normals<<<grid_for(n_out, 128), 128, 0, st>>>(nc.p, vals.p, d_runs, n_out,
+                                                       out_on_device(c, caller_nout, 2 * n_out, nout));
     c.launches += 2;
     PCLB_CUDA(cudaGetLastError());
-    if (!nc_on_device)
-      PCLB_CUDA(cudaMemcpyAsync(out_normal_curv, nout.p, 2 * n_out * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    copy_out(c, caller_nout, nout, 2 * n_out);
     PCLB_CUDA(cudaStreamSynchronize(st));
     return n_out;
   }

@@ -60,6 +60,93 @@ def test_device_pointers_everywhere(gpu):
     a = P.icp_align(ctx, dS, di, indices=d_sub, max_iterations=5, max_correspondence_distance=0.1)
     b = P.icp_align(ctx, S, hi, indices=idx_sub, max_iterations=5, max_correspondence_distance=0.1)
     assert np.array_equal(a["final"], b["final"]) and a["n_correspondences"] == b["n_correspondences"]
+    _device_pointers_other_entry_points(P, ctx, S, T, dS, dT, hi, di, nh, nd)
+
+
+def _device_pointers_other_entry_points(P, ctx, S, T, dS, dT, hi, di, nh, nd):
+    """The rest of the C-ABI with CUDA tensors for inputs and outputs.  Where the Python wrapper hands back NumPy
+    arrays the C function is called directly with the tensors' pointers."""
+    import ctypes as C
+    import torch
+    L = P.lib()
+    ptr = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    n = S.shape[0]
+
+    def dev_corr(c):
+        return torch.from_numpy(np.ascontiguousarray(c).view(np.uint8).copy()).cuda()
+
+    def corr_out(cap):
+        return torch.empty(max(cap, 1) * P.CORR_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+
+    def host_corr(t, m):
+        return t.cpu().numpy().view(P.CORR_DTYPE)[:m]
+
+    hm, hk = hi.knn_stats(T, 8)
+    dm, dk = torch.empty(n, device="cuda"), torch.empty(n, device="cuda")
+    P._check(L.pclb200_knn_stats(ctx.h, di.h, ptr(dT), n, 16, None, 0, 8, ptr(dm), ptr(dk)))
+    assert np.array_equal(dm.cpu().numpy(), hm) and np.array_equal(dk.cpu().numpy(), hk)
+    nr = torch.empty((n, 4), dtype=torch.float32, device="cuda")
+    di.normals_radius(dT, 0.05, viewpoint=(0.5, 0.5, 3.0), out=nr)
+    assert np.array_equal(nr.cpu().numpy(), hi.normals_radius(T, 0.05, viewpoint=(0.5, 0.5, 3.0))[0], equal_nan=True)
+    lab = torch.empty(n, dtype=torch.int32, device="cuda")
+    di.cluster_labels(0.01, out=lab)
+    assert np.array_equal(lab.cpu().numpy(), hi.cluster_labels(0.01))
+    cov = torch.empty((n, 9), dtype=torch.float64, device="cuda")
+    P._check(L.pclb200_gicp_covariances(ctx.h, di.h, ptr(dT), n, 16, 10, C.c_double(0.001), ptr(cov)))
+    assert np.array_equal(cov.cpu().numpy().reshape(-1, 3, 3), hi.gicp_covariances(T, k=10))
+
+    m = C.c_size_t()
+    for kind in (P.CORR_NORMAL_SHOOTING, P.CORR_BACK_PROJECTION):
+        want = hi.correspondences_normals(kind, S, nh, nh, k=10, max_distance=0.05)
+        out = corr_out(n)
+        P._check(L.pclb200_correspondences_normals(ctx.h, di.h, kind, ptr(dS), n, 16, ptr(nd), 16, ptr(nd), 16, None, 0,
+                                                   10, C.c_double(0.05), ptr(out), C.byref(m)))
+        assert want.size > 0 and np.array_equal(host_corr(out, m.value), want)
+
+    corr = hi.correspondences(S, max_distance=0.05)
+    dcorr = dev_corr(corr)
+    for kind, p in ((P.REJ_DISTANCE, 0.02), (P.REJ_MEDIAN, 1.0), (P.REJ_ONE_TO_ONE, 0.0), (P.REJ_TRIMMED, 0.7)):
+        want, want_med = ctx.reject(corr, kind, p)
+        out, med = corr_out(corr.size), C.c_double()
+        r = P.Rejector(kind, 0, float(p))
+        P._check(L.pclb200_reject(ctx.h, C.byref(r), ptr(dcorr), corr.size, ptr(out), C.byref(m), C.byref(med)))
+        assert np.array_equal(host_corr(out, m.value), want) and med.value == want_med
+    want = ctx.reject_surface_normal(corr, nh, nh, 0.5)
+    out = corr_out(corr.size)
+    P._check(L.pclb200_reject_surface_normal(ctx.h, ptr(dcorr), corr.size, ptr(nd), n, 16, ptr(nd), n, 16,
+                                             C.c_double(0.5), ptr(out), C.byref(m)))
+    assert np.array_equal(host_corr(out, m.value), want)
+    Tw = ctx.estimate_svd(S, T, corr=corr)
+    Td = np.zeros(16)
+    P._check(L.pclb200_estimate_svd(ctx.h, ptr(dS), 16, ptr(dT), 16, ptr(dcorr), corr.size, 0,
+                                    Td.ctypes.data_as(C.POINTER(C.c_double))))
+    assert np.array_equal(Td.reshape(4, 4), Tw)
+
+    hs, ds = P.Icp(ctx, max_iterations=5, max_correspondence_distance=0.1), P.Icp(ctx, max_iterations=5,
+                                                                                  max_correspondence_distance=0.1)
+    hs.set_target(hi)
+    hs.set_source(S)
+    ds.set_target(di)
+    ds.set_source(dS)
+    hs.iterate()
+    ds.iterate()
+    want = hs.get_correspondences()
+    out = corr_out(n)
+    P._check(L.pclb200_icp_get_correspondences(ds.h, ptr(out), C.byref(m)))
+    assert want.size > 0 and np.array_equal(host_corr(out, m.value), want)
+
+    # pcl::PointNormal records (48 bytes): xyz1, normal, curvature
+    PN = np.concatenate([T, nh, np.zeros((n, 4), np.float32)], axis=1)
+    dPN = torch.from_numpy(PN).cuda()
+    sub = np.arange(0, n, 2, dtype=np.int32)
+    dsub = torch.from_numpy(sub).cuda()
+    wx, wn = ctx.voxelgrid_normals(PN, 0.05, indices=sub)
+    ox, on = torch.empty((sub.size, 4), device="cuda"), torch.empty((sub.size, 8), device="cuda")
+    leaf = (C.c_float * 3)(0.05, 0.05, 0.05)
+    P._check(L.pclb200_voxelgrid_normals(ctx.h, ptr(dPN), n, 48, C.c_void_p(dPN.data_ptr() + 16), 48, ptr(dsub),
+                                         sub.size, 1, leaf, 0, ptr(ox), ptr(on), C.byref(m)))
+    assert m.value == wx.shape[0] > 0
+    assert np.array_equal(ox.cpu().numpy()[:m.value], wx) and np.array_equal(on.cpu().numpy()[:m.value], wn, equal_nan=True)
 
 
 def test_error_statuses(gpu):
