@@ -28,7 +28,7 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
                     const void* src_normals = nullptr, int enforce_same_dir = 1, int svd_correlation = 0);
 size_t correspondences(Ctx& c, const Index& tgt, const Index* src_index, const void* src, size_t n, size_t stride,
                        const int32_t* indices, size_t n_idx, int is_dense, double max_dist, pclb200_corr* out,
-                       const double* pre_T = nullptr, int pre_mode = 0, const float* gate_override = nullptr);
+                       const double* pre_T = nullptr, int pre_mode = kApplyIcp, const float* gate_override = nullptr);
 double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t stride, const int32_t* indices,
                      size_t n_idx, const double* T, int scalar_is_double, double max_range, int mode_override = -1);
 void gicp_covariances(Ctx& c, Index& idx, const void* pts, size_t n, size_t stride, int k, double gicp_epsilon,
@@ -701,7 +701,7 @@ int pclb200_validate_transformation(pclb200_ctx* ctx, const pclb200_index* idx_t
     PCLB_REQUIRE(idx_tgt && idx_tgt->idx && T && score, PCLB200_ERR_INVALID, "NULL argument");
     // transformation_validation_euclidean.hpp:62-75: T(0,0)*x + T(0,1)*y + T(0,2)*z + T(0,3) in Scalar, cast to float
     *score = fitness_score(c, *idx_tgt->idx, src, n, stride, nullptr, 0, T, scalar_is_double, max_range,
-                           scalar_is_double ? 3 : 0);
+                           scalar_is_double ? kApplyValidationDouble : kApplyIcp);
   });
 }
 
@@ -713,10 +713,8 @@ int pclb200_inliers(pclb200_ctx* ctx, const pclb200_index* idx_tgt, const void* 
     // sample_consensus_prerejective.hpp:318-338: transformPointCloud (float), then nn_dists[0] < max_range (STRICT, float)
     const float max_range = inlier_threshold * inlier_threshold;
     const float gate = std::nextafter(max_range, -std::numeric_limits<float>::infinity());  // d2 <= gate  <=>  d2 < max_range
-    double Tf[16];
-    for (int i = 0; i < 16; ++i)
-      Tf[i] = (double)(float)T[i];
-    *n_out = max_range > 0.f ? correspondences(c, *idx_tgt->idx, nullptr, src, n, stride, nullptr, 0, 1, 0.0, out, Tf, 1, &gate)
+    *n_out = max_range > 0.f ? correspondences(c, *idx_tgt->idx, nullptr, src, n, stride, nullptr, 0, 1, 0.0, out, T,
+                                               kApplyTransformsFloat, &gate)
                              : 0;
   });
 }

@@ -50,7 +50,7 @@ __global__ void k_apply_pending(float4* __restrict__ pts, size_t n, const Pendin
     pts[i] = p;
     if (normals) {
       float4 m = normals[i];
-      if (P.mode == 0 && !(isfinite(m.x) && isfinite(m.y) && isfinite(m.z)))
+      if (P.mode == kApplyIcp && !(isfinite(m.x) && isfinite(m.y) && isfinite(m.z)))
         continue;  // icp.hpp:97-98
       apply_pending_normal(P, m.x, m.y, m.z);
       normals[i] = m;
@@ -145,7 +145,7 @@ float gate_from_max_dist(double max_dist)
   return g;
 }
 
-struct Reducer {  // scratch for block_reduce_and_publish
+struct Reducer {  // scratch of the grid sums (grid_fold)
   DevBuf<double> partials;
   DevBuf<double> partials2;  // max_blocks * 128 (k_accum_dmma)
   DevBuf<unsigned> counter;
@@ -161,6 +161,7 @@ struct Reducer {  // scratch for block_reduce_and_publish
     PCLB_CUDA(cudaMemsetAsync(counter.p, 0, sizeof(unsigned), c.stream));
     PCLB_CUDA(cudaMemsetAsync(accum.p, 0, kAccum * sizeof(double), c.stream));
   }
+  GridSum sum() const { return GridSum{partials.p, counter.p, accum.p}; }
 };
 
 static unsigned persistent_grid(const Ctx& c, size_t n, int block, int per_sm)
@@ -215,11 +216,12 @@ static void set_identity(double* T)
 static int transform_mode(const pclb200_icp_params& P)
 {
   if (!P.with_normals_transform)
-    return 0;
-  return P.scalar_is_double ? 2 : 1;
+    return kApplyIcp;
+  return P.scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat;
 }
 
-static void upload_pending(Icp& s, const double* T, int apply)
+// rows 0..2 of the row-major 4x4 T, applied in the operation order `mode` (kApply*)
+static Pending make_pending(const double* T, int mode, int apply)
 {
   Pending h;
   for (int i = 0; i < 12; ++i) {
@@ -227,9 +229,22 @@ static void upload_pending(Icp& s, const double* T, int apply)
     h.d[i] = T[i];
   }
   h.apply = apply;
-  h.mode = transform_mode(s.P);
-  PCLB_CUDA(cudaMemcpyAsync(s.pending.p, &h, sizeof(h), cudaMemcpyHostToDevice, s.ctx->stream));
-  PCLB_CUDA(cudaStreamSynchronize(s.ctx->stream));  // h is a stack object
+  h.mode = mode;
+  return h;
+}
+
+static void upload_pending(Ctx& c, Pending* d, const Pending& h)
+{
+  PCLB_CUDA(cudaMemcpyAsync(d, &h, sizeof(h), cudaMemcpyHostToDevice, c.stream));
+  PCLB_CUDA(cudaStreamSynchronize(c.stream));  // h is a stack object
+}
+
+// pts[0..n) (and their normals, when given) transformed in place by T in the operation order `mode`; d: device scratch
+static void transform_on_device(Ctx& c, Pending* d, const double* T, int mode, float4* pts, size_t n, float4* normals)
+{
+  upload_pending(c, d, make_pending(T, mode, 1));
+  k_apply_pending<<<persistent_grid(c, n, 256, 8), 256, 0, c.stream>>>(pts, n, d, normals);
+  ++c.launches;
 }
 
 void icp_reset_state(Icp& s, const double* guess)
@@ -260,7 +275,7 @@ Icp* icp_create(Ctx& c, const pclb200_icp_params& P)
   s->skip_count.alloc(1, c.stream);
   s->red.init(c, (unsigned)c.sm_count * 16);
   icp_reset_state(*s, nullptr);
-  upload_pending(*s, s->loop.final_T, 0);
+  upload_pending(c, s->pending.p, make_pending(s->loop.final_T, transform_mode(P), 0));
   return s.release();
 }
 
@@ -511,12 +526,9 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
     for (int i = 0; i < 16; ++i)
       if (s.loop.final_T[i] != ((i % 5 == 0) ? 1.0 : 0.0))
         guess_identity = false;
-  if (!guess_identity) {
-    upload_pending(s, s.loop.final_T, 1);
-    k_apply_pending<<<persistent_grid(c, s.n_q, 256, 8), 256, 0, st>>>(s.cur.p, s.n_q, s.pending.p, s.cur_normals.p);
-    ++c.launches;
-  }
-  upload_pending(s, s.loop.last_T, 0);
+  if (!guess_identity)
+    transform_on_device(c, s.pending.p, s.loop.final_T, transform_mode(s.P), s.cur.p, s.n_q, s.cur_normals.p);
+  upload_pending(c, s.pending.p, make_pending(s.loop.last_T, transform_mode(s.P), 0));
   PCLB_CUDA(cudaGetLastError());
 }
 
@@ -793,19 +805,10 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
   }
   DevBuf<Pending> pend;
   pend.alloc(1, st);
-  Pending h;
-  for (int i = 0; i < 12; ++i) {
-    h.f[i] = (float)s.loop.final_T[i];
-    h.d[i] = s.loop.final_T[i];
-  }
-  h.apply = 1;
-  h.mode = transform_mode(s.P);
-  PCLB_CUDA(cudaMemcpyAsync(pend.p, &h, sizeof(h), cudaMemcpyHostToDevice, st));
   {
     ProfScope ps(c, "transform_out");
-    k_apply_pending<<<persistent_grid(c, s.n_all, 256, 8), 256, 0, st>>>(tmp.p, s.n_all, pend.p, do_n ? tmpn.p : nullptr);
+    transform_on_device(c, pend.p, s.loop.final_T, transform_mode(s.P), tmp.p, s.n_all, do_n ? tmpn.p : nullptr);
   }
-  ++c.launches;
   const bool normals_inside =
       do_n && s.src_normal_off >= 0 &&
       static_cast<unsigned char*>(out_normals) - static_cast<unsigned char*>(out_pts) == s.src_normal_off && stride_n == stride_out;
@@ -914,9 +917,7 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
   a.corr = d_corr;
   a.n = n;
   a.ox = a.oy = a.oz = 0.f;
-  a.pub.partials = red.partials.p;
-  a.pub.counter = red.counter.p;
-  a.pub.accum = red.accum.p;
+  a.pub = red.sum();
   if (est == PCLB200_EST_SVD) {
     // shift by the first target point to keep the fp64 sums small
     float4 first;
@@ -931,8 +932,8 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
     k_accum_pairs<PCLB200_EST_POINT_TO_PLANE_LLS><<<grid, 256, 0, st>>>(a);
   else
     k_accum_pairs<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS><<<grid, 256, 0, st>>>(a);
-  k_solve<<<1, 32, 0, st>>>(red.accum.p, est, scalar_is_double, 0, (double)a.ox, (double)a.oy, (double)a.oz, 1, nullptr,
-                            so.p, svd_correlation, nullptr, CritParams{});
+  k_solve<<<1, 32, 0, st>>>(red.accum.p, est, scalar_is_double, kApplyIcp, (double)a.ox, (double)a.oy, (double)a.oz, 1,
+                            nullptr, so.p, svd_correlation, nullptr, CritParams{});
   c.launches += 2;
   SolveOut h;
   PCLB_CUDA(cudaMemcpyAsync(&h, so.p, sizeof(h), cudaMemcpyDeviceToHost, st));
@@ -957,17 +958,7 @@ size_t correspondences(Ctx& c, const Index& tgt, const Index* src_index, const v
   DevBuf<Pending> pend;
   if (pre_T) {  // the caller's cloud is searched after a rigid transform (consumers that validate a pose)
     pend.alloc(1, st);
-    Pending h;
-    for (int i = 0; i < 12; ++i) {
-      h.f[i] = (float)pre_T[i];
-      h.d[i] = pre_T[i];
-    }
-    h.apply = 1;
-    h.mode = pre_mode;
-    PCLB_CUDA(cudaMemcpyAsync(pend.p, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-    PCLB_CUDA(cudaStreamSynchronize(st));  // h is a stack object
-    k_apply_pending<<<persistent_grid(c, nq, 256, 8), 256, 0, st>>>(dense.p, nq, pend.p, nullptr);
-    ++c.launches;
+    transform_on_device(c, pend.p, pre_T, pre_mode, dense.p, nq, nullptr);
   }
   DevBuf<int32_t> staged_ind;
   const int32_t* d_ind = on_device(c, indices, n_idx, staged_ind);
@@ -1005,28 +996,15 @@ double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t
   load_xyz_as_float4(c, src, n, stride, use_sub ? indices : nullptr, use_sub ? n_idx : 0, dense.p, st);
   DevBuf<Pending> pend;
   pend.alloc(1, st);
-  Pending h;
-  for (int i = 0; i < 12; ++i) {
-    h.f[i] = (float)T[i];
-    h.d[i] = scalar_is_double ? T[i] : (double)(float)T[i];
-  }
-  h.apply = 1;
-  h.mode = mode_override >= 0 ? mode_override : (scalar_is_double ? 2 : 1);  // default: pcl::transformPointCloud
-  PCLB_CUDA(cudaMemcpyAsync(pend.p, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-  k_apply_pending<<<persistent_grid(c, nq, 256, 8), 256, 0, st>>>(dense.p, nq, pend.p, nullptr);
-  ++c.launches;
+  // default: pcl::transformPointCloud
+  const int mode = mode_override >= 0 ? mode_override : (scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat);
+  transform_on_device(c, pend.p, T, mode, dense.p, nq, nullptr);
   QueryBatch qb;
   make_query_batch(c, tgt, dense.p, nq, qb);
   Reducer red;
   const unsigned grid = persistent_grid(c, nq, 256, 8);
   red.init(c, grid);
-  IterArgs pub;
-  memset(&pub, 0, sizeof(pub));
-  pub.partials = red.partials.p;
-  pub.counter = red.counter.p;
-  pub.accum = red.accum.p;
-  pub.d_error = c.d_error;
-  k_fitness<<<grid, 256, 0, st>>>(tree_view(tgt), qb.q.p, nq, max_range, pub);
+  k_fitness<<<grid, 256, 0, st>>>(tree_view(tgt), qb.q.p, nq, max_range, red.sum(), c.d_error);
   ++c.launches;
   double acc[2];
   PCLB_CUDA(cudaMemcpyAsync(acc, red.accum.p, sizeof(acc), cudaMemcpyDeviceToHost, st));

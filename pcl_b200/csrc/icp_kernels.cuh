@@ -1,5 +1,6 @@
 // icp_kernels.cuh — the device side of one ICP iteration: the loop state, the search kernel (k_search), the normal
-// equations on the fp64 tensor cores (k_accum_dmma) and per-thread (k_accum, k_accum_pairs), the single-thread solve with
+// equations on the fp64 tensor cores (k_accum_dmma) and per-thread (k_accum, k_accum_pairs: add_pair_terms),
+// one fixed-order grid sum for all of them (grid_fold), the single-thread solve with
 // the convergence criteria in its tail (k_solve).  A header so that icp.cu stays the host-side driver and so that
 // tests/host/icp_host_test.cpp can compile the SAME source for the host (a lock-step emulation of a thread block) and run
 // whole iterations against the oracle's arithmetic.
@@ -23,8 +24,7 @@ struct Pending {
   float f[12];   // rows 0..2 of T_k, already rounded like the reference (cast<float>)
   double d[12];  // same rows in double (Transformer<double> path)
   int apply;     // 0 = identity / nothing to apply
-  int mode;      // 0: icp.hpp:49-111 order, 1: transforms.hpp SSE float order, 2: transforms.hpp double order,
-                 // 3: transformation_validation_euclidean.hpp:62-75 with a double matrix (left-to-right, cast at the end)
+  int mode;      // kApply* (internal.cuh): the reference's operation order
 };
 
 struct SolveOut {
@@ -61,23 +61,23 @@ struct CritParams {  // what DefaultConvergenceCriteria and the tracking heurist
 __device__ __forceinline__ void apply_pending(const Pending& P, float& x, float& y, float& z)
 {
   const float px = x, py = y, pz = z;
-  if (P.mode == 0) {
+  if (P.mode == kApplyIcp) {
     x = ((P.f[0] * px + P.f[1] * py) + P.f[2] * pz) + P.f[3];
     y = ((P.f[4] * px + P.f[5] * py) + P.f[6] * pz) + P.f[7];
     z = ((P.f[8] * px + P.f[9] * py) + P.f[10] * pz) + P.f[11];
   }
-  else if (P.mode == 1) {
+  else if (P.mode == kApplyTransformsFloat) {
     x = P.f[0] * px + (P.f[1] * py + (P.f[2] * pz + P.f[3]));
     y = P.f[4] * px + (P.f[5] * py + (P.f[6] * pz + P.f[7]));
     z = P.f[8] * px + (P.f[9] * py + (P.f[10] * pz + P.f[11]));
   }
-  else if (P.mode == 3) {
+  else if (P.mode == kApplyValidationDouble) {
     const double dx = px, dy = py, dz = pz;
     x = (float)(((P.d[0] * dx + P.d[1] * dy) + P.d[2] * dz) + P.d[3]);
     y = (float)(((P.d[4] * dx + P.d[5] * dy) + P.d[6] * dz) + P.d[7]);
     z = (float)(((P.d[8] * dx + P.d[9] * dy) + P.d[10] * dz) + P.d[11]);
   }
-  else {
+  else {  // kApplyTransformsDouble
     const double dx = px, dy = py, dz = pz;
     x = (float)(((P.d[3] + dx * P.d[0]) + dy * P.d[1]) + dz * P.d[2]);
     y = (float)(((P.d[7] + dx * P.d[4]) + dy * P.d[5]) + dz * P.d[6]);
@@ -88,17 +88,17 @@ __device__ __forceinline__ void apply_pending(const Pending& P, float& x, float&
 __device__ __forceinline__ void apply_pending_normal(const Pending& P, float& x, float& y, float& z)
 {
   const float px = x, py = y, pz = z;
-  if (P.mode == 0) {
+  if (P.mode == kApplyIcp) {
     x = (P.f[0] * px + P.f[1] * py) + P.f[2] * pz;
     y = (P.f[4] * px + P.f[5] * py) + P.f[6] * pz;
     z = (P.f[8] * px + P.f[9] * py) + P.f[10] * pz;
   }
-  else if (P.mode == 1) {
+  else if (P.mode == kApplyTransformsFloat) {
     x = P.f[0] * px + (P.f[1] * py + P.f[2] * pz);
     y = P.f[4] * px + (P.f[5] * py + P.f[6] * pz);
     z = P.f[8] * px + (P.f[9] * py + P.f[10] * pz);
   }
-  else {
+  else {  // the double orders
     const double dx = px, dy = py, dz = pz;
     x = (float)((dx * P.d[0] + dy * P.d[1]) + dz * P.d[2]);
     y = (float)((dx * P.d[4] + dy * P.d[5]) + dz * P.d[6]);
@@ -144,8 +144,54 @@ __device__ __forceinline__ void peer_exchange(const IterArgs& a)
   peer_exchange(a.peer, a.seq, a.accum, a.accum, kAccum, 0.0, [](double s, double x) { return s + x; }, a.d_error);
 }
 
+// scratch of a grid sum (grid_fold): per-block partials, the ticket counter (zero between launches), the totals
+struct GridSum {
+  double* partials;
+  unsigned* counter;
+  double* accum;
+};
+
+// The fixed-order grid sum of WIDTH slots.  rows[w * WIDTH + t]: the sums of slot t over the pairs of warp w of this
+// block, w < nwarps, in shared memory.  Thread t < WIDTH adds them up over the warps into partials[block * STRIDE + t];
+// the LAST block to take a ticket adds those up over the blocks, in block order (bitwise reproducible), into out[t] and
+// returns true, and the caller's last block then publishes the totals and resets the counter.  Must be called by every
+// thread of every block.  is_last: a __shared__ flag declared by the caller, so that it keeps its place in the caller's
+// shared memory.  The pointers are taken by reference, so that a kernel reads them from its parameters where they are
+// used.
+template <int WIDTH, int STRIDE>
+__device__ __forceinline__ bool grid_fold(const double* rows, int nwarps, double* const& partials,
+                                          unsigned* const& counter, bool& is_last, double* out)
+{
+  if (threadIdx.x < WIDTH) {
+    double v = 0.0;
+    for (int w = 0; w < nwarps; ++w)
+      v += rows[w * WIDTH + threadIdx.x];
+    partials[(size_t)blockIdx.x * STRIDE + threadIdx.x] = v;
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned tk = atomicAdd(counter, 1u);
+    is_last = (tk == gridDim.x - 1);
+  }
+  __syncthreads();
+  const bool last = is_last;
+  if (last) {
+    __threadfence();
+    if (threadIdx.x < WIDTH) {
+      double v = 0.0;
+      for (unsigned b = 0; b < gridDim.x; ++b)
+        v += __ldcg(&partials[(size_t)b * STRIDE + threadIdx.x]);
+      out[threadIdx.x] = v;
+    }
+  }
+  return last;
+}
+
+// per-thread accumulators acc[0..NACC) -> block (fixed order) -> grid (grid_fold) -> g.accum[0..kAccum), zero beyond
+// NACC.  Returns true in the last block.
 template <int NACC>
-__device__ __forceinline__ void block_reduce_and_publish(double* acc, const IterArgs& a)
+__device__ __forceinline__ bool block_reduce_and_publish(const double* acc, const GridSum& g)
 {
   __shared__ double sm[8][NACC];
   __shared__ bool is_last;
@@ -160,33 +206,13 @@ __device__ __forceinline__ void block_reduce_and_publish(double* acc, const Iter
       sm[warp][t] = v;
   }
   __syncthreads();
-  if (threadIdx.x < NACC) {
-    double v = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w)
-      v += sm[w][threadIdx.x];
-    a.partials[(size_t)blockIdx.x * kAccum + threadIdx.x] = v;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned t = atomicAdd(a.counter, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    if (threadIdx.x < NACC) {
-      double v = 0.0;
-      for (unsigned b = 0; b < gridDim.x; ++b)  // fixed order => bitwise reproducible
-        v += __ldcg(&a.partials[(size_t)b * kAccum + threadIdx.x]);
-      a.accum[threadIdx.x] = v;
-    }
-    if (threadIdx.x >= NACC && threadIdx.x < kAccum)
-      a.accum[threadIdx.x] = 0.0;
-    if (threadIdx.x == 0)
-      *a.counter = 0;
-    peer_exchange(a);
-  }
+  if (!grid_fold<NACC, kAccum>(&sm[0][0], blockDim.x >> 5, g.partials, g.counter, is_last, g.accum))
+    return false;
+  if (threadIdx.x >= NACC && threadIdx.x < kAccum)
+    g.accum[threadIdx.x] = 0.0;
+  if (threadIdx.x == 0)
+    *g.counter = 0;
+  return true;
 }
 
 // match of one query, in the (Hilbert) slot order of `cur`: this iteration's result and the next iteration's seed
@@ -368,36 +394,16 @@ __device__ __forceinline__ void fold_tiles_and_publish(const IterArgs& a, double
       s_tiles[warp][64 + g * 8] = v;
   }
   __syncthreads();
-  if (threadIdx.x < 128) {
-    double vsum = 0.0;
-    for (int w = 0; w < NWARPS; ++w)
-      vsum += s_tiles[w][threadIdx.x];
-    a.partials2[(size_t)blockIdx.x * 128 + threadIdx.x] = vsum;
-  }
-  __threadfence();
+  if (!grid_fold<128, 128>(&s_tiles[0][0], NWARPS, a.partials2, a.counter, is_last, s_fin))
+    return;
   __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned tk = atomicAdd(a.counter, 1u);
-    is_last = (tk == gridDim.x - 1);
+  if (threadIdx.x < kAccum) {
+    const int src = dmma_accum_source(EST, threadIdx.x);
+    a.accum[threadIdx.x] = src >= 0 ? s_fin[src] : 0.0;
   }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    if (threadIdx.x < 128) {
-      double vsum = 0.0;
-      for (unsigned b = 0; b < gridDim.x; ++b)  // fixed order => bitwise reproducible
-        vsum += __ldcg(&a.partials2[(size_t)b * 128 + threadIdx.x]);
-      s_fin[threadIdx.x] = vsum;
-    }
-    __syncthreads();
-    if (threadIdx.x < kAccum) {
-      const int src = dmma_accum_source(EST, threadIdx.x);
-      a.accum[threadIdx.x] = src >= 0 ? s_fin[src] : 0.0;
-    }
-    if (threadIdx.x == 0)
-      *a.counter = 0;
-    peer_exchange(a);
-  }
+  if (threadIdx.x == 0)
+    *a.counter = 0;
+  peer_exchange(a);
 }
 
 // Search kernel, one query per thread: apply the pending T_k in place (reference fp32 operation order, icp.hpp:49-111)
@@ -562,17 +568,79 @@ k_accum_dmma(const IterArgs a, const Match* __restrict__ match)
   fold_tiles_and_publish<EST, 8>(a, ca + da, cb + db, w);
 }
 
-// Accumulation kernel: one streaming pass over (source point, match) pairs; fp64 sums, fixed reduction order.
+// One pair's terms of the normal equations (slot layout at the top of this file), added to acc[2..): p source point, q
+// target point, o the accumulation origin (SVD), nq the target normal (LLS), np the source normal and enforce_same_dir
+// (symmetric objective).  A pair whose normal is not finite adds nothing here: the estimator skips it, but it is still a
+// correspondence, so the callers count it in acc[0..1] first.
+template <int EST>
+__device__ __forceinline__ void add_pair_terms(double* acc, const float4& p, const float4& q, const float3& o,
+                                               const float4& nq, const float4& np, int enforce_same_dir)
+{
+  if (EST == PCLB200_EST_SVD) {
+    const double px = (double)p.x - (double)o.x, py = (double)p.y - (double)o.y, pz = (double)p.z - (double)o.z;
+    const double qx = (double)q.x - (double)o.x, qy = (double)q.y - (double)o.y, qz = (double)q.z - (double)o.z;
+    acc[2] += px; acc[3] += py; acc[4] += pz;
+    acc[5] += qx; acc[6] += qy; acc[7] += qz;
+    acc[8] += qx * px; acc[9] += qx * py; acc[10] += qx * pz;
+    acc[11] += qy * px; acc[12] += qy * py; acc[13] += qy * pz;
+    acc[14] += qz * px; acc[15] += qz * py; acc[16] += qz * pz;
+  }
+  else if (EST == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS) {
+    // symmetric_point_to_plane_lls.hpp:166-193: n = n1 +/- n2, v = [(p+q) x n, n], A^T A += v v^T, A^T b += v ((q-p).n)
+    const float4 &n1 = np, &n2 = nq;
+    const double d12 = (double)n1.x * n2.x + (double)n1.y * n2.y + (double)n1.z * n2.z;
+    const double sg = (!enforce_same_dir || d12 >= 0.0) ? 1.0 : -1.0;
+    const double nx = (double)n1.x + sg * n2.x, ny = (double)n1.y + sg * n2.y, nz = (double)n1.z + sg * n2.z;
+    if (!(isfinite(nx) && isfinite(ny) && isfinite(nz)))
+      return;
+    const double sx = (double)p.x + q.x, sy = (double)p.y + q.y, sz = (double)p.z + q.z;
+    const double v[6] = {sy * nz - sz * ny, sz * nx - sx * nz, sx * ny - sy * nx, nx, ny, nz};
+    const double b = ((double)q.x - p.x) * nx + ((double)q.y - p.y) * ny + ((double)q.z - p.z) * nz;
+    int t = 2;
+#pragma unroll
+    for (int r = 0; r < 6; ++r)
+#pragma unroll
+      for (int cc = r; cc < 6; ++cc)
+        acc[t++] += v[r] * v[cc];
+#pragma unroll
+    for (int r = 0; r < 6; ++r)
+      acc[23 + r] += v[r] * b;
+  }
+  else {
+    if (!(isfinite(nq.x) && isfinite(nq.y) && isfinite(nq.z)))
+      return;  // point_to_plane_lls.hpp:182-190
+    const float sx = p.x, sy = p.y, sz = p.z, dx = q.x, dy = q.y, dz = q.z, nx = nq.x, ny = nq.y, nz = nq.z;
+    // float expressions widened to double, exactly as :202-204 and :235 (no fma: -fmad=false)
+    const double A = (double)(nz * sy - ny * sz);
+    const double B = (double)(nx * sz - nz * sx);
+    const double C = (double)(ny * sx - nx * sy);
+    const double D = (double)(nx * dx + ny * dy + nz * dz - nx * sx - ny * sy - nz * sz);
+    acc[2] += A * A; acc[3] += A * B; acc[4] += A * C;
+    acc[5] += A * (double)nx; acc[6] += A * (double)ny; acc[7] += A * (double)nz;
+    acc[8] += B * B; acc[9] += B * C;
+    acc[10] += B * (double)nx; acc[11] += B * (double)ny; acc[12] += B * (double)nz;
+    acc[13] += C * C;
+    acc[14] += C * (double)nx; acc[15] += C * (double)ny; acc[16] += C * (double)nz;
+    acc[17] += (double)(nx * nx); acc[18] += (double)(nx * ny); acc[19] += (double)(nx * nz);
+    acc[20] += (double)(ny * ny); acc[21] += (double)(ny * nz);
+    acc[22] += (double)(nz * nz);
+    acc[23] += A * D; acc[24] += B * D; acc[25] += C * D;
+    acc[26] += (double)nx * D; acc[27] += (double)ny * D; acc[28] += (double)nz * D;
+  }
+}
+
+// The symmetric objective inside the loop (the other estimators run on k_accum_dmma): one streaming pass over (source
+// point, match) pairs, per-thread fp64 sums, fixed reduction order.
 template <int EST>
 __global__ void __launch_bounds__(256)
 k_accum(const IterArgs a, const Match* __restrict__ match)
 {
+  static_assert(EST == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS, "the other estimators accumulate in k_accum_dmma");
   if (a.ctrl && a.ctrl->done)
     return;
-  constexpr int NACC = EST == PCLB200_EST_SVD ? kAccSvd : kAccLls;
-  double acc[NACC];
+  double acc[kAccLls];
 #pragma unroll
-  for (int t = 0; t < NACC; ++t)
+  for (int t = 0; t < kAccLls; ++t)
     acc[t] = 0.0;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < a.n; i += (size_t)gridDim.x * blockDim.x) {
     const Match m = match[i];
@@ -582,61 +650,12 @@ k_accum(const IterArgs a, const Match* __restrict__ match)
     const float4 q = ldg4(a.pts + m.pos);
     acc[0] += 1.0;
     acc[1] += (double)m.d2;
-    if (EST == PCLB200_EST_SVD) {
-      const double px = (double)p.x - (double)a.ox, py = (double)p.y - (double)a.oy, pz = (double)p.z - (double)a.oz;
-      const double qx = (double)q.x - (double)a.ox, qy = (double)q.y - (double)a.oy, qz = (double)q.z - (double)a.oz;
-      acc[2] += px; acc[3] += py; acc[4] += pz;
-      acc[5] += qx; acc[6] += qy; acc[7] += qz;
-      acc[8] += qx * px; acc[9] += qx * py; acc[10] += qx * pz;
-      acc[11] += qy * px; acc[12] += qy * py; acc[13] += qy * pz;
-      acc[14] += qz * px; acc[15] += qz * py; acc[16] += qz * pz;
-    }
-    else if (EST == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS) {
-      // symmetric_point_to_plane_lls.hpp:166-193: n = n1 +/- n2, v = [(p+q) x n, n], A^T A += v v^T, A^T b += v ((q-p).n)
-      const float4 n2 = ldg4(a.tgt_normals + m.pos);
-      const float4 n1 = a.cur_normals[i];
-      const double d12 = (double)n1.x * n2.x + (double)n1.y * n2.y + (double)n1.z * n2.z;
-      const double sg = (!a.enforce_same_dir || d12 >= 0.0) ? 1.0 : -1.0;
-      const double nx = (double)n1.x + sg * n2.x, ny = (double)n1.y + sg * n2.y, nz = (double)n1.z + sg * n2.z;
-      if (!(isfinite(nx) && isfinite(ny) && isfinite(nz)))
-        continue;
-      const double sx = (double)p.x + q.x, sy = (double)p.y + q.y, sz = (double)p.z + q.z;
-      const double v[6] = {sy * nz - sz * ny, sz * nx - sx * nz, sx * ny - sy * nx, nx, ny, nz};
-      const double b = ((double)q.x - p.x) * nx + ((double)q.y - p.y) * ny + ((double)q.z - p.z) * nz;
-      int t = 2;
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
-#pragma unroll
-        for (int cc = r; cc < 6; ++cc)
-          acc[t++] += v[r] * v[cc];
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
-        acc[23 + r] += v[r] * b;
-    }
-    else {
-      const float4 nn = ldg4(a.tgt_normals + m.pos);
-      if (!(isfinite(nn.x) && isfinite(nn.y) && isfinite(nn.z)))
-        continue;  // point_to_plane_lls.hpp:182-190 (pair skipped by the estimator, still a correspondence)
-      const float sx = p.x, sy = p.y, sz = p.z, dx = q.x, dy = q.y, dz = q.z, nx = nn.x, ny = nn.y, nz = nn.z;
-      // float expressions widened to double, exactly as :202-204 and :235 (no fma: -fmad=false)
-      const double A = (double)(nz * sy - ny * sz);
-      const double B = (double)(nx * sz - nz * sx);
-      const double C = (double)(ny * sx - nx * sy);
-      const double D = (double)(nx * dx + ny * dy + nz * dz - nx * sx - ny * sy - nz * sz);
-      acc[2] += A * A; acc[3] += A * B; acc[4] += A * C;
-      acc[5] += A * (double)nx; acc[6] += A * (double)ny; acc[7] += A * (double)nz;
-      acc[8] += B * B; acc[9] += B * C;
-      acc[10] += B * (double)nx; acc[11] += B * (double)ny; acc[12] += B * (double)nz;
-      acc[13] += C * C;
-      acc[14] += C * (double)nx; acc[15] += C * (double)ny; acc[16] += C * (double)nz;
-      acc[17] += (double)(nx * nx); acc[18] += (double)(nx * ny); acc[19] += (double)(nx * nz);
-      acc[20] += (double)(ny * ny); acc[21] += (double)(ny * nz);
-      acc[22] += (double)(nz * nz);
-      acc[23] += A * D; acc[24] += B * D; acc[25] += C * D;
-      acc[26] += (double)nx * D; acc[27] += (double)ny * D; acc[28] += (double)nz * D;
-    }
+    const float4 n2 = ldg4(a.tgt_normals + m.pos);
+    const float4 n1 = a.cur_normals[i];
+    add_pair_terms<EST>(acc, p, q, float3{}, n2, n1, a.enforce_same_dir);
   }
-  block_reduce_and_publish<NACC>(acc, a);
+  if (block_reduce_and_publish<kAccLls>(acc, GridSum{a.partials, a.counter, a.accum}))
+    peer_exchange(a);
 }
 
 // ---- accumulation over an explicit correspondence list (stand-alone estimators) ------------------------
@@ -649,7 +668,7 @@ struct PairArgs {
   const pclb200_corr* corr;   // nullable: pair i <-> i
   size_t n;
   float ox, oy, oz;
-  IterArgs pub;               // partials / counter / accum
+  GridSum pub;                // the grid sum's partials / counter / totals
 };
 
 template <int EST>
@@ -668,59 +687,13 @@ k_accum_pairs(const PairArgs a)
     acc[0] += 1.0;
     if (a.corr)
       acc[1] += (double)a.corr[i].distance;
-    if (EST == PCLB200_EST_SVD) {
-      const double px = (double)p.x - (double)a.ox, py = (double)p.y - (double)a.oy, pz = (double)p.z - (double)a.oz;
-      const double qx = (double)q.x - (double)a.ox, qy = (double)q.y - (double)a.oy, qz = (double)q.z - (double)a.oz;
-      acc[2] += px; acc[3] += py; acc[4] += pz;
-      acc[5] += qx; acc[6] += qy; acc[7] += qz;
-      acc[8] += qx * px; acc[9] += qx * py; acc[10] += qx * pz;
-      acc[11] += qy * px; acc[12] += qy * py; acc[13] += qy * pz;
-      acc[14] += qz * px; acc[15] += qz * py; acc[16] += qz * pz;
-    }
-    else if (EST == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS) {
-      const float4 n2 = ldg4(a.tgt_normals + mi);
-      const float4 n1 = ldg4(a.src_normals + qi);
-      const double d12 = (double)n1.x * n2.x + (double)n1.y * n2.y + (double)n1.z * n2.z;
-      const double sg = (!a.enforce_same_dir || d12 >= 0.0) ? 1.0 : -1.0;
-      const double nx = (double)n1.x + sg * n2.x, ny = (double)n1.y + sg * n2.y, nz = (double)n1.z + sg * n2.z;
-      if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && isfinite(q.x) && isfinite(q.y) && isfinite(q.z) &&
-            isfinite(nx) && isfinite(ny) && isfinite(nz)))
-        continue;
-      const double sx = (double)p.x + q.x, sy = (double)p.y + q.y, sz = (double)p.z + q.z;
-      const double v[6] = {sy * nz - sz * ny, sz * nx - sx * nz, sx * ny - sy * nx, nx, ny, nz};
-      const double b = ((double)q.x - p.x) * nx + ((double)q.y - p.y) * ny + ((double)q.z - p.z) * nz;
-      int t = 2;
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
-#pragma unroll
-        for (int cc = r; cc < 6; ++cc)
-          acc[t++] += v[r] * v[cc];
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
-        acc[23 + r] += v[r] * b;
-    }
-    else {
-      const float4 nn = ldg4(a.tgt_normals + mi);
-      if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && isfinite(q.x) && isfinite(q.y) && isfinite(q.z) &&
-            isfinite(nn.x) && isfinite(nn.y) && isfinite(nn.z)))
-        continue;
-      const float sx = p.x, sy = p.y, sz = p.z, dx = q.x, dy = q.y, dz = q.z, nx = nn.x, ny = nn.y, nz = nn.z;
-      const double A = (double)(nz * sy - ny * sz);
-      const double B = (double)(nx * sz - nz * sx);
-      const double C = (double)(ny * sx - nx * sy);
-      const double D = (double)(nx * dx + ny * dy + nz * dz - nx * sx - ny * sy - nz * sz);
-      acc[2] += A * A; acc[3] += A * B; acc[4] += A * C;
-      acc[5] += A * (double)nx; acc[6] += A * (double)ny; acc[7] += A * (double)nz;
-      acc[8] += B * B; acc[9] += B * C;
-      acc[10] += B * (double)nx; acc[11] += B * (double)ny; acc[12] += B * (double)nz;
-      acc[13] += C * C;
-      acc[14] += C * (double)nx; acc[15] += C * (double)ny; acc[16] += C * (double)nz;
-      acc[17] += (double)(nx * nx); acc[18] += (double)(nx * ny); acc[19] += (double)(nx * nz);
-      acc[20] += (double)(ny * ny); acc[21] += (double)(ny * nz);
-      acc[22] += (double)(nz * nz);
-      acc[23] += A * D; acc[24] += B * D; acc[25] += C * D;
-      acc[26] += (double)nx * D; acc[27] += (double)ny * D; acc[28] += (double)nz * D;
-    }
+    if (EST == PCLB200_EST_SVD)
+      add_pair_terms<EST>(acc, p, q, make_float3(a.ox, a.oy, a.oz), float4{}, float4{}, 0);
+    // a caller's list may pair a non-finite point (the search never does): the LLS estimators skip the pair
+    else if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && isfinite(q.x) && isfinite(q.y) && isfinite(q.z))
+      add_pair_terms<EST>(acc, p, q, float3{}, ldg4(a.tgt_normals + mi),
+                          EST == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS ? ldg4(a.src_normals + qi) : float4{},
+                          a.enforce_same_dir);
   }
   block_reduce_and_publish<NACC>(acc, a.pub);
 }
@@ -1188,7 +1161,7 @@ k_corr(const TreeView T, const float4* __restrict__ q,
 
 // fitness: sum of d2 <= max_range and count (registration.hpp:146-163)
 __global__ void __launch_bounds__(256)
-k_fitness(const TreeView T, const float4* __restrict__ q, size_t nq, double max_range, IterArgs pub)
+k_fitness(const TreeView T, const float4* __restrict__ q, size_t nq, double max_range, GridSum sum, int* d_error)
 {
   double acc[2] = {0.0, 0.0};
   bool overflow = false;
@@ -1206,8 +1179,8 @@ k_fitness(const TreeView T, const float4* __restrict__ q, size_t nq, double max_
     }
   }
   if (overflow)
-    atomicExch(pub.d_error, kErrStackOverflow);
-  block_reduce_and_publish<2>(acc, pub);
+    atomicExch(d_error, kErrStackOverflow);
+  block_reduce_and_publish<2>(acc, sum);
 }
 
 // GeneralizedIterativeClosestPoint::computeCovariances, one thread per point over exact k-NN rows (driver: gicp_covariances)

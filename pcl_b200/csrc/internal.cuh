@@ -319,6 +319,14 @@ void apply_rejector(Ctx& c, const pclb200_rejector& r, const RejectArrays& a, in
 // accumulators of one ICP iteration (all fp64), see icp.cu
 constexpr int kAccum = 40;
 
+// the operation order of the reference that a rigid transform on the device reproduces (Pending::mode, icp_kernels.cuh)
+enum {
+  kApplyIcp = 0,               // icp.hpp:49-111, float
+  kApplyTransformsFloat = 1,   // transforms.hpp, SSE float order
+  kApplyTransformsDouble = 2,  // transforms.hpp, double order
+  kApplyValidationDouble = 3,  // transformation_validation_euclidean.hpp:62-75 with a double matrix (left to right, cast at the end)
+};
+
 // Cross-GPU exchange block of the fused reduce (comm.cu): every rank owns one, mapped into every peer through CUDA IPC
 //   flags[kMaxRanks]                  u64, the latest sequence number published by each peer
 //   slots[2][kMaxRanks][kAccum]       fp64: the accumulators of one ICP iteration (accumulate kernels, icp_kernels.cuh)

@@ -193,10 +193,8 @@ int main()
         std::vector<double> partials(grid * kAccum, 0.0), accum(kAccum, -1.0);
         unsigned counter = 0;
         int d_error = 0;
-        IterArgs pub;
-        std::memset(&pub, 0, sizeof pub);
-        pub.partials = partials.data(); pub.counter = &counter; pub.accum = accum.data(); pub.d_error = &d_error;
-        launch(grid, 256, [&] { k_fitness(TV, q.data(), (size_t)ns, max_range, pub); });
+        const GridSum sum{partials.data(), &counter, accum.data()};
+        launch(grid, 256, [&] { k_fitness(TV, q.data(), (size_t)ns, max_range, sum, &d_error); });
         const double got = accum[0] > 0 ? accum[1] / accum[0] : std::numeric_limits<double>::max();
         const double wantf = orc_fitness_score(ot, src.data(), ns, 4, nullptr, ns, 1, T, dbl, max_range, 2);
         CHECK(d_error == 0 && std::fabs(got - wantf) <= 1e-12 * std::fabs(wantf), "fitness %s max_range %g: %.17g, the oracle's %.17g", dbl ? "double" : "float", max_range,
