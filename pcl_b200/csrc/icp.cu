@@ -36,12 +36,9 @@ bool comm_peer_view(Ctx& c, PeerView* view, unsigned long long* seq);
 bool comm_peer_fused(const Ctx& c);  // the per-iteration exchange happens inside the accumulate kernel
 
 // ---- misc streaming kernels ------------------------------------------------------------------------------
-__global__ void k_apply_pending(float4* __restrict__ pts, size_t n, const Pending* __restrict__ pending,
-                                float4* __restrict__ normals /* nullable */)
+__device__ __forceinline__ void transform_range(const Pending& P, float4* __restrict__ pts, size_t n,
+                                                float4* __restrict__ normals /* nullable */)
 {
-  const Pending P = *pending;
-  if (!P.apply)
-    return;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     float4 p = pts[i];
     if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z)))
@@ -58,7 +55,66 @@ __global__ void k_apply_pending(float4* __restrict__ pts, size_t n, const Pendin
   }
 }
 
+// the transform k_solve left for the next iteration
+__global__ void k_apply_pending(float4* __restrict__ pts, size_t n, const Pending* __restrict__ pending,
+                                float4* __restrict__ normals /* nullable */)
+{
+  const Pending P = *pending;
+  if (P.apply)
+    transform_range(P, pts, n, normals);
+}
+
+// a transform known to the host, passed by value so that no host buffer has to outlive the launch
+__global__ void k_transform(float4* __restrict__ pts, size_t n, const Pending P, float4* __restrict__ normals)
+{
+  transform_range(P, pts, n, normals);
+}
+
+__global__ void k_set_pending(Pending* p, const Pending P) { *p = P; }
 __global__ void k_clear_apply(Pending* p) { p->apply = 0; }
+
+// output record i = source record i with xyz (and the normal at float nrm_word, when >= 0) transformed by P as
+// k_transform does: a non-finite point keeps its whole record, a non-finite normal under kApplyIcp stays as it was.  Every
+// record is read once and written once.  vec: stride is a multiple of 16 and both arrays are 16-byte aligned.
+__global__ void k_assemble_records(const unsigned char* __restrict__ raw, size_t n, size_t stride, int nrm_word,
+                                   const Pending P, int vec, unsigned char* __restrict__ out)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const float* r = reinterpret_cast<const float*>(raw + i * stride);
+  float p[3] = {r[0], r[1], r[2]}, m[3] = {0.f, 0.f, 0.f};
+  if (nrm_word >= 0) {
+    m[0] = r[nrm_word]; m[1] = r[nrm_word + 1]; m[2] = r[nrm_word + 2];
+  }
+  if (isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2])) {
+    apply_pending(P, p[0], p[1], p[2]);
+    if (nrm_word >= 0 && !(P.mode == kApplyIcp && !(isfinite(m[0]) && isfinite(m[1]) && isfinite(m[2]))))
+      apply_pending_normal(P, m[0], m[1], m[2]);  // icp.hpp:97-98
+  }
+  // the normal is written after xyz: it wins where a caller's layout lets the two overlap
+  auto word = [&](int q, float v) {
+    const int qn = q - nrm_word;
+    return nrm_word >= 0 && qn >= 0 && qn < 3 ? m[qn] : q < 3 ? p[q] : v;
+  };
+  if (vec) {
+    const float4* r4 = reinterpret_cast<const float4*>(r);
+    float4* o4 = reinterpret_cast<float4*>(out + i * stride);
+    for (int k = 0; k < (int)(stride / 16); ++k) {
+      float4 v = r4[k];
+      v.x = word(4 * k, v.x);
+      v.y = word(4 * k + 1, v.y);
+      v.z = word(4 * k + 2, v.z);
+      v.w = word(4 * k + 3, v.w);
+      o4[k] = v;
+    }
+  }
+  else {
+    float* o = reinterpret_cast<float*>(out + i * stride);
+    for (int q = 0; q < (int)(stride / 4); ++q)
+      o[q] = word(q, r[q]);
+  }
+}
 
 // strided write-back of a dense float4 array: xyz into out + i*stride (+ optional w = 1 when stride >= 16)
 __global__ void k_scatter_xyz(const float4* __restrict__ src, size_t n, unsigned char* __restrict__ out, size_t stride,
@@ -233,17 +289,19 @@ static Pending make_pending(const double* T, int mode, int apply)
   return h;
 }
 
-static void upload_pending(Ctx& c, Pending* d, const Pending& h)
+// the session's Pending slot set to h, in stream order (h travels as a kernel argument: nothing waits for the copy)
+static void set_pending(Ctx& c, Pending* d, const Pending& h)
 {
-  PCLB_CUDA(cudaMemcpyAsync(d, &h, sizeof(h), cudaMemcpyHostToDevice, c.stream));
-  PCLB_CUDA(cudaStreamSynchronize(c.stream));  // h is a stack object
+  k_set_pending<<<1, 1, 0, c.stream>>>(d, h);
+  ++c.launches;
 }
 
-// pts[0..n) (and their normals, when given) transformed in place by T in the operation order `mode`; d: device scratch
-static void transform_on_device(Ctx& c, Pending* d, const double* T, int mode, float4* pts, size_t n, float4* normals)
+// pts[0..n) (and their normals, when given) transformed in place by T in the operation order `mode`
+static void transform_on_device(Ctx& c, const double* T, int mode, float4* pts, size_t n, float4* normals)
 {
-  upload_pending(c, d, make_pending(T, mode, 1));
-  k_apply_pending<<<persistent_grid(c, n, 256, 8), 256, 0, c.stream>>>(pts, n, d, normals);
+  if (n == 0)
+    return;
+  k_transform<<<persistent_grid(c, n, 256, 8), 256, 0, c.stream>>>(pts, n, make_pending(T, mode, 1), normals);
   ++c.launches;
 }
 
@@ -275,7 +333,7 @@ Icp* icp_create(Ctx& c, const pclb200_icp_params& P)
   s->skip_count.alloc(1, c.stream);
   s->red.init(c, (unsigned)c.sm_count * 16);
   icp_reset_state(*s, nullptr);
-  upload_pending(c, s->pending.p, make_pending(s->loop.final_T, transform_mode(P), 0));
+  set_pending(c, s->pending.p, make_pending(s->loop.final_T, transform_mode(P), 0));
   return s.release();
 }
 
@@ -448,6 +506,7 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   cudaStream_t st = c.stream;
   PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
   PCLB_REQUIRE(src != nullptr && n > 0, PCLB200_ERR_INVALID, "icp: empty source");
+  PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
   s.n_all = n;
   s.shard_comm = 0;
   s.src_all.alloc(n, st);
@@ -456,49 +515,62 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   s.src_normal_off = -1;
   if (src_normals) {
     const ptrdiff_t off = static_cast<const unsigned char*>(src_normals) - static_cast<const unsigned char*>(src);
-    if (stride_n == stride && off > 0 && (size_t)off + 12 <= stride)
+    if (stride_n == stride && off > 0 && off % 4 == 0 && (size_t)off + 12 <= stride)
       s.src_normal_off = off;
   }
-  const void* src_dev = src;
+  // The records are read once, from device memory: host records take one contiguous H2D into the session's own copy
+  // (src_raw, or src_all when they already are PointXYZ float4s), device records are copied by the staging pass itself.
+  // Every field other than xyz / normals is carried through to the output.
+  const unsigned char* recs = static_cast<const unsigned char*>(src);
+  unsigned char* copy = nullptr;
+  float4* dense = s.src_all.p;
+  const bool host_src = !is_device_ptr(src);
   if (stride != 16) {
-    // one contiguous H2D of the records; every field other than xyz/normals is carried through to the output
-    PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
     s.src_raw.alloc(n * stride, st);
-    PCLB_CUDA(cudaMemcpyAsync(s.src_raw.p, src, n * stride, cudaMemcpyDefault, st));
-    src_dev = s.src_raw.p;
+    if (host_src) {
+      PCLB_CUDA(cudaMemcpyAsync(s.src_raw.p, src, n * stride, cudaMemcpyHostToDevice, st));
+      recs = s.src_raw.p;
+    }
+    else
+      copy = s.src_raw.p;
   }
-  load_xyz_as_float4(c, src_dev, n, stride, nullptr, 0, s.src_all.p, st);
+  else if (host_src) {
+    PCLB_CUDA(cudaMemcpyAsync(s.src_all.p, src, n * 16, cudaMemcpyHostToDevice, st));
+    recs = reinterpret_cast<const unsigned char*>(s.src_all.p);
+    dense = nullptr;
+  }
+  s.n_q = indices ? n_idx : n;
+  s.src_orig.release();
+  QueryBatch qb;
+  {
+    ProfScope ps(c, "query_sort");
+    stage_records(c, *s.tgt, recs, n, stride, copy, dense, indices ? nullptr : &qb);
+    if (indices) {
+      // index subset: the queries are gathered from the staged points and sorted on their own
+      s.src_orig.alloc(n_idx, st);
+      PCLB_CUDA(cudaMemcpyAsync(s.src_orig.p, indices, n_idx * sizeof(int32_t), cudaMemcpyDefault, st));
+      DevBuf<float4> sub;
+      sub.alloc(n_idx, st);
+      if (n_idx) {
+        k_gather_subset<<<grid_for(n_idx, 256), 256, 0, st>>>(s.src_all.p, s.src_orig.p, n_idx, sub.p);
+        ++c.launches;
+      }
+      make_query_batch(c, *s.tgt, sub.p, s.n_q, qb);
+    }
+  }
+  s.cur = std::move(qb.q);
+  // Nothing in the loop reads the source normals except through cur_normals; the output reads normals that live in the
+  // records from src_raw.  So a dense copy is staged only for cur_normals or for normals kept outside the records.
   s.have_src_normals = src_normals != nullptr;
-  if (src_normals) {
+  s.src_normals.release();
+  const bool normals_in_raw = s.src_normal_off >= 0 && s.src_raw.p;
+  if (src_normals && (needs_cur_normals(s) || !normals_in_raw)) {
     s.src_normals.alloc(n, st);
-    if (s.src_normal_off >= 0 && s.src_raw.p)
+    if (normals_in_raw)
       load_vec3_as_float4(c, s.src_raw.p + s.src_normal_off, n, stride, s.src_normals.p, st);
     else
       load_vec3_as_float4(c, src_normals, n, stride_n, s.src_normals.p, st);
   }
-  else
-    s.src_normals.release();
-  const float4* d_q = s.src_all.p;
-  DevBuf<float4> sub;
-  s.n_q = n;
-  s.src_orig.release();
-  if (indices) {
-    s.n_q = n_idx;
-    s.src_orig.alloc(n_idx, st);
-    PCLB_CUDA(cudaMemcpyAsync(s.src_orig.p, indices, n_idx * sizeof(int32_t), cudaMemcpyDefault, st));
-    sub.alloc(n_idx, st);
-    if (n_idx) {
-      k_gather_subset<<<grid_for(n_idx, 256), 256, 0, st>>>(s.src_all.p, s.src_orig.p, n_idx, sub.p);
-      ++c.launches;
-    }
-    d_q = sub.p;
-  }
-  QueryBatch qb;
-  {
-    ProfScope ps(c, "query_sort");
-    make_query_batch(c, *s.tgt, d_q, s.n_q, qb);
-  }
-  s.cur = std::move(qb.q);
   s.cur_normals.release();
   if (needs_cur_normals(s)) {
     PCLB_REQUIRE(s.have_src_normals, PCLB200_ERR_INVALID,
@@ -527,8 +599,8 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
       if (s.loop.final_T[i] != ((i % 5 == 0) ? 1.0 : 0.0))
         guess_identity = false;
   if (!guess_identity)
-    transform_on_device(c, s.pending.p, s.loop.final_T, transform_mode(s.P), s.cur.p, s.n_q, s.cur_normals.p);
-  upload_pending(c, s.pending.p, make_pending(s.loop.last_T, transform_mode(s.P), 0));
+    transform_on_device(c, s.loop.final_T, transform_mode(s.P), s.cur.p, s.n_q, s.cur_normals.p);
+  set_pending(c, s.pending.p, make_pending(s.loop.last_T, transform_mode(s.P), 0));
   PCLB_CUDA(cudaGetLastError());
 }
 
@@ -620,16 +692,21 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     if (track_mode != PCLB200_TRACK_AUTO)  // AUTO carries the last decision over from the previous call
       s.loop.track_next = track_mode == PCLB200_TRACK_ON ? 1 : 0;
     LoopCtrl* h_ctrl = static_cast<LoopCtrl*>(c.pinned);
-    int* h_err = reinterpret_cast<int*>(h_ctrl + 1);
+    unsigned long long* h_skipped = reinterpret_cast<unsigned long long*>(h_ctrl + 1);
+    int* h_err = reinterpret_cast<int*>(h_skipped + 1);
+    static_assert(sizeof(LoopCtrl) % 8 == 0, "the skip count follows the loop state in the pinned block");
     *h_ctrl = s.loop;
     PCLB_CUDA(cudaMemcpyAsync(s.ctrl.p, h_ctrl, sizeof(LoopCtrl), cudaMemcpyHostToDevice, st));
+    // one synchronise reads the loop state, the skip count (statistics) and the device error flag
     auto read_back = [&]() {
       PCLB_CUDA(cudaMemcpyAsync(h_ctrl, s.ctrl.p, sizeof(LoopCtrl), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaMemcpyAsync(h_skipped, s.skip_count.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
       PCLB_CUDA(cudaMemcpyAsync(h_err, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
       PCLB_CUDA(cudaStreamSynchronize(st));
       if (*h_err)
         raise_device_error(c, *h_err);
       s.loop = *h_ctrl;
+      s.total_skipped = (int64_t)*h_skipped;
     };
     IterArgs a;
     memset(&a, 0, sizeof(a));
@@ -745,12 +822,6 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     if (!needs_host_between)
       read_back();
   }
-  if (stats) {
-    unsigned long long h = 0;
-    PCLB_CUDA(cudaMemcpyAsync(&h, s.skip_count.p, sizeof(h), cudaMemcpyDeviceToHost, st));
-    PCLB_CUDA(cudaStreamSynchronize(st));
-    s.total_skipped = (int64_t)h;
-  }
   fill_stats(s, stats);
 }
 
@@ -795,37 +866,42 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
   PCLB_REQUIRE(s.src_all.p, PCLB200_ERR_INVALID, "icp: no source");
-  DevBuf<float4> tmp, tmpn;
-  tmp.alloc(s.n_all, st);
-  PCLB_CUDA(cudaMemcpyAsync(tmp.p, s.src_all.p, s.n_all * sizeof(float4), cudaMemcpyDeviceToDevice, st));
   const bool do_n = out_normals && s.have_src_normals;
-  if (do_n) {
-    tmpn.alloc(s.n_all, st);
-    PCLB_CUDA(cudaMemcpyAsync(tmpn.p, s.src_normals.p, s.n_all * sizeof(float4), cudaMemcpyDeviceToDevice, st));
-  }
-  DevBuf<Pending> pend;
-  pend.alloc(1, st);
-  {
-    ProfScope ps(c, "transform_out");
-    transform_on_device(c, pend.p, s.loop.final_T, transform_mode(s.P), tmp.p, s.n_all, do_n ? tmpn.p : nullptr);
-  }
+  const int mode = transform_mode(s.P);
   const bool normals_inside =
       do_n && s.src_normal_off >= 0 &&
       static_cast<unsigned char*>(out_normals) - static_cast<unsigned char*>(out_pts) == s.src_normal_off && stride_n == stride_out;
   if (s.src_raw.p && stride_out == s.src_stride && (!do_n || normals_inside)) {
-    // output = *input_ (all fields), then xyz / normals overwritten: assembled on the device, one contiguous copy out
+    // output = *input_ (all fields) with xyz / normals transformed: one pass over the records, one contiguous copy out
     DevBuf<unsigned char> rec;
     unsigned char* d_rec = out_on_device(c, static_cast<unsigned char*>(out_pts), s.n_all * stride_out, rec);
-    PCLB_CUDA(cudaMemcpyAsync(d_rec, s.src_raw.p, s.n_all * stride_out, cudaMemcpyDeviceToDevice, st));
-    k_scatter_xyz<<<grid_for(s.n_all, 256), 256, 0, st>>>(tmp.p, s.n_all, d_rec, stride_out, 0, 0.f);
-    ++c.launches;
-    if (do_n) {
-      k_scatter_xyz<<<grid_for(s.n_all, 256), 256, 0, st>>>(tmpn.p, s.n_all, d_rec + s.src_normal_off, stride_out, 0, 0.f);
+    const int vec = stride_out % 16 == 0 && reinterpret_cast<uintptr_t>(d_rec) % 16 == 0;  // src_raw is 16-aligned
+    {
+      ProfScope ps(c, "transform_out");
+      k_assemble_records<<<grid_for(s.n_all, 256), 256, 0, st>>>(s.src_raw.p, s.n_all, stride_out,
+                                                                 do_n ? (int)(s.src_normal_off / 4) : -1,
+                                                                 make_pending(s.loop.final_T, mode, 1), vec, d_rec);
       ++c.launches;
     }
+    PCLB_CUDA(cudaGetLastError());
     copy_out(c, static_cast<unsigned char*>(out_pts), rec, s.n_all * stride_out);
     PCLB_CUDA(cudaStreamSynchronize(st));
     return;
+  }
+  // every other layout: dense xyz (and normals) transformed, then written to the caller's arrays
+  DevBuf<float4> tmp, tmpn;
+  tmp.alloc(s.n_all, st);
+  PCLB_CUDA(cudaMemcpyAsync(tmp.p, s.src_all.p, s.n_all * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+  if (do_n) {
+    tmpn.alloc(s.n_all, st);
+    if (s.src_normals.p)
+      PCLB_CUDA(cudaMemcpyAsync(tmpn.p, s.src_normals.p, s.n_all * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+    else  // normals that live in the records, not staged by set_source
+      load_vec3_as_float4(c, s.src_raw.p + s.src_normal_off, s.n_all, s.src_stride, tmpn.p, st);
+  }
+  {
+    ProfScope ps(c, "transform_out");
+    transform_on_device(c, s.loop.final_T, mode, tmp.p, s.n_all, do_n ? tmpn.p : nullptr);
   }
   auto write_back = [&](const DevBuf<float4>& d, void* out, size_t stride, int write_w, float w) {
     if (stride == 16 && write_w) {
@@ -955,11 +1031,8 @@ size_t correspondences(Ctx& c, const Index& tgt, const Index* src_index, const v
   DevBuf<float4> dense;
   dense.alloc(nq, st);
   load_xyz_as_float4(c, src, n, stride, indices, n_idx, dense.p, st);
-  DevBuf<Pending> pend;
-  if (pre_T) {  // the caller's cloud is searched after a rigid transform (consumers that validate a pose)
-    pend.alloc(1, st);
-    transform_on_device(c, pend.p, pre_T, pre_mode, dense.p, nq, nullptr);
-  }
+  if (pre_T)  // the caller's cloud is searched after a rigid transform (consumers that validate a pose)
+    transform_on_device(c, pre_T, pre_mode, dense.p, nq, nullptr);
   DevBuf<int32_t> staged_ind;
   const int32_t* d_ind = on_device(c, indices, n_idx, staged_ind);
   QueryBatch qb;
@@ -994,11 +1067,9 @@ double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t
   DevBuf<float4> dense;
   dense.alloc(nq, st);
   load_xyz_as_float4(c, src, n, stride, use_sub ? indices : nullptr, use_sub ? n_idx : 0, dense.p, st);
-  DevBuf<Pending> pend;
-  pend.alloc(1, st);
   // default: pcl::transformPointCloud
   const int mode = mode_override >= 0 ? mode_override : (scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat);
-  transform_on_device(c, pend.p, T, mode, dense.p, nq, nullptr);
+  transform_on_device(c, T, mode, dense.p, nq, nullptr);
   QueryBatch qb;
   make_query_batch(c, tgt, dense.p, nq, qb);
   Reducer red;

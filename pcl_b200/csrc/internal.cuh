@@ -254,6 +254,12 @@ struct QueryBatch {
 };
 void make_query_batch(Ctx& c, const Index& ref_frame, const float4* d_q /*n, w ignored*/, size_t n,
                       QueryBatch& out);
+// One pass over n strided records in device memory (xyz at offset 0, stride a multiple of 4): the whole records into
+// `copy` and xyz into `dense` (float4, w = the record's w when stride == 16, else 1), each nullable, and, when qb is given,
+// the query batch make_query_batch would make of those points (read from `dense`, or from `recs` when dense is null and
+// stride == 16) without another pass over them.
+void stage_records(Ctx& c, const Index& ref_frame, const unsigned char* recs, size_t n, size_t stride, unsigned char* copy,
+                   float4* dense, QueryBatch* qb);
 // load_xyz_as_float4 of a caller's query points into `dense` (kept alive: some kernels read it in input order), then
 // make_query_batch over it
 QueryBatch load_queries(Ctx& c, const Index& ref_frame, const void* pts, size_t n, size_t stride, const int32_t* subset,

@@ -97,19 +97,11 @@ struct SortedCloud {
   float scale = 1.f;
 };
 
-// bbox (when frame == nullptr) + keys + radix sort of n dense float4 points
-static void morton_sort(Ctx& c, const float4* d_pts, size_t n, const Index* frame, SortedCloud& out)
+// bbox + 63-bit Morton keys + radix sort of n dense float4 points (the index's order)
+static void morton_sort(Ctx& c, const float4* d_pts, size_t n, SortedCloud& out)
 {
   cudaStream_t s = c.stream;
-  if (frame) {
-    for (int d = 0; d < 3; ++d) {
-      out.lo[d] = frame->lo[d];
-      out.hi[d] = frame->hi[d];
-    }
-    out.scale = frame->morton_scale;
-    out.n_valid = n;  // callers of the query path never pass non-finite points they care about
-  }
-  else {
+  {
     DevBuf<BBoxAcc> acc;
     acc.alloc(1, s);
     BBoxAcc init;
@@ -144,26 +136,18 @@ static void morton_sort(Ctx& c, const float4* d_pts, size_t n, const Index* fram
   vals_in.alloc(n, s);
   out.keys.alloc(n, s);
   out.vals.alloc(n, s);
-  const bool hilbert = frame != nullptr;  // queries: Hilbert order (compact runs of 32); the tree itself: Morton
-  if (hilbert)
-    k_morton<true><<<grid_for(n, 256), 256, 0, s>>>(d_pts, n, out.lo[0], out.lo[1], out.lo[2], out.scale, keys_in.p,
-                                                   vals_in.p);
-  else
-    k_morton<false><<<grid_for(n, 256), 256, 0, s>>>(d_pts, n, out.lo[0], out.lo[1], out.lo[2], out.scale, keys_in.p,
-                                                    vals_in.p);
+  k_morton<false><<<grid_for(n, 256), 256, 0, s>>>(d_pts, n, out.lo[0], out.lo[1], out.lo[2], out.scale, keys_in.p,
+                                                  vals_in.p);
   ++c.launches;
   size_t tmp_bytes = 0;
-  // The index needs the full 63-bit order (leaves are radix-tree cells).  A query batch only needs spatial coherence: the
-  // top 32 bits of the Hilbert index (10.7 bits per axis, cells about a leaf wide) order it just as well and halve the
-  // radix passes (stable sort: points of one such cell keep their input order).
-  const int begin_bit = frame ? 31 : 0, end_bit = frame ? 63 : 64;
+  // the index needs the full 63-bit order (leaves are radix-tree cells)
   PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, out.keys.p, vals_in.p, out.vals.p,
-                                            (int)n, begin_bit, end_bit, s));
+                                            (int)n, 0, 64, s));
   DevBuf<unsigned char> tmp;
   tmp.alloc(tmp_bytes, s);
   PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, out.keys.p, vals_in.p, out.vals.p, (int)n,
-                                            begin_bit, end_bit, s));
-  c.launches += frame ? 5 : 9;  // onesweep: histogram + one pass per 8-bit digit
+                                            0, 64, s));
+  c.launches += 9;  // onesweep: histogram + one pass per 8-bit digit
   PCLB_CUDA(cudaGetLastError());
 }
 
@@ -174,7 +158,7 @@ static Index* build_from_dense(Ctx& c, const float4* d_pts, size_t n, const int3
   PCLB_REQUIRE(n > 0, PCLB200_ERR_EMPTY, "cannot index an empty cloud (kdtree_flann.hpp:118-129)");
   PCLB_REQUIRE(n < (size_t)0x7fffffff, PCLB200_ERR_INVALID, "cloud too large for int32 indices");
   SortedCloud sc;
-  morton_sort(c, d_pts, n, nullptr, sc);
+  morton_sort(c, d_pts, n, sc);
   PCLB_REQUIRE(sc.n_valid > 0, PCLB200_ERR_EMPTY, "no finite point in the cloud (kdtree_flann.hpp:124-129)");
   std::unique_ptr<Index> idx(new Index());
   idx->ctx = &c;
@@ -364,18 +348,47 @@ __global__ void k_gather_queries(const float4* __restrict__ q, const int32_t* __
   out[j] = make_float4(v.x, v.y, v.z, __int_as_float(slot));
 }
 
-void make_query_batch(Ctx& c, const Index& frame, const float4* d_q, size_t n, QueryBatch& out)
+void stage_records(Ctx& c, const Index& frame, const unsigned char* recs, size_t n, size_t stride, unsigned char* copy,
+                   float4* dense, QueryBatch* qb)
 {
   cudaStream_t s = c.stream;
-  out.n = n;
-  if (n == 0)
+  if (qb)
+    qb->n = n;
+  if (n == 0 || !(copy || dense || qb))
     return;
-  SortedCloud sc;
-  morton_sort(c, d_q, n, &frame, sc);
-  out.q.alloc(n, s);
-  k_gather_queries<<<grid_for(n, 256), 256, 0, s>>>(d_q, sc.vals.p, n, out.q.p);
+  DevBuf<unsigned> keys_in, keys;
+  DevBuf<int32_t> vals_in, vals;
+  if (qb) {
+    keys_in.alloc(n, s);
+    vals_in.alloc(n, s);
+  }
+  const int vec = stride % 16 == 0 && reinterpret_cast<uintptr_t>(recs) % 16 == 0 &&
+                  reinterpret_cast<uintptr_t>(copy) % 16 == 0;
+  k_stage_records<<<grid_for(n, 256), 256, 0, s>>>(recs, n, stride, vec, copy, dense, frame.lo[0], frame.lo[1],
+                                                    frame.lo[2], frame.morton_scale, keys_in.p, vals_in.p);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
+  if (!qb)
+    return;
+  // stable: the points of one key cell keep their input order
+  keys.alloc(n, s);
+  vals.alloc(n, s);
+  size_t tmp_bytes = 0;
+  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, 32, s));
+  DevBuf<unsigned char> tmp;
+  tmp.alloc(tmp_bytes, s);
+  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, 32, s));
+  c.launches += 5;  // onesweep: histogram + one pass per 8-bit digit
+  qb->q.alloc(n, s);
+  const float4* pts = dense ? dense : reinterpret_cast<const float4*>(recs);
+  k_gather_queries<<<grid_for(n, 256), 256, 0, s>>>(pts, vals.p, n, qb->q.p);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
+void make_query_batch(Ctx& c, const Index& frame, const float4* d_q, size_t n, QueryBatch& out)
+{
+  stage_records(c, frame, reinterpret_cast<const unsigned char*>(d_q), n, 16, nullptr, nullptr, &out);
 }
 
 QueryBatch load_queries(Ctx& c, const Index& frame, const void* pts, size_t n, size_t stride, const int32_t* subset,

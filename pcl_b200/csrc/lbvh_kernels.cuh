@@ -123,6 +123,48 @@ __global__ void k_morton(const float4* __restrict__ p, size_t n, float lx, float
   vals[i] = (int32_t)i;
 }
 
+// The key a query batch is sorted by: the top 32 bits (31..62) of hilbert63, ~0 for a non-finite point (it sorts last).
+// 10.7 bits per axis give cells about a leaf wide, as coherent an order as the full index, in half the radix passes.
+__device__ __forceinline__ unsigned hilbert_key32(float x, float y, float z, float lx, float ly, float lz, float scale)
+{
+  if (!(isfinite(x) && isfinite(y) && isfinite(z)))
+    return ~0u;
+  return (unsigned)(hilbert63(x, y, z, lx, ly, lz, scale) >> 31);
+}
+
+// One pass over n strided records (xyz at offset 0): the whole record into `copy`, xyz into `dense` as float4 (w = the
+// record's w when stride == 16, else 1) and, into keys / vals, the point's hilbert_key32 and its slot.  Each output is
+// nullable.  vec: stride is a multiple of 16 and recs / copy are 16-byte aligned (the copy moves float4s).
+__global__ void k_stage_records(const unsigned char* __restrict__ recs, size_t n, size_t stride, int vec,
+                                unsigned char* __restrict__ copy, float4* __restrict__ dense, float lx, float ly, float lz,
+                                float scale, unsigned* __restrict__ keys, int32_t* __restrict__ vals)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const float* r = reinterpret_cast<const float*>(recs + i * stride);
+  const float x = r[0], y = r[1], z = r[2];
+  if (copy) {
+    if (vec) {
+      const float4* r4 = reinterpret_cast<const float4*>(r);
+      float4* o4 = reinterpret_cast<float4*>(copy + i * stride);
+      for (size_t k = 0; k < stride / 16; ++k)
+        o4[k] = r4[k];
+    }
+    else {
+      float* o = reinterpret_cast<float*>(copy + i * stride);
+      for (size_t k = 0; k < stride / 4; ++k)
+        o[k] = r[k];
+    }
+  }
+  if (dense)
+    dense[i] = make_float4(x, y, z, stride == 16 ? r[3] : 1.f);
+  if (keys) {
+    keys[i] = hilbert_key32(x, y, z, lx, ly, lz, scale);
+    vals[i] = (int32_t)i;
+  }
+}
+
 // sorted gather: out[j] = {xyz of slot vals[j], orig index bits}; pads the tail with +inf sentinels
 __global__ void k_gather_sorted(const float4* __restrict__ p, const int32_t* __restrict__ vals,
                                 const int32_t* __restrict__ orig_of_slot, size_t n_valid, size_t n_padded,
