@@ -695,8 +695,16 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     unsigned long long* h_skipped = reinterpret_cast<unsigned long long*>(h_ctrl + 1);
     int* h_err = reinterpret_cast<int*>(h_skipped + 1);
     static_assert(sizeof(LoopCtrl) % 8 == 0, "the skip count follows the loop state in the pinned block");
+    const bool first = s.loop.iterations == 0;
+    if (first)  // the first iteration's SVD origin (LoopCtrl::origin); k_seed_origin replaces it on a single rank
+      for (int r = 0; r < 3; ++r)
+        s.loop.origin[r] = 0.5f * (T.lo[r] + T.hi[r]);
     *h_ctrl = s.loop;
     PCLB_CUDA(cudaMemcpyAsync(s.ctrl.p, h_ctrl, sizeof(LoopCtrl), cudaMemcpyHostToDevice, st));
+    if (first && s.P.estimator == PCLB200_EST_SVD && !comm_active(c)) {
+      k_seed_origin<<<1, 1, 0, st>>>(s.cur.p, nullptr, s.n_q, s.ctrl.p->origin);
+      ++c.launches;
+    }
     // one synchronise reads the loop state, the skip count (statistics) and the device error flag
     auto read_back = [&]() {
       PCLB_CUDA(cudaMemcpyAsync(h_ctrl, s.ctrl.p, sizeof(LoopCtrl), cudaMemcpyDeviceToHost, st));
@@ -718,9 +726,7 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     a.n = s.n_q;
     a.pending = s.pending.p;
     a.gate = gate_from_max_dist(s.P.max_correspondence_distance);
-    a.ox = 0.5f * (T.lo[0] + T.hi[0]);
-    a.oy = 0.5f * (T.lo[1] + T.hi[1]);
-    a.oz = 0.5f * (T.lo[2] + T.hi[2]);
+    a.origin = s.ctrl.p->origin;
     a.partials = s.red.partials.p;
     a.partials2 = s.red.partials2.p;
     a.counter = s.red.counter.p;
@@ -807,9 +813,8 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
       }
       {
         ProfScope ps(c, "solve");
-        k_solve<<<1, 32, 0, st>>>(s.red.accum.p, s.P.estimator, s.P.scalar_is_double, transform_mode(s.P), (double)a.ox,
-                                  (double)a.oy, (double)a.oz, 3, s.pending.p, s.solve_out.p, s.P.svd_no_umeyama, s.ctrl.p,
-                                  crit);
+        k_solve<<<1, 32, 0, st>>>(s.red.accum.p, s.P.estimator, s.P.scalar_is_double, transform_mode(s.P), a.origin, 3,
+                                  s.pending.p, s.solve_out.p, s.P.svd_no_umeyama, s.ctrl.p, crit);
         ++c.launches;
       }
       PCLB_CUDA(cudaGetLastError());
@@ -994,21 +999,23 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
   a.n = n;
   a.ox = a.oy = a.oz = 0.f;
   a.pub = red.sum();
+  DevBuf<float4> origin;  // the SVD sums' origin (icp_kernels.cuh): the first pair's target point that is finite, else 0
   if (est == PCLB200_EST_SVD) {
-    // shift by the first target point to keep the fp64 sums small
-    float4 first;
-    PCLB_CUDA(cudaMemcpyAsync(&first, dt.p, sizeof(float4), cudaMemcpyDeviceToHost, st));
+    origin.alloc(1, st);
+    PCLB_CUDA(cudaMemsetAsync(origin.p, 0, sizeof(float4), st));
+    k_seed_origin<<<1, 1, 0, st>>>(dt.p, d_corr, n, &origin.p->x);
+    float4 o;
+    PCLB_CUDA(cudaMemcpyAsync(&o, origin.p, sizeof(float4), cudaMemcpyDeviceToHost, st));
     PCLB_CUDA(cudaStreamSynchronize(st));
-    if (std::isfinite(first.x) && std::isfinite(first.y) && std::isfinite(first.z)) {
-      a.ox = first.x; a.oy = first.y; a.oz = first.z;
-    }
+    a.ox = o.x; a.oy = o.y; a.oz = o.z;
     k_accum_pairs<PCLB200_EST_SVD><<<grid, 256, 0, st>>>(a);
+    ++c.launches;
   }
   else if (est == PCLB200_EST_POINT_TO_PLANE_LLS)
     k_accum_pairs<PCLB200_EST_POINT_TO_PLANE_LLS><<<grid, 256, 0, st>>>(a);
   else
     k_accum_pairs<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS><<<grid, 256, 0, st>>>(a);
-  k_solve<<<1, 32, 0, st>>>(red.accum.p, est, scalar_is_double, kApplyIcp, (double)a.ox, (double)a.oy, (double)a.oz, 1,
+  k_solve<<<1, 32, 0, st>>>(red.accum.p, est, scalar_is_double, kApplyIcp, origin.p ? &origin.p->x : nullptr, 1,
                             nullptr, so.p, svd_correlation, nullptr, CritParams{});
   c.launches += 2;
   SolveOut h;

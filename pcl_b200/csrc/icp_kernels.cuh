@@ -14,7 +14,10 @@ namespace pclb200 {
 
 // accumulator slots (fp64)
 //   common : [0] accepted pairs, [1] sum of squared distances
-//   SVD    : [2..4] sum(p-o)  [5..7] sum(q-o)  [8..16] sum (q-o)(p-o)^T row-major
+//   SVD    : [2..4] sum(p-o)  [5..7] sum(q-o)  [8..16] sum (q-o)(p-o)^T row-major, about an origin o near the pairs:
+//            k_solve forms sum(q-o)(p-o)^T / n - m_q m_p^T (m = centroid - o), whose relative error grows like
+//            (|m| / spread of the pairs)^2, so o must lie near the pairs.  o is a float point (p - o is exact in fp64):
+//            in the loop LoopCtrl::origin, stand-alone the first pair's target point that is finite.
 //   LLS    : [2..22] upper triangle of A^T A (row-major order 0,1,..5,7,..), [23..28] A^T b
 constexpr int kAccSvd = 17;
 constexpr int kAccLls = 29;
@@ -50,6 +53,11 @@ struct LoopCtrl {
   double prev_mse, mse, n_corr;
   long long total_corr;
   double final_T[16], last_T[16];
+  // origin of the SVD sums (x, y, z; [3] unused), on the device because the iterations are enqueued ahead: k_solve sets
+  // it to the float-rounded centroid of each iteration's target points, taken from the (cross-rank) totals so that every
+  // rank holds the same one.  The first iteration uses the first finite point of the staged source (k_seed_origin) on a
+  // single rank, and the target's bounding-box centre with a communicator.
+  float origin[4];
 };
 
 struct CritParams {  // what DefaultConvergenceCriteria and the tracking heuristic need (pclb200_icp_params subset)
@@ -115,7 +123,7 @@ struct IterArgs {
   size_t n;
   const Pending* pending;
   float gate;
-  float ox, oy, oz;           // accumulation origin (target bbox centre)
+  const float* origin;        // origin of the SVD sums: LoopCtrl::origin (3 floats)
   double* partials;           // gridDim.x * kAccum
   double* partials2;          // gridDim.x * 128 (two 8x8 fp64 tiles per block: k_accum_dmma)
   unsigned* counter;
@@ -315,7 +323,7 @@ __device__ __forceinline__ void mma_rows(const IterArgs& a, float* __restrict__ 
   *reinterpret_cast<float4*>(tB + lane * 8 + 4) = make_float4(rb[4], rb[5], rb[6], rb[7]);
   __syncwarp();
   const int g = lane >> 2, t = lane & 3;
-  const double og = g == 0 ? (double)a.ox : (g == 1 ? (double)a.oy : (double)a.oz);
+  const double og = EST == PCLB200_EST_SVD && g < 3 ? (double)a.origin[g] : 0.0;
 #pragma unroll
   for (int st = 0; st < 8; ++st) {
     const int row = (4 * st + t) * 8;
@@ -883,9 +891,10 @@ __device__ bool has_converged_dev(LoopCtrl& L, const CritParams& P, const double
   return false;
 }
 
-__global__ void k_solve(const double* __restrict__ accum, int est, int scalar_is_double, int mode, double ox,
-                        double oy, double oz, int min_corr, Pending* pending, SolveOut* out, int svd_correlation,
-                        LoopCtrl* ctrl, CritParams crit)
+// origin: the SVD sums' origin (3 floats in device memory; nullptr = 0)
+__global__ void k_solve(const double* __restrict__ accum, int est, int scalar_is_double, int mode, const float* origin,
+                        int min_corr, Pending* pending, SolveOut* out, int svd_correlation, LoopCtrl* ctrl,
+                        CritParams crit)
 {
   if (threadIdx.x != 0 || blockIdx.x != 0)
     return;
@@ -938,13 +947,19 @@ __global__ void k_solve(const double* __restrict__ accum, int est, int scalar_is
           R[3 * r + c] = a;
         }
     }
-    const double o[3] = {ox, oy, oz};
+    double o[3] = {0.0, 0.0, 0.0};
+    if (origin)
+      for (int r = 0; r < 3; ++r)
+        o[r] = origin[r];
     for (int r = 0; r < 3; ++r) {
       for (int c = 0; c < 3; ++c)
         T[4 * r + c] = R[3 * r + c];
       T[4 * r + 3] = (mq[r] + o[r]) - (R[3 * r] * (mp[0] + o[0]) + R[3 * r + 1] * (mp[1] + o[1]) +
                                        R[3 * r + 2] * (mp[2] + o[2]));
     }
+    if (ctrl)  // the next iteration's pairs lie about where this one's did
+      for (int r = 0; r < 3; ++r)
+        ctrl->origin[r] = (float)(mq[r] + o[r]);
   }
   else if (ok) {
     double A[6][7];
@@ -1046,6 +1061,21 @@ __global__ void k_solve(const double* __restrict__ accum, int est, int scalar_is
                      : crit.track_mode == PCLB200_TRACK_OFF ? 0 : (disp < 0.5 * sqrt(fmax(L.mse, 0.0)) ? 1 : 0);
     }
     L.lb_valid = tracked;  // the search of THIS iteration wrote the bounds iff it was a TRACK search
+  }
+}
+
+// An origin of the SVD sums (slot layout at the top of this file): the first finite point of pts, or of
+// pts[corr[i].index_match] over a pair list; `out` is left as it was when there is none.  One thread: the scan normally stops at the first point.
+__global__ void k_seed_origin(const float4* __restrict__ pts, const pclb200_corr* __restrict__ corr, size_t n, float* out)
+{
+  for (size_t i = 0; i < n; ++i) {
+    const float4 p = pts[corr ? (size_t)corr[i].index_match : i];
+    if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
+      out[0] = p.x;
+      out[1] = p.y;
+      out[2] = p.z;
+      return;
+    }
   }
 }
 

@@ -147,7 +147,10 @@ static void run_align(const char* name, const Scene& S, int estimator, bool scal
   a.n = ns;
   a.pending = &pending;
   a.gate = gate_from_max_dist(max_dist);
-  a.ox = 0.5f * (I.lo[0] + I.hi[0]); a.oy = 0.5f * (I.lo[1] + I.hi[1]); a.oz = 0.5f * (I.lo[2] + I.hi[2]);
+  // the first iteration's SVD origin as icp.cu sets it on a single rank: the bbox centre, replaced by the first finite source point
+  for (int r = 0; r < 3; ++r) ctrl.origin[r] = 0.5f * (I.lo[r] + I.hi[r]);
+  if (estimator == PCLB200_EST_SVD) k_seed_origin(cur.data(), nullptr, ns, ctrl.origin);
+  a.origin = ctrl.origin;
   a.partials2 = partials2.data();
   a.counter = &counter;
   a.accum = accum.data();
@@ -265,6 +268,7 @@ static void run_align(const char* name, const Scene& S, int estimator, bool scal
       else
         warp_emu::run_block(256, [&] { k_accum<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS>(a, match.data()); });
       double ref[kAccum] = {0};
+      const double o[3] = {ctrl.origin[0], ctrl.origin[1], ctrl.origin[2]};   // k_solve moves it for the next iteration
       for (std::size_t i = 0; i < ns; ++i) {
         const Match m = match[i];
         if (!match_accepted(m)) continue;
@@ -272,7 +276,7 @@ static void run_align(const char* name, const Scene& S, int estimator, bool scal
         ref[0] += 1.0;
         ref[1] += (double)m.d2;
         if (estimator == PCLB200_EST_SVD) {
-          const double P3[3] = {(double)p.x - a.ox, (double)p.y - a.oy, (double)p.z - a.oz}, Q3[3] = {(double)q.x - a.ox, (double)q.y - a.oy, (double)q.z - a.oz};
+          const double P3[3] = {(double)p.x - o[0], (double)p.y - o[1], (double)p.z - o[2]}, Q3[3] = {(double)q.x - o[0], (double)q.y - o[1], (double)q.z - o[2]};
           for (int d = 0; d < 3; ++d) { ref[2 + d] += P3[d]; ref[5 + d] += Q3[d]; }
           for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) ref[8 + 3 * r + c] += Q3[r] * P3[c];
         }
@@ -297,7 +301,7 @@ static void run_align(const char* name, const Scene& S, int estimator, bool scal
     else if (estimator == PCLB200_EST_SVD)   // the driver enqueues these regardless: they must return at once
       warp_emu::run_block(256, [&] { k_accum_dmma<PCLB200_EST_SVD>(a, match.data()); });
     warp_emu::run_block(32, [&] {
-      k_solve(accum.data(), estimator, scalar_double ? 1 : 0, tmode, (double)a.ox, (double)a.oy, (double)a.oz, 3, &pending, &solve_out,
+      k_solve(accum.data(), estimator, scalar_double ? 1 : 0, tmode, a.origin, 3, &pending, &solve_out,
               svd_correlation ? 1 : 0, &ctrl, crit);
     });
     skipped_total = (long)skip_count;
@@ -403,7 +407,8 @@ static void run_estimators(std::mt19937& rng)
     pa.pub.partials = partials.data();
     pa.pub.counter = &counter;
     pa.pub.accum = accum.data();
-    if (est == PCLB200_EST_SVD) { pa.ox = tgt[0].x; pa.oy = tgt[0].y; pa.oz = tgt[0].z; }
+    float o[3] = {0.f, 0.f, 0.f};   // icp.cu: estimate_pairs
+    if (est == PCLB200_EST_SVD) { k_seed_origin(tgt.data(), pa.corr, pa.n, o); pa.ox = o[0]; pa.oy = o[1]; pa.oz = o[2]; }
     blockDim.x = 256;
     counter = 0;
     if (est == PCLB200_EST_SVD) warp_emu::run_block(256, [&] { k_accum_pairs<PCLB200_EST_SVD>(pa); });
@@ -412,7 +417,7 @@ static void run_estimators(std::mt19937& rng)
     SolveOut so;
     std::memset(&so, 0, sizeof so);
     warp_emu::run_block(32, [&] {
-      k_solve(accum.data(), est, scalar_double ? 1 : 0, 0, (double)pa.ox, (double)pa.oy, (double)pa.oz, 1, nullptr, &so, correlation ? 1 : 0, nullptr, CritParams{});
+      k_solve(accum.data(), est, scalar_double ? 1 : 0, 0, est == PCLB200_EST_SVD ? o : nullptr, 1, nullptr, &so, correlation ? 1 : 0, nullptr, CritParams{});
     });
     for (int i = 0; i < 16; ++i) T[i] = so.T[i];
   };
@@ -523,6 +528,41 @@ int main()
   const double t2[3] = {0.4, 0.3, -0.2};
   surface(3000, B, 900, 4.0, t2);
   run_align("SVD float, tight gate (few pairs)", B, PCLB200_EST_SVD, false, 0.02, 1e-9, 10, PCLB200_TRACK_OFF, false);
+  {
+    // a 10 cm object inside a sparse +-500 m map, 500 m from the map's centre: the SVD sums must be taken about an origin
+    // near the pairs, or sum(q-o)(p-o)^T / n - m_q m_p^T cancels (about 1e-6 in the rotation about the map's centre)
+    Scene F;
+    const int n_map = 3000, n_patch = 4000, n_src = 1500;
+    const double c0[3] = {400.0, -300.0, 5.0};
+    auto bump = [](double x, double y) { return 0.01 * std::sin(60.0 * x) * std::cos(45.0 * y); };
+    F.tgt.assign(8 * (std::size_t)(n_map + n_patch), 0.f);
+    for (int i = 0; i < n_map + n_patch; ++i) {
+      float* r = &F.tgt[8 * (std::size_t)i];
+      if (i < n_map) {
+        r[0] = 1000.f * U(rng) - 500.f; r[1] = 1000.f * U(rng) - 500.f; r[2] = 20.f * U(rng) - 10.f;
+      }
+      else {
+        const double x = 0.1 * U(rng), y = 0.1 * U(rng);
+        r[0] = (float)(c0[0] + x); r[1] = (float)(c0[1] + y); r[2] = (float)(c0[2] + bump(x, y));
+      }
+      r[3] = 1.f; r[6] = 1.f;
+    }
+    double R[9];
+    rot(0.3, 0.5, 1.0, 0.5, R);
+    const double ctr[3] = {c0[0] + 0.05, c0[1] + 0.05, c0[2]}, sh[3] = {0.001, -0.0005, 0.0007};
+    F.src.assign(4 * (std::size_t)n_src, 1.f);
+    F.src_n.assign(8 * (std::size_t)n_src, 0.f);
+    for (int i = 0; i < n_src; ++i) {
+      const double x = 0.01 + 0.08 * U(rng), y = 0.01 + 0.08 * U(rng);
+      const double d[3] = {c0[0] + x - ctr[0], c0[1] + y - ctr[1], c0[2] + bump(x, y) - ctr[2]};
+      for (int r = 0; r < 3; ++r) {
+        F.src[4 * (std::size_t)i + r] = (float)(ctr[r] + R[3 * r] * d[0] + R[3 * r + 1] * d[1] + R[3 * r + 2] * d[2] + sh[r]);
+        F.src_n[8 * (std::size_t)i + r] = F.src[4 * (std::size_t)i + r];
+      }
+      F.src_n[8 * (std::size_t)i + 3] = 1.f;
+    }
+    run_align("SVD double, 10 cm patch 500 m out", F, PCLB200_EST_SVD, true, 0.01, 1e-14, 15, PCLB200_TRACK_OFF, false);
+  }
   run_estimators(rng);
   std::printf("%ld checks, %ld failures\n%s\n", g_checks, g_fail, g_fail ? "FAILED" : "PASSED");
   return g_fail ? 1 : 0;

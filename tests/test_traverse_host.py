@@ -70,19 +70,21 @@ def test_warp_knn_kernel_on_an_emulated_warp(tmp_path, device_built):
 
 
 @pytest.mark.parametrize("device_built", [False, True], ids=["reference-index", "device-built-index"])
-def test_whole_icp_iterations_on_an_emulated_block(tmp_path, device_built):
+def test_whole_icp_iterations_about_the_svd_origin_on_an_emulated_block(tmp_path, device_built):
     """icp_kernels.cuh — k_search, k_accum_dmma (the m8n8k4 fp64 MMA emulated fragment by fragment), k_accum, k_solve with the
-    convergence criteria in its tail — on an emulated 256-thread block, driven like icp.cu's icp_iterate: every
-    iteration's correspondences equal brute force, the accumulated normal equations equal plain fp64 sums, and iterations /
+    convergence criteria in its tail, k_seed_origin — on an emulated 256-thread block, driven like icp.cu's icp_iterate
+    (the SVD sums about the loop's device-side origin, which k_solve moves every iteration): every iteration's
+    correspondences equal brute force, the accumulated normal equations equal plain fp64 sums, and iterations /
     state / counts / final transform of twelve aligns (SVD, point-to-plane, the symmetric objective, ICPWithNormals,
     reciprocal correspondences; float and double; gates; tracking off / on / automatic; rejector chains inside the loop —
     median + one-to-one, distance + trimmed, surface-normal + one-to-one; normal-shooting and back-projection
-    correspondences) equal the oracle's loop (1e-5 float, 1e-9 double); the four stand-alone estimators against the oracle's."""
+    correspondences; a 10 cm patch 500 m from the centre of its map) equal the oracle's loop (1e-5 float, 1e-9 double); the
+    four stand-alone estimators against the oracle's."""
     import oracle
     oracle.build()
     odir = os.path.join(ROOT, "oracle")
     out = _run(tmp_path, "icp_host_test.cpp", (), DEVICE_BUILD if device_built else (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
-    assert "tracking automatic" in out and "point-to-plane LLS double" in out and "reciprocal" in out and "trimmed rejectors" in out and "back-projection" in out
+    assert "tracking automatic" in out and "point-to-plane LLS double" in out and "reciprocal" in out and "trimmed rejectors" in out and "back-projection" in out and "500 m out" in out
 
 
 def test_voxelgrid_kernels_on_the_host(tmp_path):
