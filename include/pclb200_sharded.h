@@ -20,7 +20,8 @@ extern "C" {
  * index pclb200_index_build makes of that map with subset = ids.  Non-finite points are dropped as by pclb200_index_build.  ids (host or
  * device, n entries) must be distinct and lie in [0, 2^31 - 2], else PCLB200_ERR_INVALID.  What maps ids back to
  * records of the cloud an index was built from refuses a labelled index (PCLB200_ERR_INVALID): the normal-based
- * correspondence estimators, normal estimation with k > 32 or a radius, GICP covariances, pclb200_cluster_labels. */
+ * correspondence estimators, normal estimation with k > 32 or a radius, GICP covariances, pclb200_cluster_labels.
+ * The normals of a sharded map come from pclb200_normals_knn_sharded / pclb200_normals_radius_sharded. */
 PCLB200_API int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                         const int32_t* ids, pclb200_index** out);
 
@@ -46,6 +47,22 @@ PCLB200_API int pclb200_fitness_score_sharded(pclb200_ctx* ctx, const pclb200_in
                                               const int32_t* src_indices, size_t n_idx, int is_dense,
                                               const double T[16], int scalar_is_double, double max_range,
                                               double* score);
+
+/* Collective over the context's communicator: every rank passes its tile (built with pclb200_index_build_ids) and its
+ * OWN queries (any points; typically the tile's records).  out[i] is, bit for bit, what pclb200_normals_knn /
+ * pclb200_normals_radius returns for query i against one index of the whole map (the union of the tiles' ids),
+ * including NaN rows; *is_dense_out covers this rank's queries.  Arrays, strides, indices and out follow
+ * pclb200_normals_knn; a rank with no queries still takes part.  Each rank fetches, from the other ranks' tiles, the
+ * points within its queries' k-th nearest distance in its own tile (or the radius) and indexes its tile plus those points:
+ * both are resident at the peak.  An id held by two ranks must name the same point.  PCLB200_ERR_INVALID on every rank,
+ * before any exchange, without an active communicator, for a tile built without ids, and for k <= 0 / radius <= 0. */
+PCLB200_API int pclb200_normals_knn_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n,
+                                            size_t stride, const int32_t* indices, size_t n_idx, int is_dense, int k,
+                                            const float viewpoint[3], float* out, int* is_dense_out);
+PCLB200_API int pclb200_normals_radius_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts,
+                                               size_t n, size_t stride, const int32_t* indices, size_t n_idx,
+                                               int is_dense, double radius, const float viewpoint[3], float* out,
+                                               int* is_dense_out);
 
 #ifdef __cplusplus
 }

@@ -78,7 +78,8 @@ SYMBOLS = [
     "pclb200_comm_init",
 ]
 # every symbol include/pclb200_sharded.h declares (the sharded-target extension; tests/test_sharded_target_symbols.py)
-SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", "pclb200_fitness_score_sharded"]
+SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", "pclb200_fitness_score_sharded",
+                   "pclb200_normals_knn_sharded", "pclb200_normals_radius_sharded"]
 
 _lib = None
 
@@ -139,6 +140,8 @@ def lib():
     L.pclb200_fitness_score_sharded.argtypes = [vp, vp, vp, sz, sz, vp, sz, C.c_int, dp, C.c_int, C.c_double, dp]
     L.pclb200_normals_knn.argtypes = [vp, vp, vp, sz, sz, vp, sz, C.c_int, C.c_int, fp, vp, C.POINTER(C.c_int)]
     L.pclb200_normals_radius.argtypes = [vp, vp, vp, sz, sz, vp, sz, C.c_int, C.c_double, fp, vp, C.POINTER(C.c_int)]
+    L.pclb200_normals_knn_sharded.argtypes = L.pclb200_normals_knn.argtypes
+    L.pclb200_normals_radius_sharded.argtypes = L.pclb200_normals_radius.argtypes
     L.pclb200_correspondences_normals.argtypes = [vp, vp, C.c_int, vp, sz, sz, vp, sz, vp, sz, vp, sz, C.c_int, C.c_double,
                                                   vp, C.POINTER(sz)]
     L.pclb200_reject_surface_normal.argtypes = [vp, vp, sz, vp, sz, sz, vp, sz, sz, C.c_double, vp, C.POINTER(sz)]
@@ -602,6 +605,29 @@ class Index:
         _check(lib().pclb200_normals_radius(self.ctx.h, self.h, b.ptr, b.rows, b.stride, ib.ptr, ib.rows, int(is_dense),
                                             float(radius), vp, ob.ptr, C.byref(dense)))
         return out, bool(dense.value)
+
+    def _normals_sharded(self, fn, cloud, param, viewpoint, indices, is_dense, out):
+        b = _Buf(cloud)
+        ib = _Buf(indices, np.int32)
+        n = ib.rows if indices is not None else b.rows
+        if out is None:
+            out = np.empty((n, 4), dtype=np.float32)
+        ob = _Buf(out)
+        vp = (C.c_float * 3)(*[float(v) for v in viewpoint])
+        dense = C.c_int()
+        _check(fn(self.ctx.h, self.h, b.ptr, b.rows, b.stride, ib.ptr, ib.rows, int(is_dense), param, vp, ob.ptr,
+                  C.byref(dense)))
+        return out, bool(dense.value)
+
+    def normals_knn_sharded(self, cloud, k, viewpoint=(0, 0, 0), indices=None, is_dense=True, out=None):
+        """Collective normals_knn over a map sharded across the communicator's ranks (this index = this rank's tile,
+        built with ids=...; cloud = this rank's own queries): bit for bit one index of the whole map's answer."""
+        return self._normals_sharded(lib().pclb200_normals_knn_sharded, cloud, int(k), viewpoint, indices, is_dense, out)
+
+    def normals_radius_sharded(self, cloud, radius, viewpoint=(0, 0, 0), indices=None, is_dense=True, out=None):
+        """Collective normals_radius over a map sharded across the communicator's ranks (see normals_knn_sharded)."""
+        return self._normals_sharded(lib().pclb200_normals_radius_sharded, cloud, float(radius), viewpoint, indices,
+                                     is_dense, out)
 
 
 def clusters_from_labels(labels, min_size=1, max_size=2 ** 32 - 1):

@@ -47,6 +47,7 @@ void comm_import(Ctx& c, int rank, int nranks, const void* handles);
 void comm_set_mode(Ctx& c, int mode);
 void comm_init(Ctx& c, int rank, int nranks, const void* unique_id);
 void comm_destroy(Ctx& c);
+bool comm_active(const Ctx& c);
 
 static thread_local std::string g_last_error;
 
@@ -154,6 +155,25 @@ static void normals(Ctx& c, const Index& idx, const void* pts, size_t n, size_t 
   check_device_error(c);
   if (is_dense_out)
     *is_dense_out = flag ? 0 : 1;
+}
+
+// Shared body of pclb200_normals_knn_sharded / _radius_sharded (collective): the caller's queries staged once, the local
+// map of this rank (shard_normals.cu: its tile plus the halo its queries need), then the single-GPU normals on that map.
+template <typename Launch>
+static void normals_sharded(Ctx& c, const Index& tile, const void* pts, size_t n, size_t stride, const int32_t* indices,
+                            size_t n_idx, int k, float r2, float* out, int* is_dense_out, Launch&& launch)
+{
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+               "sharded normals need an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
+  PCLB_REQUIRE(tile.labelled, PCLB200_ERR_INVALID,
+               "sharded normals: every rank's tile must be built with pclb200_index_build_ids");
+  const size_t nq = indices ? n_idx : n;
+  DevBuf<float4> dense;
+  dense.alloc(nq, c.stream);
+  load_xyz_as_float4(c, pts, n, stride, indices, n_idx, dense.p, c.stream);
+  std::unique_ptr<Index> local(sharded_normals_map(c, tile, dense.p, nq, k, r2));
+  normals(c, *local, dense.p, nq, sizeof(float4), nullptr, 0, out, is_dense_out,
+          [&](const float4* d_q, size_t m, float4* d_out, int* d_flag) { launch(*local, d_q, m, d_out, d_flag); });
 }
 
 extern "C" {
@@ -784,6 +804,37 @@ int pclb200_normals_radius(pclb200_ctx* ctx, const pclb200_index* h, const void*
             [&](const float4* d_q, size_t nq, float4* d_out, int* d_flag) {
               launch_normals_radius(c, *h->idx, d_q, nq, (float)(radius * radius), viewpoint, d_out, d_flag);
             });
+  });
+}
+
+int pclb200_normals_knn_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n, size_t stride,
+                                const int32_t* indices, size_t n_idx, int is_dense, int k, const float viewpoint[3],
+                                float* out, int* is_dense_out)
+{
+  (void)is_dense;
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && out && viewpoint, PCLB200_ERR_INVALID, "NULL argument");
+    PCLB_REQUIRE(k > 0, PCLB200_ERR_INVALID, "k must be positive (feature.hpp:135-176)");
+    normals_sharded(c, *idx_tile->idx, pts, n, stride, indices, n_idx, k, 0.f, out, is_dense_out,
+                    [&](Index& local, const float4* d_q, size_t nq, float4* d_out, int* d_flag) {
+                      launch_normals(c, local, d_q, nq, k, viewpoint, d_out, d_flag);
+                    });
+  });
+}
+
+int pclb200_normals_radius_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n,
+                                   size_t stride, const int32_t* indices, size_t n_idx, int is_dense, double radius,
+                                   const float viewpoint[3], float* out, int* is_dense_out)
+{
+  (void)is_dense;
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && out && viewpoint, PCLB200_ERR_INVALID, "NULL argument");
+    PCLB_REQUIRE(radius > 0.0, PCLB200_ERR_INVALID, "radius must be positive (feature.hpp:135-176)");
+    const float r2 = (float)(radius * radius);
+    normals_sharded(c, *idx_tile->idx, pts, n, stride, indices, n_idx, 0, r2, out, is_dense_out,
+                    [&](Index& local, const float4* d_q, size_t nq, float4* d_out, int* d_flag) {
+                      launch_normals_radius(c, local, d_q, nq, r2, viewpoint, d_out, d_flag);
+                    });
   });
 }
 

@@ -308,6 +308,8 @@ bool comm_active(const Ctx& c) { return c.comm && c.comm->nranks > 1; }
 
 int comm_nranks(const Ctx& c) { return comm_active(c) ? c.comm->nranks : 1; }
 
+int comm_rank(const Ctx& c) { return comm_active(c) ? c.comm->rank : 0; }
+
 bool comm_peer_fused(const Ctx& c) { return comm_active(c) && c.comm->peer_ok && c.comm->mode == PCLB200_REDUCE_FUSED; }
 
 // view + next sequence number for a fused in-kernel exchange; returns false when the NCCL path must be used

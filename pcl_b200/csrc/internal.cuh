@@ -252,8 +252,15 @@ struct Index {
 Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* subset, size_t n_subset);
 // point i labelled ids[i] (non-negative, distinct, < 2^31 - 1) instead of i: one tile of a map sharded across ranks
 Index* build_index_ids(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* ids);
-// device-resident source already dense float4 (w ignored): used for the reciprocal source tree
-Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig /*nullable*/);
+// device-resident source already dense float4 (w ignored): used for the reciprocal source tree (rebuilt every iteration:
+// no cell table) and for the local map of normals over a sharded map (shard_normals.cu: with the cell table)
+Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig /*nullable*/,
+                               bool cell_table = false);
+// The local map of normal estimation over a map sharded across the communicator's ranks (collective): this rank's tile
+// (labelled) plus every point of the other tiles that can be a neighbour of one of the dense queries d_q[0..nq) on the
+// whole map, sorted by id and indexed as an ordinary index (record i = the i-th smallest id).  k > 0: the k nearest; else
+// the radius neighbours of r2.
+Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2);
 void ensure_pos_of_orig(Ctx& c, Index& idx);
 
 // Morton-ordered batch of query points (dense float4 xyz + original slot), so neighbouring threads
@@ -310,6 +317,9 @@ void launch_normals(Ctx& c, Index& idx, const float4* d_q, size_t nq, int k, con
 void launch_normals_radius(Ctx& c, Index& idx, const float4* d_q, size_t nq, float r2, const float vp[3], float4* d_out,
                            int* d_not_dense);
 void launch_knn_stats(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_mean, float* d_kth);
+// launch_knn_stats's d_kth through materialised k-NN lists (nq * k entries of scratch), whatever k: the warp-cooperative
+// search answers k = 12..32 on an index with a cell table, much faster than the per-thread statistics kernel
+void launch_knn_kth(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_kth);
 // correspondences chosen among the k nearest with the help of normals; surface-normal rejector (normals_corr.cu)
 size_t correspondences_by_normals(Ctx& c, Index& tgt, int kind, const void* src, size_t n, size_t stride,
                                   const void* src_normals, size_t stride_sn, const void* tgt_normals, size_t stride_tn,

@@ -308,9 +308,9 @@ Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32
   return build_from_dense(c, dense.p, cnt, on_device(c, subset, n_subset, d_sub), n, true);
 }
 
-Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig)
+Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig, bool cell_table)
 {
-  return build_from_dense(c, d_pts, n, d_orig, n, false);  // rebuilt every reciprocal iteration: no cell table
+  return build_from_dense(c, d_pts, n, d_orig, n, cell_table);
 }
 
 // ---- labelled index: one tile of a map, its points carrying the caller's ids -------------------------------------

@@ -54,23 +54,35 @@ void launch_knn(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, f
   PCLB_CUDA(cudaGetLastError());
 }
 
+// exact lists first (launch_knn: the warp-cooperative search where it applies), folded afterwards.  NaN queries get empty
+// rows from the walk (no box is ever within a NaN bound) and are zeroed by the fold.
+static void knn_stats_from_lists(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_mean, float* d_kth)
+{
+  cudaStream_t s = c.stream;
+  DevBuf<int32_t> li;
+  DevBuf<float> ld;
+  li.alloc(nq * (size_t)k, s);
+  ld.alloc(nq * (size_t)k, s);
+  launch_knn(c, idx, d_q, nq, k, __builtin_inff(), li.p, ld.p);
+  k_stats_from_lists<<<grid_for(nq, 256), 256, 0, s>>>(d_q, nq, k, li.p, ld.p, d_mean, d_kth);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
+void launch_knn_kth(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_kth)
+{
+  if (nq && k > 0)
+    knn_stats_from_lists(c, idx, d_q, nq, k, nullptr, d_kth);
+}
+
 void launch_knn_stats(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_mean, float* d_kth)
 {
   if (!nq || k <= 0)
     return;
   cudaStream_t s = c.stream;
   const unsigned g = grid_for(nq, 128);
-  if (k > 32) {
-    // large neighbourhoods (StatisticalOutlierRemoval's usual mean_k = 50): exact lists first, folded afterwards.
-    // NaN queries get empty rows from the walk (no box is ever within a NaN bound) and are zeroed by the fold.
-    DevBuf<int32_t> li;
-    DevBuf<float> ld;
-    li.alloc(nq * (size_t)k, s);
-    ld.alloc(nq * (size_t)k, s);
-    launch_knn(c, idx, d_q, nq, k, __builtin_inff(), li.p, ld.p);
-    k_stats_from_lists<<<grid_for(nq, 256), 256, 0, s>>>(d_q, nq, k, li.p, ld.p, d_mean, d_kth);
-    ++c.launches;
-    PCLB_CUDA(cudaGetLastError());
+  if (k > 32) {  // large neighbourhoods (StatisticalOutlierRemoval's usual mean_k = 50)
+    knn_stats_from_lists(c, idx, d_q, nq, k, d_mean, d_kth);
     return;
   }
 #define PCLB_STAT_CASE(KK) \
