@@ -21,7 +21,8 @@ extern "C" {
  * device, n entries) must be distinct and lie in [0, 2^31 - 2], else PCLB200_ERR_INVALID.  What maps ids back to
  * records of the cloud an index was built from refuses a labelled index (PCLB200_ERR_INVALID): the normal-based
  * correspondence estimators, normal estimation with k > 32 or a radius, GICP covariances, pclb200_cluster_labels.
- * The normals of a sharded map come from pclb200_normals_knn_sharded / pclb200_normals_radius_sharded. */
+ * The normals of a sharded map come from pclb200_normals_knn_sharded / pclb200_normals_radius_sharded, and the clusters
+ * of a sharded map come from pclb200_cluster_labels_sharded. */
 PCLB200_API int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                         const int32_t* ids, pclb200_index** out);
 
@@ -63,6 +64,28 @@ PCLB200_API int pclb200_normals_radius_sharded(pclb200_ctx* ctx, const pclb200_i
                                                size_t n, size_t stride, const int32_t* indices, size_t n_idx,
                                                int is_dense, double radius, const float viewpoint[3], float* out,
                                                int* is_dense_out);
+
+/* Euclidean clustering of a map sharded across the ranks of the context's communicator (collective: every rank passes its
+ * tile, built with pclb200_index_build_ids; the whole map is the union of the tiles' ids).  n_labels is the number of
+ * records the tile was built from.  out_labels[i] is, byte for byte, what pclb200_cluster_labels returns at ids[i] for one
+ * index of the whole map: the smallest id of the record's component of the d2 < tolerance^2 graph (tolerance narrowed to
+ * float as there), -1 for a non-finite record.  out_sizes (nullable) receives the number of distinct ids in that
+ * component on the whole map (what EuclideanClusterExtraction's min / max cluster size compare), 0 for a non-finite
+ * record.  Both may be host or device memory.  An id held by two ranks must name the same point; it gets the same label
+ * on both and counts once.  Each rank fetches the other tiles' points within the tolerance of its tile's box, clusters
+ * its tile plus those points, and one exchange of labels along that halo stitches components across any number of tiles;
+ * tile and halo are resident at the peak.  PCLB200_ERR_INVALID on every rank, before any exchange, without an active
+ * communicator, for a tile built without ids, for a negative tolerance and for n_labels other than the tile's records. */
+PCLB200_API int pclb200_cluster_labels_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, double tolerance,
+                                               int32_t* out_labels, int64_t* out_sizes, size_t n_labels);
+
+/* Collective over the context's communicator: every rank's send[0..n) concatenated in rank order, the same on every
+ * rank.  *n_total is the total; recv (host or device, nullable) receives it when capacity >= *n_total, else nothing is
+ * written there (every rank sees the same total, so all of them can call again with room).  It lets every rank learn,
+ * for instance, the (size, label) pairs of every cluster pclb200_cluster_labels_sharded found on the other ranks.
+ * PCLB200_ERR_INVALID on every rank without an active communicator. */
+PCLB200_API int pclb200_comm_allgather_u64(pclb200_ctx* ctx, const uint64_t* send, size_t n, uint64_t* recv,
+                                           size_t capacity, size_t* n_total);
 
 #ifdef __cplusplus
 }

@@ -79,7 +79,8 @@ SYMBOLS = [
 ]
 # every symbol include/pclb200_sharded.h declares (the sharded-target extension; tests/test_sharded_target_symbols.py)
 SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", "pclb200_fitness_score_sharded",
-                   "pclb200_normals_knn_sharded", "pclb200_normals_radius_sharded"]
+                   "pclb200_normals_knn_sharded", "pclb200_normals_radius_sharded", "pclb200_cluster_labels_sharded",
+                   "pclb200_comm_allgather_u64"]
 
 _lib = None
 
@@ -146,6 +147,8 @@ def lib():
                                                   vp, C.POINTER(sz)]
     L.pclb200_reject_surface_normal.argtypes = [vp, vp, sz, vp, sz, sz, vp, sz, sz, C.c_double, vp, C.POINTER(sz)]
     L.pclb200_cluster_labels.argtypes = [vp, vp, C.c_double, vp, sz]
+    L.pclb200_cluster_labels_sharded.argtypes = [vp, vp, C.c_double, vp, vp, sz]
+    L.pclb200_comm_allgather_u64.argtypes = [vp, vp, sz, vp, sz, C.POINTER(sz)]
     L.pclb200_voxelgrid.argtypes = [vp, vp, sz, sz, vp, sz, C.c_int, fp, C.c_uint, vp, C.POINTER(sz)]
     L.pclb200_voxelgrid_tile.argtypes = [vp, vp, sz, sz, fp, fp, C.c_uint, vp, C.POINTER(sz)]
     L.pclb200_voxelgrid_normals.argtypes = [vp, vp, sz, sz, vp, sz, vp, sz, C.c_int, fp, C.c_uint, vp, vp, C.POINTER(sz)]
@@ -279,6 +282,16 @@ class Context:
 
     def comm_set_mode(self, mode):
         _check(lib().pclb200_comm_set_mode(self.h, int(mode)))
+
+    def allgather_u64(self, values):
+        """Collective: every rank's uint64 values concatenated in rank order (the same array on every rank)."""
+        v = np.ascontiguousarray(values, dtype=np.uint64)
+        total = C.c_size_t()
+        _check(lib().pclb200_comm_allgather_u64(self.h, C.c_void_p(v.ctypes.data), v.size, None, 0, C.byref(total)))
+        out = np.empty(max(total.value, 1), dtype=np.uint64)
+        _check(lib().pclb200_comm_allgather_u64(self.h, C.c_void_p(v.ctypes.data), v.size, C.c_void_p(out.ctypes.data),
+                                                out.size, C.byref(total)))
+        return out[:total.value]
 
     def comm_export(self):
         buf = C.create_string_buffer(64)
@@ -591,6 +604,38 @@ class Index:
         """EuclideanClusterExtraction::extract: list of index arrays (ascending inside a cluster), largest first,
         equal sizes ordered by their smallest index."""
         return clusters_from_labels(self.cluster_labels(tolerance), min_size, max_size)
+
+    def cluster_labels_sharded(self, tolerance, out=None, sizes=None):
+        """Collective cluster_labels over a map sharded across the communicator's ranks (this index = this rank's tile,
+        built with ids=...): (labels, sizes) per record of the tile.  labels[i] is the whole map's label of ids[i] (the
+        smallest id of its component, -1 for a non-finite record); sizes[i] the number of distinct ids in that component
+        (0 for a non-finite record).  out / sizes: numpy or torch, host or cuda."""
+        if out is None:
+            out = np.empty(self.n_cloud, dtype=np.int32)
+        if sizes is None:
+            sizes = np.empty(self.n_cloud, dtype=np.int64)
+        ob, sb = _Buf(out, np.int32), _Buf(sizes, np.int64)
+        _check(lib().pclb200_cluster_labels_sharded(self.ctx.h, self.h, float(tolerance), ob.ptr, sb.ptr, self.n_cloud))
+        return out, sizes
+
+    def euclidean_clusters_sharded(self, tolerance, ids, min_size=1, max_size=2 ** 32 - 1):
+        """Collective euclidean_clusters over a sharded map (ids: the ids this tile was built with).  This rank's part of
+        every whole-map cluster whose size is within [min_size, max_size], as ascending id arrays, in the order
+        euclidean_clusters gives the whole map (size descending, then smallest id).  Every rank returns a list of the
+        same length; a rank that holds no point of a cluster gets an empty array in its place, and an id held by two
+        ranks is in both ranks' parts."""
+        ids = np.asarray(ids, dtype=np.int64)
+        labels, sizes = self.cluster_labels_sharded(tolerance)
+        keep = (labels >= 0) & (sizes >= min_size) & (sizes <= max_size)
+        # (size << 32) | label of every cluster in the window, from every rank (sizes and labels are below 2^31)
+        mine = np.unique((sizes[keep].astype(np.uint64) << np.uint64(32)) | labels[keep].astype(np.uint64))
+        every = np.unique(self.ctx.allgather_u64(mine))
+        size, label = (every >> np.uint64(32)).astype(np.int64), (every & np.uint64(0xffffffff)).astype(np.int64)
+        label = label[np.lexsort((label, -size))]
+        order = np.lexsort((ids[keep], labels[keep]))  # this rank's records of the window by (label, id)
+        lab_sorted, id_sorted = labels[keep][order], ids[keep][order]
+        lo, hi = np.searchsorted(lab_sorted, label, "left"), np.searchsorted(lab_sorted, label, "right")
+        return [id_sorted[a:b].astype(np.int32) for a, b in zip(lo, hi)]
 
     def normals_radius(self, cloud, radius, viewpoint=(0, 0, 0), indices=None, is_dense=True, out=None):
         """NormalEstimation with setRadiusSearch(radius)."""

@@ -171,7 +171,8 @@ static void normals_sharded(Ctx& c, const Index& tile, const void* pts, size_t n
   DevBuf<float4> dense;
   dense.alloc(nq, c.stream);
   load_xyz_as_float4(c, pts, n, stride, indices, n_idx, dense.p, c.stream);
-  std::unique_ptr<Index> local(sharded_normals_map(c, tile, dense.p, nq, k, r2));
+  static const ShardedMapStages stages{"sharded_normals_bound", "sharded_normals_halo", "sharded_normals_build"};
+  std::unique_ptr<Index> local(sharded_local_map(c, tile, dense.p, nq, k, r2, stages));
   normals(c, *local, dense.p, nq, sizeof(float4), nullptr, 0, out, is_dense_out,
           [&](const float4* d_q, size_t m, float4* d_out, int* d_flag) { launch(*local, d_q, m, d_out, d_flag); });
 }
@@ -853,6 +854,46 @@ int pclb200_cluster_labels(pclb200_ctx* ctx, const pclb200_index* h, double tole
     cluster_labels(c, idx, tolerance, out_on_device(c, out_labels, n_labels, tmp));
     copy_out(c, out_labels, tmp, n_labels);
     check_device_error(c);
+  });
+}
+
+int pclb200_cluster_labels_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, double tolerance, int32_t* out_labels,
+                                   int64_t* out_sizes, size_t n_labels)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && out_labels, PCLB200_ERR_INVALID, "NULL argument");
+    PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+                 "sharded clusters need an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
+    const Index& tile = *idx_tile->idx;
+    PCLB_REQUIRE(tile.labelled, PCLB200_ERR_INVALID,
+                 "sharded clusters: every rank's tile must be built with pclb200_index_build_ids");
+    PCLB_REQUIRE(tolerance >= 0.0, PCLB200_ERR_INVALID, "negative cluster tolerance");
+    PCLB_REQUIRE(n_labels == tile.n_cloud, PCLB200_ERR_INVALID,
+                 "out_labels must hold one entry per record the tile was built from");
+    DevBuf<int32_t> tmp;
+    DevBuf<int64_t> tmp_sizes;
+    cluster_labels_sharded(c, tile, tolerance, out_on_device(c, out_labels, n_labels, tmp),
+                           out_on_device(c, out_sizes, n_labels, tmp_sizes));
+    copy_out(c, out_labels, tmp, n_labels);
+    copy_out(c, out_sizes, tmp_sizes, n_labels);
+    check_device_error(c);
+  });
+}
+
+int pclb200_comm_allgather_u64(pclb200_ctx* ctx, const uint64_t* send, size_t n, uint64_t* recv, size_t capacity,
+                               size_t* n_total)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(n_total && (send || !n), PCLB200_ERR_INVALID, "NULL argument");
+    PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+                 "allgather needs an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
+    DevBuf<unsigned long long> staging, all;
+    const unsigned long long* d = on_device(c, reinterpret_cast<const unsigned long long*>(send), n, staging);
+    const size_t total = allgather_u64(c, d, n, all);
+    if (recv && total && capacity >= total)
+      PCLB_CUDA(cudaMemcpyAsync(recv, all.p, total * sizeof(uint64_t), cudaMemcpyDefault, c.stream));
+    check_device_error(c);
+    *n_total = total;
   });
 }
 

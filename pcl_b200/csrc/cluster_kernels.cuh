@@ -3,38 +3,9 @@
 #pragma once
 #include "internal.cuh"
 #include "traverse.cuh"
+#include "union_find.cuh"
 
 namespace pclb200 {
-
-__device__ __forceinline__ int cc_find(int* parent, int x)
-{
-  volatile int* vp = parent;
-  int cur = x;
-  while (true) {
-    const int p = vp[cur];
-    if (p == cur)
-      return cur;
-    const int gp = vp[p];
-    if (gp != p)
-      vp[cur] = gp;  // path halving: gp was an ancestor of cur and stays one (roots never become roots again)
-    cur = p;
-  }
-}
-
-__device__ __forceinline__ void cc_unite(int* parent, int a, int b)
-{
-  while (true) {
-    a = cc_find(parent, a);
-    b = cc_find(parent, b);
-    if (a == b)
-      return;
-    const int hi = a > b ? a : b, lo = a > b ? b : a;
-    if (atomicCAS(parent + hi, hi, lo) == hi)
-      return;
-    a = hi;  // somebody hooked `hi` first: start again from the new roots
-    b = lo;
-  }
-}
 
 struct UnionVisitor {
   float qx, qy, qz, r2, r2_below;

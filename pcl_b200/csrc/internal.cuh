@@ -253,14 +253,28 @@ Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32
 // point i labelled ids[i] (non-negative, distinct, < 2^31 - 1) instead of i: one tile of a map sharded across ranks
 Index* build_index_ids(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* ids);
 // device-resident source already dense float4 (w ignored): used for the reciprocal source tree (rebuilt every iteration:
-// no cell table) and for the local map of normals over a sharded map (shard_normals.cu: with the cell table)
+// no cell table) and for the local map of a sharded map (shard_normals.cu: with the cell table)
 Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig /*nullable*/,
                                bool cell_table = false);
-// The local map of normal estimation over a map sharded across the communicator's ranks (collective): this rank's tile
+// The local map of a map sharded across the communicator's ranks (collective, shard_normals.cu): this rank's tile
 // (labelled) plus every point of the other tiles that can be a neighbour of one of the dense queries d_q[0..nq) on the
 // whole map, sorted by id and indexed as an ordinary index (record i = the i-th smallest id).  k > 0: the k nearest; else
-// the radius neighbours of r2.
-Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2);
+// every point within d2 <= r2 (normals: the radius neighbours; clusters: the tile's points as queries, every edge).
+// stages names the ProfScopes; trace (nullable) receives what the halo exchange moved, for a caller that answers back
+// along it (shard_cluster.cu).
+struct ShardedMapStages {
+  const char* bound;  // the k-th distance bound (k > 0)
+  const char* halo;   // boxes and halo exchange
+  const char* build;  // sort by id and index
+};
+struct HaloTrace {
+  std::vector<unsigned long long> cnt;  // R x R: cnt[s R + r] = points rank s sent to rank r (s == r: its whole tile)
+  DevBuf<unsigned> local_ids;           // the local map's ids by record (ascending, each once; the first n_cloud)
+  DevBuf<unsigned> recv_ids;            // the received points' ids: by sender, each sender's segment in its order
+  DevBuf<unsigned> sent_ids;            // the ids this rank sent: by destination, each segment in the order it wrote it
+};
+Index* sharded_local_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2,
+                         const ShardedMapStages& stages, HaloTrace* trace = nullptr);
 void ensure_pos_of_orig(Ctx& c, Index& idx);
 
 // Morton-ordered batch of query points (dense float4 xyz + original slot), so neighbouring threads
@@ -330,6 +344,12 @@ size_t reject_surface_normal(Ctx& c, const pclb200_corr* in, size_t n, const voi
 
 // connected components of the d2 < tolerance^2 graph over the indexed points (cluster.cu)
 void cluster_labels(Ctx& c, const Index& idx, double tolerance, int32_t* d_labels /* idx.n_cloud */);
+// the same over a map sharded across the communicator's ranks (collective, shard_cluster.cu): labels and, when d_sizes is
+// not null, component sizes of the tile's records (tile.n_cloud entries each, on the device)
+void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t* d_labels, int64_t* d_sizes);
+// every rank's d_send[0..n) concatenated in rank order, identically on every rank (collective, shard_cluster.cu: the
+// count exchange, then comm_scratch_tables); returns the total
+size_t allgather_u64(Ctx& c, const unsigned long long* d_send, size_t n, DevBuf<unsigned long long>& out);
 
 // flat per-correspondence arrays the rejectors work on (reject.cu)
 struct RejectArrays {

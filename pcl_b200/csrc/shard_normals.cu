@@ -1,7 +1,9 @@
 // shard_normals.cu — normal estimation over a map sharded across the ranks of a communicator (pclb200_normals_knn_sharded /
 // _radius_sharded, capi.cu).  Each rank gathers, for its own queries, a halo out of the other ranks' tiles that provably
 // holds every whole-map neighbour of every query, indexes its tile plus that halo as an ordinary index sorted by id, and
-// runs the unchanged single-GPU normals on it (DESIGN.md §5, "Normals of a sharded map").
+// runs the unchanged single-GPU normals on it (DESIGN.md §5, "Normals of a sharded map").  Clustering a sharded map
+// (shard_cluster.cu) builds its local map here too, with the tile's points as the queries and the tolerance as the radius,
+// and takes a HaloTrace of the exchange so that it can answer every received point back to its sender.
 //
 //   bound   rho_q^2 = the k-th nearest squared distance of q in this rank's tile (launch_knn_kth; +inf when the tile
 //           holds fewer than k points), or r^2.  The tile is part of the map, so every member of q's whole-map list,
@@ -40,18 +42,18 @@ static unsigned persistent_blocks(const Ctx& c, size_t n)
 
 // Steps bound and boxes: every rank's box, on the device (kHaloBoxWords keys per rank, folded over the ranks)
 static void exchange_boxes(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2, int R, int me,
-                           DevBuf<unsigned long long>& boxes)
+                           const ShardedMapStages& stages, DevBuf<unsigned long long>& boxes)
 {
   cudaStream_t st = c.stream;
   DevBuf<float> rho2;
   if (k > 0 && nq) {
-    ProfScope ps(c, "sharded_normals_bound");
+    ProfScope ps(c, stages.bound);
     QueryBatch qb;
     make_query_batch(c, tile, d_q, nq, qb);
     rho2.alloc(nq, st);
     launch_knn_kth(c, tile, qb.q.p, nq, k, rho2.p);  // by slot = by dense position
   }
-  ProfScope ps(c, "sharded_normals_halo");
+  ProfScope ps(c, stages.halo);
   boxes.alloc((size_t)kHaloBoxWords * R, st);
   PCLB_CUDA(cudaMemsetAsync(boxes.p, 0xff, boxes.bytes(), st));
   if (nq) {
@@ -62,19 +64,20 @@ static void exchange_boxes(Ctx& c, const Index& tile, const float4* d_q, size_t 
   comm_allreduce_u64(c, boxes.p, boxes.p, boxes.n, kU64Min);
 }
 
-Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2)
+Index* sharded_local_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2,
+                         const ShardedMapStages& stages, HaloTrace* trace)
 {
   cudaStream_t st = c.stream;
-  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID, "sharded normals need an active communicator");
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID, "the local map of a sharded map needs an active communicator");
   const int R = comm_nranks(c), me = comm_rank(c);
   DevBuf<unsigned long long> boxes;
-  exchange_boxes(c, tile, d_q, nq, k, r2, R, me, boxes);
+  exchange_boxes(c, tile, d_q, nq, k, r2, R, me, stages, boxes);
 
   // the halo: counts of every (source, destination) pair on every rank, then the points
   DevBuf<float4> local;  // tile, then halo
   size_t n_local = 0;
   {
-    ProfScope ps(c, "sharded_normals_halo");
+    ProfScope ps(c, stages.halo);
     const size_t np = tile.pts.n;
     DevBuf<unsigned long long> d_cnt, cursor;
     d_cnt.alloc((size_t)R * R, st);
@@ -156,6 +159,28 @@ Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t 
     k_halo_select<<<persistent_blocks(c, np), 256, 0, st>>>(tile.pts.p, np, boxes.p, R, me, out);
     ++c.launches;
     PCLB_CUDA(cudaGetLastError());
+    if (trace) {
+      trace->cnt = cnt;
+      unsigned long long n_sent = 0;
+      HaloReadSet own;  // this rank's segments, by destination, before any rank rewrites its table
+      memset(&own, 0, sizeof(own));
+      for (int r = 0; r < R; ++r)
+        if (r != me) {
+          own.src[own.n] = out.dst[r];
+          own.begin[own.n + 1] = own.begin[own.n] + sent(me, r);
+          ++own.n;
+          n_sent += sent(me, r);
+        }
+      trace->sent_ids.alloc(n_sent, st);
+      if (n_sent) {
+        DevBuf<float4> copy;
+        copy.alloc(n_sent, st);
+        k_halo_gather<<<persistent_blocks(c, n_sent), 256, 0, st>>>(own, copy.p);
+        k_halo_ids<<<grid_for(n_sent, 256), 256, 0, st>>>(copy.p, n_sent, trace->sent_ids.p);
+        c.launches += 2;
+        PCLB_CUDA(cudaGetLastError());
+      }
+    }
     if (all) {
       if (t.peer)
         comm_barrier(c);
@@ -172,7 +197,7 @@ Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t 
   }
 
   // the local map: sorted by id, each id once, indexed
-  ProfScope ps(c, "sharded_normals_build");
+  ProfScope ps(c, stages.build);
   DevBuf<unsigned> ids, ids_sorted, ids_unique;
   DevBuf<float4> sorted, uniq;
   DevBuf<int> d_m;
@@ -184,6 +209,13 @@ Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t 
   d_m.alloc(1, st);
   k_halo_ids<<<grid_for(n_local, 256), 256, 0, st>>>(local.p, n_local, ids.p);
   ++c.launches;
+  const size_t n_tile = tile.n_valid;
+  if (trace) {
+    trace->recv_ids.alloc(n_local - n_tile, st);
+    if (n_local > n_tile)
+      PCLB_CUDA(cudaMemcpyAsync(trace->recv_ids.p, ids.p + n_tile, (n_local - n_tile) * sizeof(unsigned),
+                                cudaMemcpyDeviceToDevice, st));
+  }
   size_t tb = 0, tb2 = 0;
   PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, ids.p, ids_sorted.p, local.p, sorted.p, (int)n_local, 0, 31, st));
   PCLB_CUDA(cub::DeviceSelect::UniqueByKey(nullptr, tb2, ids_sorted.p, sorted.p, ids_unique.p, uniq.p, d_m.p, (int)n_local,
@@ -199,7 +231,10 @@ Index* sharded_normals_map(Ctx& c, const Index& tile, const float4* d_q, size_t 
   PCLB_CUDA(cudaStreamSynchronize(st));
   local.release();
   sorted.release();
-  return build_index_from_device(c, uniq.p, (size_t)m, nullptr, true);
+  Index* built = build_index_from_device(c, uniq.p, (size_t)m, nullptr, true);
+  if (trace)
+    trace->local_ids = std::move(ids_unique);
+  return built;
 }
 
 }  // namespace pclb200
