@@ -1,5 +1,4 @@
-// comm.cu — cross-GPU exchanges of a sharded source, and of a sharded target (icp.cu: the per-query keys and records of
-// exchange_shard_matches travel through comm_peer_tables, the same mapped tables as the one-to-one rejector's).
+// comm.cu — cross-GPU exchanges of a sharded source, and the tables of every exchange that moves whole arrays.
 //
 // The reference has no multi-GPU path.  Here the source cloud is sharded across ranks (one process per
 // GPU, target index replicated); every ICP iteration sums kAccum (= 40) doubles, issued on the same stream as the
@@ -8,6 +7,10 @@
 // (peer_exchange.cuh): the accumulators inside the accumulate kernels, the u64 collectives in k_peer_u64.  Without the
 // mappings they fall back to ncclAllReduce.  NCCL is bound at run time (dlopen of libnccl.so.2 — the copy torch
 // already loaded, if any) so the library has no link-time dependency and single-GPU users never touch it.
+//
+// Arrays too large for the exchange block (the one-to-one rejector's table, the sharded target's matches, the halo and
+// label answers of a sharded map, allgather_u64) go through PeerTables: one u64 table per rank, mapped into every rank,
+// with a barrier to publish and one to release; or, under NCCL, one all-reduce to publish (internal.cuh).
 #include <dlfcn.h>
 
 #include <algorithm>
@@ -16,6 +19,7 @@
 
 #include "internal.cuh"
 #include "peer_exchange.cuh"
+#include "peer_tables.cuh"
 
 namespace pclb200 {
 
@@ -69,8 +73,8 @@ enum { ncclMax = 2 };
 enum { ncclMin = 3 };
 
 // n u64 per rank, mapped into every rank: the one-to-one rejector table of one ICP session (reject.cu:
-// apply_rejector_sharded, ~0 between iterations) or the sharded-target exchange arrays (icp.cu)
-struct OneToOneEntry {
+// apply_rejector_sharded, ~0 between iterations), the sharded-target exchange arrays (icp.cu) or a communicator's scratch
+struct PeerTableEntry {
   unsigned long long comm_id = 0;       // the communicator it was made for
   int rank = 0, nranks = 0;
   size_t n = 0;
@@ -93,7 +97,7 @@ struct OneToOneEntry {
     mapped = false;
     comm_id = 0;
   }
-  ~OneToOneEntry() { release(); }
+  ~PeerTableEntry() { release(); }
 };
 
 struct Comm {
@@ -107,8 +111,8 @@ struct Comm {
   bool peer_ok = false;
   unsigned long long seq = 0;         // the last sequence number drawn (next_seq)
   unsigned long long id = 0;          // distinct per communicator made in this process
-  std::vector<std::weak_ptr<OneToOneEntry>> o2o;  // the sessions' peer tables made for this communicator
-  std::shared_ptr<OneToOneEntry> scratch;         // comm_scratch_tables
+  std::vector<std::weak_ptr<PeerTableEntry>> tables;  // the peer tables made for this communicator
+  std::shared_ptr<PeerTableEntry> scratch;            // comm_scratch_tables
   Comm();
 };
 
@@ -204,10 +208,10 @@ static void setup_peer_reduce(Ctx& c, Comm& cm)
 
 static void teardown_peer_reduce(Comm& cm)
 {
-  for (auto& w : cm.o2o)
+  for (auto& w : cm.tables)
     if (auto e = w.lock())
       e->release();
-  cm.o2o.clear();
+  cm.tables.clear();
   for (int p = 0; p < cm.nranks && p < kMaxRanks; ++p)
     if (p != cm.rank && cm.peer_block[p])
       cudaIpcCloseMemHandle(cm.peer_block[p]);
@@ -396,7 +400,7 @@ unsigned long long comm_shard_offset(Ctx& c, unsigned long long n_q, unsigned lo
 // Maps every rank's table into this process: the IPC handles travel through the u64 region (one exchange), then every
 // rank reports whether it could open all of them (a second one) so that all ranks take the same decision.  The caller
 // releases the table when this throws.
-static void map_one_to_one(Ctx& c, OneToOneEntry& e)
+static void map_peer_table(Ctx& c, PeerTableEntry& e)
 {
   Comm& cm = *c.comm;
   cudaStream_t st = c.stream;
@@ -419,12 +423,7 @@ static void map_one_to_one(Ctx& c, OneToOneEntry& e)
   e.mapped = true;
 }
 
-OneToOneTables comm_one_to_one_tables(Ctx& c, std::shared_ptr<OneToOneEntry>& owner, size_t n_cloud)
-{
-  return comm_peer_tables(c, owner, n_cloud);
-}
-
-OneToOneTables comm_scratch_tables(Ctx& c, size_t n_words)
+PeerTables comm_scratch_tables(Ctx& c, size_t n_words)
 {
   PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID, "no communicator");
   return comm_peer_tables(c, c.comm->scratch, n_words);
@@ -443,33 +442,35 @@ void comm_allreduce_u32_max(Ctx& c, const unsigned* d_send, unsigned* d_recv, si
   ++c.launches;
 }
 
-OneToOneTables comm_peer_tables(Ctx& c, std::shared_ptr<OneToOneEntry>& owner, size_t n_words)
+PeerTables comm_peer_tables(Ctx& c, std::shared_ptr<PeerTableEntry>& owner, size_t n_words)
 {
   PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID, "no communicator");
   Comm& cm = *c.comm;
   if (!owner)
-    owner = std::make_shared<OneToOneEntry>();
-  OneToOneEntry* e = owner.get();
+    owner = std::make_shared<PeerTableEntry>();
+  PeerTableEntry* e = owner.get();
   const size_t n = std::max<size_t>(n_words, 1);
-  if (e->local && (e->n != n || e->comm_id != cm.id))  // another target or another communicator: a new table
+  if (e->local && (e->n != n || e->comm_id != cm.id))  // another size or another communicator: a new table
     e->release();
   if (!e->local) {
     e->comm_id = cm.id;
     e->rank = cm.rank;
     e->nranks = cm.nranks;
     e->n = n;
-    cm.o2o.erase(std::remove_if(cm.o2o.begin(), cm.o2o.end(), [](const std::weak_ptr<OneToOneEntry>& w) { return w.expired(); }),
-                 cm.o2o.end());
-    cm.o2o.push_back(owner);
+    cm.tables.erase(std::remove_if(cm.tables.begin(), cm.tables.end(),
+                                   [](const std::weak_ptr<PeerTableEntry>& w) { return w.expired(); }),
+                    cm.tables.end());
+    cm.tables.push_back(owner);
     PCLB_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->local), n * sizeof(unsigned long long)));
     PCLB_CUDA(cudaMemsetAsync(e->local, 0xff, n * sizeof(unsigned long long), c.stream));
   }
-  OneToOneTables t;
+  PeerTables t;
   t.local = e->local;
+  t.words = n;
   if (comm_peer_fused(c)) {
     if (!e->mapped) {
       try {
-        map_one_to_one(c, *e);
+        map_peer_table(c, *e);
       }
       catch (const Error&) {
         e->release();
@@ -484,24 +485,71 @@ OneToOneTables comm_peer_tables(Ctx& c, std::shared_ptr<OneToOneEntry>& owner, s
   else {
     if (!e->recv)
       PCLB_CUDA(cudaMalloc(reinterpret_cast<void**>(&e->recv), n * sizeof(unsigned long long)));
+    t.send = e->local;
+    t.recv = e->recv;
     t.n_read = 1;
     t.read[0] = e->recv;
   }
   return t;
 }
 
-void comm_one_to_one_reduce(Ctx& c, const OneToOneTables& t, size_t n_cloud)
+PeerTables comm_segment_tables(Ctx& c, const unsigned long long* n, size_t elem_bytes)
 {
-  if (t.peer)
-    peer_u64(c, nullptr, nullptr, 0, kU64Sum);  // every rank's atomicMin pass is complete
-  else
-    comm_allreduce_u64(c, t.local, const_cast<unsigned long long*>(t.read[0]), std::max<size_t>(n_cloud, 1), kU64Min);
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID, "no communicator");
+  const int R = c.comm->nranks;
+  size_t at[kMaxRanks + 1];
+  const size_t most = segment_table_words(n, R, elem_bytes, at);
+  if (comm_peer_fused(c))
+    return comm_scratch_tables(c, most);
+  PeerTables t = comm_scratch_tables(c, at[R]);
+  PCLB_CUDA(cudaMemsetAsync(t.send, 0, t.words * sizeof(unsigned long long), c.stream));
+  t.local = t.send + at[c.comm->rank];
+  t.n_read = R;
+  for (int s = 0; s < R; ++s)
+    t.read[s] = t.recv + at[s];
+  return t;
 }
 
-void comm_one_to_one_done(Ctx& c, const OneToOneTables& t)
+void comm_tables_publish(Ctx& c, const PeerTables& t, int op)
 {
   if (t.peer)
-    peer_u64(c, nullptr, nullptr, 0, kU64Sum);  // no peer still reads this rank's table: the sparse reset may follow
+    peer_u64(c, nullptr, nullptr, 0, kU64Sum);  // every rank's writes to its table are complete
+  else
+    comm_allreduce_u64(c, t.send, t.recv, t.words, op);
+}
+
+void comm_tables_release(Ctx& c, const PeerTables& t)
+{
+  if (t.peer)
+    peer_u64(c, nullptr, nullptr, 0, kU64Sum);  // no peer still reads this rank's table: it may be rewritten
+}
+
+size_t allgather_u64(Ctx& c, const unsigned long long* d_send, size_t n, DevBuf<unsigned long long>& out)
+{
+  cudaStream_t st = c.stream;
+  const int R = comm_nranks(c), me = comm_rank(c);
+  std::vector<unsigned long long> cnt(R, 0);  // every rank's count
+  {
+    DevBuf<unsigned long long> d_cnt;
+    d_cnt.alloc(R, st);
+    cnt[me] = n;
+    PCLB_CUDA(cudaMemcpyAsync(d_cnt.p, cnt.data(), R * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
+    comm_allreduce_u64(c, d_cnt.p, d_cnt.p, R, kU64Sum);
+    PCLB_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt.p, R * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    check_device_error(c);
+  }
+  unsigned long long total = 0;
+  for (int s = 0; s < R; ++s)
+    total += cnt[s];
+  out.alloc(total, st);
+  if (!total)
+    return 0;
+  const PeerTables t = comm_segment_tables(c, cnt.data(), sizeof(unsigned long long));
+  gather_segments(c, one_segment(d_send, n), t.local);  // the write a peer reads after the barrier: a kernel
+  comm_tables_publish(c, t, kU64Sum);
+  gather_segments(c, table_runs<unsigned long long>(t, cnt.data()), out.p);
+  comm_tables_release(c, t);
+  return (size_t)total;
 }
 
 }  // namespace pclb200

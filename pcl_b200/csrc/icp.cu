@@ -222,13 +222,6 @@ struct Reducer {  // scratch of the grid sums (grid_fold)
   GridSum sum() const { return GridSum{partials.p, counter.p, accum.p}; }
 };
 
-static unsigned persistent_grid(const Ctx& c, size_t n, int block, int per_sm)
-{
-  size_t want = (n + block - 1) / block;
-  size_t cap = (size_t)c.sm_count * per_sm;
-  return (unsigned)std::max<size_t>(1, std::min(want, cap));
-}
-
 struct Icp {
   Ctx* ctx = nullptr;
   pclb200_icp_params P;
@@ -258,7 +251,7 @@ struct Icp {
   std::vector<pclb200_rejector> rejectors;  // applied in order after every search (icp.hpp:187-201)
   // sharded source: global position of this rank's slot 0 (offset_r, DESIGN.md §5), valid for communicator shard_comm
   unsigned long long shard_offset = 0, shard_comm = 0;
-  std::shared_ptr<OneToOneEntry> o2o;  // one-to-one rejector table of a sharded session
+  std::shared_ptr<PeerTableEntry> o2o;  // one-to-one rejector table of a sharded session
   // sharded target (icp_set_target_sharded): `tgt` is this rank's tile, `frame` the union of all tiles' boxes (lo, hi,
   // morton_scale: the frame of one index over the whole map).  Per iteration the tile's matches are published in
   // `shard_tab` (keys, then point records, then normal records; mapped into every rank) and the winners gathered into
@@ -266,7 +259,7 @@ struct Icp {
   bool sharded_target = false;
   Index frame;
   bool shard_checked = false;  // the first iterate after set_source checked that every rank staged n_q queries
-  std::shared_ptr<OneToOneEntry> shard_tab;
+  std::shared_ptr<PeerTableEntry> shard_tab;
   DevBuf<Match> gmatch;
   DevBuf<float4> gpts, gnrm;
   Reducer red;
@@ -313,7 +306,7 @@ static void transform_on_device(Ctx& c, const double* T, int mode, float4* pts, 
 {
   if (n == 0)
     return;
-  k_transform<<<persistent_grid(c, n, 256, 8), 256, 0, c.stream>>>(pts, n, make_pending(T, mode, 1), normals);
+  k_transform<<<persistent_blocks(c, n), 256, 0, c.stream>>>(pts, n, make_pending(T, mode, 1), normals);
   ++c.launches;
 }
 
@@ -404,7 +397,7 @@ static void prepare_sharded_rejectors(Icp& s)
     PCLB_REQUIRE(!s.tgt->labelled, PCLB200_ERR_INVALID,
                  "icp: the one-to-one rejector on a sharded source keeps a table per target record, which an index built "
                  "with caller ids does not define");
-    comm_one_to_one_tables(c, s.o2o, s.tgt->n_cloud);
+    comm_peer_tables(c, s.o2o, s.tgt->n_cloud);
   }
 }
 
@@ -614,10 +607,10 @@ static void exchange_shard_matches(Icp& s, bool with_normals)
   const size_t n = s.n_q;
   const size_t kw = (n + 1) & ~(size_t)1;  // key words, rounded up so that the records are 16-byte aligned
   const size_t words = kw + 2 * n * (with_normals ? 2 : 1);
-  const OneToOneTables t = comm_peer_tables(c, s.shard_tab, words);
-  auto records = [&](const unsigned long long* base) {
+  const PeerTables t = comm_peer_tables(c, s.shard_tab, words);
+  auto records = [&](unsigned long long* base) {
     ShardRecords r;
-    r.key = const_cast<unsigned long long*>(base);
+    r.key = base;
     r.pts = reinterpret_cast<float4*>(r.key + kw);
     r.nrm = with_normals ? r.pts + n : nullptr;
     return r;
@@ -627,10 +620,9 @@ static void exchange_shard_matches(Icp& s, bool with_normals)
   memset(&rs, 0, sizeof(rs));
   rs.n = t.n_read;
   for (int r = 0; r < t.n_read; ++r) {
-    const ShardRecords x = records(t.read[r]);
-    rs.key[r] = x.key;
-    rs.pts[r] = x.pts;
-    rs.nrm[r] = x.nrm;
+    rs.key[r] = t.read[r];
+    rs.pts[r] = reinterpret_cast<const float4*>(t.read[r] + kw);
+    rs.nrm[r] = with_normals ? rs.pts[r] + n : nullptr;
   }
   if (n) {
     k_shard_publish<<<grid_for(n, 256), 256, 0, st>>>(s.match.p, n, s.tgt->pts.p, with_normals ? s.tgt_normals.p : nullptr,
@@ -640,7 +632,7 @@ static void exchange_shard_matches(Icp& s, bool with_normals)
   if (t.peer)
     comm_barrier(c);
   else {
-    const ShardRecords all = records(t.read[0]);
+    const ShardRecords all = records(t.recv);
     comm_allreduce_u64(c, mine.key, all.key, n, kU64Min);
     if (n) {
       k_shard_keep_winners<<<grid_for(n, 256), 256, 0, st>>>(all.key, n, s.ctrl.p, mine);
@@ -653,8 +645,7 @@ static void exchange_shard_matches(Icp& s, bool with_normals)
     k_shard_gather<<<grid_for(n, 256), 256, 0, st>>>(rs, n, s.ctrl.p, s.gmatch.p, s.gpts.p, with_normals ? s.gnrm.p : nullptr);
     ++c.launches;
   }
-  if (t.peer)
-    comm_barrier(c);
+  comm_tables_release(c, t);
   PCLB_CUDA(cudaGetLastError());
 }
 
@@ -934,9 +925,9 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     a.cells = tree_view(T).cells;
     a.ctrl = s.ctrl.p;
     a.track_sel = track_mode == PCLB200_TRACK_AUTO;  // the search runs only in the flavour of the device's decision
-    const unsigned grid = persistent_grid(c, s.n_q, 256, 8);
-    const unsigned wgrid = persistent_grid(c, s.n_q, 256, 18);
-    const unsigned agrid = std::min(persistent_grid(c, s.n_q, 256, kAccumBlocksPerSM), s.red.max_blocks);
+    const unsigned grid = persistent_blocks(c, s.n_q);
+    const unsigned wgrid = persistent_blocks(c, s.n_q, 256, 18);
+    const unsigned agrid = std::min(persistent_blocks(c, s.n_q, 256, kAccumBlocksPerSM), s.red.max_blocks);
     const int n_enq = std::min(max_steps, std::max(1, s.P.max_iterations - s.loop.iterations));
     // sharded target: the accumulate kernels read the gathered records and the global matches
     const bool shard_nrm = s.sharded_target && s.P.estimator != PCLB200_EST_SVD && s.tgt_normals.p;
@@ -1200,7 +1191,7 @@ void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const voi
     load_vec3_as_float4(c, src_normals, n_src, stride_s, dsn.p, st);
   }
   Reducer red;
-  const unsigned grid = persistent_grid(c, n, 256, 4);
+  const unsigned grid = persistent_blocks(c, n, 256, 4);
   red.init(c, grid);
   DevBuf<SolveOut> so;
   so.alloc(1, st);
@@ -1296,7 +1287,7 @@ double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t
   QueryBatch qb;
   make_query_batch(c, tgt, dense.p, nq, qb);
   Reducer red;
-  const unsigned grid = persistent_grid(c, nq, 256, 8);
+  const unsigned grid = persistent_blocks(c, nq);
   red.init(c, grid);
   k_fitness<<<grid, 256, 0, st>>>(tree_view(tgt), qb.q.p, nq, max_range, red.sum(), c.d_error);
   ++c.launches;
@@ -1328,25 +1319,16 @@ double fitness_score_sharded(Ctx& c, const Index& tile, const void* src, size_t 
   transform_on_device(c, T, scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat, dense.p, nq, nullptr);
   QueryBatch qb;
   make_query_batch(c, tile, dense.p, nq, qb);
-  const OneToOneTables t = comm_scratch_tables(c, nq);
-  ShardReadSet rs;
-  memset(&rs, 0, sizeof(rs));
-  rs.n = t.n_read;
-  for (int r = 0; r < t.n_read; ++r)
-    rs.key[r] = t.read[r];
-  const unsigned grid = persistent_grid(c, nq, 256, 8);
+  const PeerTables t = comm_scratch_tables(c, nq);
+  const unsigned grid = persistent_blocks(c, nq);
   k_fitness_keys<<<grid, 256, 0, st>>>(tree_view(tile), qb.q.p, nq, t.local, c.d_error);
   ++c.launches;
-  if (t.peer)
-    comm_barrier(c);
-  else
-    comm_allreduce_u64(c, t.local, const_cast<unsigned long long*>(t.read[0]), nq, kU64Min);
+  comm_tables_publish(c, t, kU64Min);
   Reducer red;
   red.init(c, grid);
-  k_fitness_reduce<<<grid, 256, 0, st>>>(rs, nq, max_range, red.sum());
+  k_fitness_reduce<<<grid, 256, 0, st>>>(peer_table_set(t), nq, max_range, red.sum());
   ++c.launches;
-  if (t.peer)
-    comm_barrier(c);  // no rank rewrites its table (the next call) while a peer may still read it
+  comm_tables_release(c, t);  // no rank rewrites its table (the next call) while a peer may still read it
   PCLB_CUDA(cudaGetLastError());
   double acc[2];
   PCLB_CUDA(cudaMemcpyAsync(acc, red.accum.p, sizeof(acc), cudaMemcpyDeviceToHost, st));

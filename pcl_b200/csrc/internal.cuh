@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cfloat>
 #include <cstdint>
 #include <cstdio>
@@ -147,6 +148,11 @@ bool is_device_ptr(const void* p);
 // blocks of a 1-D launch over n items.  Only the .cu drivers launch; the kernel headers compiled by g++ for the host
 // tests (tests/host) bring their own launcher and grid size.
 inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
+// the same for a grid-stride kernel, capped at per_sm blocks per SM (at least one block)
+inline unsigned persistent_blocks(const Ctx& c, size_t n, int block = 256, int per_sm = 8)
+{
+  return (unsigned)std::max<size_t>(1, std::min<size_t>(grid_for(n, block), (size_t)c.sm_count * per_sm));
+}
 #endif
 
 // Any caller array may live in host or device memory (DESIGN.md §1).  The kernels read an input through on_device: the
@@ -347,8 +353,8 @@ void cluster_labels(Ctx& c, const Index& idx, double tolerance, int32_t* d_label
 // the same over a map sharded across the communicator's ranks (collective, shard_cluster.cu): labels and, when d_sizes is
 // not null, component sizes of the tile's records (tile.n_cloud entries each, on the device)
 void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t* d_labels, int64_t* d_sizes);
-// every rank's d_send[0..n) concatenated in rank order, identically on every rank (collective, shard_cluster.cu: the
-// count exchange, then comm_scratch_tables); returns the total
+// every rank's d_send[0..n) concatenated in rank order, identically on every rank (collective, comm.cu: the count
+// exchange, then comm_segment_tables); returns the total
 size_t allgather_u64(Ctx& c, const unsigned long long* d_send, size_t n, DevBuf<unsigned long long>& out);
 
 // flat per-correspondence arrays the rejectors work on (reject.cu)
@@ -398,23 +404,35 @@ enum { kU64Sum = 0, kU64Min = 1 };
 void comm_allreduce_u64(Ctx& c, const unsigned long long* d_send, unsigned long long* d_recv, size_t count, int op);
 // global position of this rank's first query (sum of n_q over the lower ranks) and the total; one exchange, synchronises
 unsigned long long comm_shard_offset(Ctx& c, unsigned long long n_q, unsigned long long* total);
-// per-session table of the one-to-one rejector: one u64 per target record on every rank (see DESIGN.md §5)
-struct OneToOneTables {
-  unsigned long long* local = nullptr;          // this rank's atomicMin table (all ~0 between iterations)
-  int n_read = 0;                               // tables to compare against: every rank's (peer path) or the NCCL minimum
+// Tables of u64 through which the ranks' kernels exchange whole arrays (DESIGN.md §5): the one-to-one rejector's, the
+// sharded target's, and the scratch of the sharded normals, clusters and fitness.  Every exchange is: this rank's kernels
+// write `local`; comm_tables_publish; kernels read the tables (peer_tables.cuh: peer_table_set, segment_reads);
+// comm_tables_release.
+//   peer path  every rank's own table, mapped into every rank: read[s] = rank s's.  Publish and release are barriers, the
+//              second so that no rank rewrites its table while a peer may still read it.
+//   NCCL path  publish is one all-reduce of send[0..words) into recv; release is nothing.  comm_peer_tables: send = local,
+//              and read[0] = recv is the reduction.  comm_segment_tables: the per-rank tables end to end in one zeroed
+//              table, so that a u64 sum with one writer per word copies them; read[s] = rank s's table in recv.
+struct PeerTables {
+  unsigned long long* local = nullptr;          // this rank's table
+  int n_read = 0;                               // tables to read
   const unsigned long long* read[kMaxRanks] = {};
-  bool peer = false;                            // peer path: a barrier before the reads and one before the reset
+  bool peer = false;
+  unsigned long long* send = nullptr;           // NCCL path: the all-reduce of comm_tables_publish
+  unsigned long long* recv = nullptr;
+  size_t words = 0;
 };
-// The session owns its table (freed with the session); the communicator keeps a weak reference and unmaps / frees the
-// table when it is destroyed first.  Allocated and mapped on first use, again after a new communicator or target size.
-struct OneToOneEntry;
-OneToOneTables comm_one_to_one_tables(Ctx& c, std::shared_ptr<OneToOneEntry>& owner, size_t n_cloud);
-void comm_one_to_one_reduce(Ctx& c, const OneToOneTables& t, size_t n_cloud);  // barrier, or NCCL min all-reduce
-void comm_one_to_one_done(Ctx& c, const OneToOneTables& t);                    // barrier before the sparse reset
-// The same machinery for any table of n_words u64 per rank (the sharded-target exchange of icp.cu): allocated (initially
-// all ~0) and, on the peer path, mapped into every rank on first use and again when n_words or the communicator changes.
-OneToOneTables comm_peer_tables(Ctx& c, std::shared_ptr<OneToOneEntry>& owner, size_t n_words);
-OneToOneTables comm_scratch_tables(Ctx& c, size_t n_words);  // a table owned by the communicator (one call's scratch)
+// The owner (a session) holds its table, freed with it; the communicator keeps a weak reference and unmaps / frees the
+// table when it is destroyed first.  A table of n_words u64 (initially all ~0) is allocated and, on the peer path, mapped
+// into every rank on first use, and again when n_words or the communicator changes.
+struct PeerTableEntry;
+PeerTables comm_peer_tables(Ctx& c, std::shared_ptr<PeerTableEntry>& owner, size_t n_words);
+PeerTables comm_scratch_tables(Ctx& c, size_t n_words);  // a table owned by the communicator (one call's scratch)
+// a table per rank of n[s] elements of elem_bytes (every rank passes the same n), from the scratch table: peer path, every
+// rank's sized to the largest; NCCL path, laid end to end in rank order, each from a word boundary, zeroed
+PeerTables comm_segment_tables(Ctx& c, const unsigned long long* n, size_t elem_bytes);
+void comm_tables_publish(Ctx& c, const PeerTables& t, int op);  // barrier, or the NCCL all-reduce (kU64Sum / kU64Min)
+void comm_tables_release(Ctx& c, const PeerTables& t);          // barrier, or nothing
 void comm_barrier(Ctx& c);  // peer path: every rank has reached this point of its stream; NCCL path: nothing
 // NCCL path only: element-wise max of uint32 bit patterns (an exact copy of the one non-zero contribution)
 void comm_allreduce_u32_max(Ctx& c, const unsigned* d_send, unsigned* d_recv, size_t count);
@@ -425,7 +443,7 @@ struct ShardedRejectArgs {
   const float4* tgt_pts = nullptr;  // Morton-ordered target, w = original index: the one-to-one table index
   size_t n_cloud = 0;               // target records
   unsigned long long offset = 0;    // global position of slot 0 of this rank
-  std::shared_ptr<OneToOneEntry>* o2o = nullptr;  // the session's one-to-one table
+  std::shared_ptr<PeerTableEntry>* o2o = nullptr;  // the session's one-to-one table
 };
 void apply_rejector_sharded(Ctx& c, const pclb200_rejector& r, const RejectArrays& a, const ShardedRejectArgs& s);
 

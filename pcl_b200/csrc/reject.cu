@@ -154,16 +154,11 @@ void apply_rejector_sharded(Ctx& c, const pclb200_rejector& r, const RejectArray
     return;
   }
   PCLB_REQUIRE(r.kind == PCLB200_REJ_ONE_TO_ONE, PCLB200_ERR_INVALID, "rejector kind has no sharded form");
-  const OneToOneTables t = comm_one_to_one_tables(c, *s.o2o, s.n_cloud);
-  O2OReadSet rs;
-  memset(&rs, 0, sizeof(rs));
-  rs.n = t.n_read;
-  for (int p = 0; p < t.n_read; ++p)
-    rs.t[p] = t.read[p];
+  const PeerTables t = comm_peer_tables(c, *s.o2o, s.n_cloud);
   k_o2o_min<<<g, 256, 0, st>>>(a.d2, a.tie, a.match, a.acc, n, s.offset, s.tgt_pts, t.local);
-  comm_one_to_one_reduce(c, t, s.n_cloud);
-  k_o2o_keep<<<g, 256, 0, st>>>(a.d2, a.tie, a.match, a.acc, n, s.offset, s.tgt_pts, rs);
-  comm_one_to_one_done(c, t);
+  comm_tables_publish(c, t, kU64Min);
+  k_o2o_keep<<<g, 256, 0, st>>>(a.d2, a.tie, a.match, a.acc, n, s.offset, s.tgt_pts, peer_table_set(t));
+  comm_tables_release(c, t);  // no peer still reads this rank's table: the sparse reset may follow
   k_o2o_reset<<<g, 256, 0, st>>>(a.match, n, s.tgt_pts, t.local);
   c.launches += 3;
   PCLB_CUDA(cudaGetLastError());

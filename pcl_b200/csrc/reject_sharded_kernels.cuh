@@ -11,6 +11,7 @@
 // can compile the kernels for the host and simulate several ranks in one process.
 #pragma once
 #include "internal.cuh"
+#include "peer_tables.cuh"
 
 namespace pclb200 {
 
@@ -152,15 +153,10 @@ __global__ void k_o2o_min(const float* __restrict__ d2, const unsigned* __restri
   atomicMin(&table[t], sel_key<true>(d2, tie, i, offset));
 }
 
-struct O2OReadSet {
-  int n;
-  const unsigned long long* t[kMaxRanks];
-};
-
 // step 2 (after the barrier / the min all-reduce): an entry survives iff no table holds a smaller key for its target
 __global__ void k_o2o_keep(const float* __restrict__ d2, const unsigned* __restrict__ tie, const int* __restrict__ mt,
                            int* __restrict__ acc, size_t n, unsigned long long offset, const float4* __restrict__ tgt_pts,
-                           const O2OReadSet tabs)
+                           const PeerTableSet<unsigned long long> tabs)
 {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n || !acc[i])

@@ -19,9 +19,9 @@
 //   labels  each tile record's final label; its size is counted by the lowest rank that holds its id in its tile (a
 //           higher rank received the id from it in the halo): local components locally, graph nodes in one dense array,
 //           the same on every rank, summed over the ranks and folded onto the roots.
-// Every exchange moves a count known to every rank, so all ranks take the same branches; a table moves through
-// comm_scratch_tables: peer path, each rank's table with a barrier before the reads and one after them; NCCL path, a
-// zeroed table with one contributor per entry and one u64 sum all-reduce.
+// Every exchange moves a count known to every rank, so all ranks take the same branches.  The answers and the edges move
+// through comm_segment_tables in the layout of peer_tables.cuh, the node counts through comm_scratch_tables; each
+// exchange is comm_tables_publish before the reads and comm_tables_release after them.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -29,19 +29,13 @@
 #include <vector>
 
 #include "internal.cuh"
+#include "peer_tables.cuh"
 #include "shard_cluster_kernels.cuh"
 
 namespace pclb200 {
 
-bool comm_active(const Ctx& c);
-bool comm_peer_fused(const Ctx& c);
 int comm_nranks(const Ctx& c);
 int comm_rank(const Ctx& c);
-
-static unsigned persistent_blocks(const Ctx& c, size_t n)
-{
-  return (unsigned)std::max<size_t>(1, std::min<size_t>(grid_for(n, 256), (size_t)c.sm_count * 8));
-}
 
 // sorted unique copy of keys[0..n) (u32 or u64) into out; returns how many
 template <typename K>
@@ -69,75 +63,6 @@ static size_t sort_unique(Ctx& c, const K* keys, size_t n, DevBuf<K>& out)
   return (size_t)m;
 }
 
-// n u64 words from `from` into `to` with a kernel (the write a peer may read after the next barrier)
-static void copy_u64(Ctx& c, const unsigned long long* from, size_t n, unsigned long long* to)
-{
-  if (!n)
-    return;
-  ScReadSet<unsigned long long> one;
-  memset(&one, 0, sizeof(one));
-  one.n = 1;
-  one.src[0] = from;
-  one.begin[1] = n;
-  k_sc_gather<<<persistent_blocks(c, n), 256, 0, c.stream>>>(one, to);
-  ++c.launches;
-  PCLB_CUDA(cudaGetLastError());
-}
-
-size_t allgather_u64(Ctx& c, const unsigned long long* d_send, size_t n, DevBuf<unsigned long long>& out)
-{
-  cudaStream_t st = c.stream;
-  const int R = comm_nranks(c), me = comm_rank(c);
-  std::vector<unsigned long long> cnt(R, 0);  // every rank's count
-  {
-    DevBuf<unsigned long long> d_cnt;
-    d_cnt.alloc(R, st);
-    cnt[me] = n;
-    PCLB_CUDA(cudaMemcpyAsync(d_cnt.p, cnt.data(), R * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
-    comm_allreduce_u64(c, d_cnt.p, d_cnt.p, R, kU64Sum);
-    PCLB_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt.p, R * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    check_device_error(c);
-  }
-  unsigned long long total = 0, most = 0, below = 0;
-  for (int s = 0; s < R; ++s) {
-    if (s < me)
-      below += cnt[s];
-    total += cnt[s];
-    most = std::max(most, cnt[s]);
-  }
-  out.alloc(total, st);
-  if (!total)
-    return 0;
-  const bool peer = comm_peer_fused(c);
-  const size_t words = (size_t)(peer ? most : total);
-  OneToOneTables t = comm_scratch_tables(c, words);
-  if (!t.peer)
-    PCLB_CUDA(cudaMemsetAsync(t.local, 0, words * sizeof(unsigned long long), st));
-  copy_u64(c, d_send, n, t.local + (t.peer ? 0 : below));
-  ScReadSet<unsigned long long> rs;
-  memset(&rs, 0, sizeof(rs));
-  if (t.peer) {
-    comm_barrier(c);
-    for (int s = 0; s < R; ++s) {
-      rs.src[s] = t.read[s];
-      rs.begin[s + 1] = rs.begin[s] + cnt[s];
-    }
-    rs.n = R;
-  }
-  else {
-    comm_allreduce_u64(c, t.local, const_cast<unsigned long long*>(t.read[0]), words, kU64Sum);
-    rs.n = 1;
-    rs.src[0] = t.read[0];
-    rs.begin[1] = total;
-  }
-  k_sc_gather<<<persistent_blocks(c, total), 256, 0, st>>>(rs, out.p);
-  ++c.launches;
-  PCLB_CUDA(cudaGetLastError());
-  if (t.peer)
-    comm_barrier(c);
-  return (size_t)total;
-}
-
 void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t* d_labels, int64_t* d_sizes)
 {
   cudaStream_t st = c.stream;
@@ -156,17 +81,13 @@ void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t
     local.reset(sharded_local_map(c, tile, tile.pts.p, tile.pts.n, 0, r2, stages, &tr));
   }
   const size_t m = local->n_cloud;
-  auto sent = [&](int s, int r) { return s == r ? 0ull : tr.cnt[(size_t)s * R + r]; };
-  unsigned long long all = 0, most_in = 0, lower = 0;
-  for (int r = 0; r < R; ++r) {
-    unsigned long long in = 0;
-    for (int s = 0; s < R; ++s)
-      in += sent(s, r);
-    most_in = std::max(most_in, in);
-    all += in;
-  }
-  for (int s = 0; s < me; ++s)
-    lower += sent(s, me);
+  // the answers go back along the halo: rank r sends sender s one u32 per point it received from s (transposed counts)
+  const std::vector<unsigned long long> ans = segment_answers(tr.cnt, R);
+  const std::vector<unsigned long long> n_ans = segment_table_sizes(ans.data(), R);
+  unsigned long long all = 0;
+  for (int r = 0; r < R; ++r)
+    all += n_ans[r];
+  const unsigned long long lower = segment_start(ans.data(), R, me, me);  // received from the ranks below
   const size_t n_recv = tr.recv_ids.n, n_sent = tr.sent_ids.n;
 
   DevBuf<int32_t> lab;
@@ -187,54 +108,24 @@ void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t
   size_t n_nodes = 0;
   {
     ProfScope ps(c, "sharded_cluster_stitch");
-    // the answers: u32 per received point; peer path, in the receiver's table in the order it received them (by sender);
-    // NCCL path, in one table of runs by receiver, each run by sender
     DevBuf<unsigned long long> edges;
     edges.alloc(n_sent, st);
     if (all) {
-      const bool peer = comm_peer_fused(c);
-      const size_t words = (size_t)((peer ? most_in : all) + 1) / 2;
-      OneToOneTables t = comm_scratch_tables(c, words);
-      auto run_of = [&](int r) {  // NCCL layout: the answers of the ranks below r come first
-        unsigned long long off = 0;
-        for (int x = 0; x < r; ++x)
-          for (int s = 0; s < R; ++s)
-            off += sent(s, x);
-        return off;
-      };
-      unsigned* mine = reinterpret_cast<unsigned*>(t.local);
-      if (!t.peer)
-        PCLB_CUDA(cudaMemsetAsync(t.local, 0, words * sizeof(unsigned long long), st));
+      const PeerTables t = comm_segment_tables(c, n_ans.data(), sizeof(unsigned));
       if (n_recv) {
         k_sc_answer<<<persistent_blocks(c, n_recv), 256, 0, st>>>(tr.recv_ids.p, n_recv, tr.local_ids.p, m, lab_id.p,
-                                                                  t.peer ? mine : mine + run_of(me));
+                                                                  reinterpret_cast<unsigned*>(t.local));
         ++c.launches;
         PCLB_CUDA(cudaGetLastError());
       }
-      if (t.peer)
-        comm_barrier(c);
-      else  // each u32 has one writer and is zero elsewhere: the u64 sum carries nothing between the halves
-        comm_allreduce_u64(c, t.local, const_cast<unsigned long long*>(t.read[0]), words, kU64Sum);
-      ScReadSet<unsigned> rs;  // the answers to this rank's segments, by destination
-      memset(&rs, 0, sizeof(rs));
-      for (int r = 0; r < R; ++r) {
-        if (r == me)
-          continue;
-        unsigned long long off = t.peer ? 0 : run_of(r);
-        for (int s = 0; s < me; ++s)
-          off += sent(s, r);
-        rs.src[rs.n] = reinterpret_cast<const unsigned*>(t.read[t.peer ? r : 0]) + off;
-        rs.begin[rs.n + 1] = rs.begin[rs.n] + sent(me, r);
-        ++rs.n;
-      }
+      comm_tables_publish(c, t, kU64Sum);  // NCCL: every word has one writer, so the u64 sum copies it
       if (n_sent) {
-        k_sc_edges<<<persistent_blocks(c, n_sent), 256, 0, st>>>(tr.sent_ids.p, n_sent, tr.local_ids.p, m, lab_id.p, rs,
-                                                                 edges.p);
+        k_sc_edges<<<persistent_blocks(c, n_sent), 256, 0, st>>>(tr.sent_ids.p, n_sent, tr.local_ids.p, m, lab_id.p,
+                                                                 segment_reads<unsigned>(t, ans.data(), R, me), edges.p);
         ++c.launches;
         PCLB_CUDA(cudaGetLastError());
       }
-      if (t.peer)
-        comm_barrier(c);
+      comm_tables_release(c, t);
     }
     DevBuf<unsigned long long> uniq;
     const size_t n_uniq = sort_unique(c, edges.p, n_sent, uniq);
@@ -282,25 +173,12 @@ void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
   if (n_nodes) {  // the node counts summed over the ranks, then folded onto the roots
-    OneToOneTables t = comm_scratch_tables(c, n_nodes);
-    copy_u64(c, node_cnt.p, n_nodes, t.local);
-    ScReadSet<unsigned long long> tables;
-    memset(&tables, 0, sizeof(tables));
-    if (t.peer) {
-      comm_barrier(c);
-      tables.n = R;
-      for (int s = 0; s < R; ++s)
-        tables.src[s] = t.read[s];
-    }
-    else {
-      comm_allreduce_u64(c, t.local, const_cast<unsigned long long*>(t.read[0]), n_nodes, kU64Sum);
-      tables.n = 1;
-      tables.src[0] = t.read[0];
-    }
-    k_sc_sum<<<persistent_blocks(c, n_nodes), 256, 0, st>>>(tables, n_nodes, node_cnt.p);
+    const PeerTables t = comm_scratch_tables(c, n_nodes);
+    gather_segments(c, one_segment(node_cnt.p, n_nodes), t.local);  // the write a peer reads after the barrier: a kernel
+    comm_tables_publish(c, t, kU64Sum);
+    k_sc_sum<<<persistent_blocks(c, n_nodes), 256, 0, st>>>(peer_table_set(t), n_nodes, node_cnt.p);
     ++c.launches;
-    if (t.peer)
-      comm_barrier(c);
+    comm_tables_release(c, t);
     k_sc_fold<<<persistent_blocks(c, n_nodes), 256, 0, st>>>(node_cnt.p, n_nodes, root.p, comp.p);
     ++c.launches;
     PCLB_CUDA(cudaGetLastError());

@@ -6,19 +6,19 @@
 //   k_sc_answer      per received halo point, its local label on this rank: the answer its sender reads back
 //   k_sc_mark_lower  records of C_r that a lower rank also holds in its tile (counted there, not here)
 //   k_sc_edges       per point this rank sent, the edge (its label here, the label its receiver answered) as one u64
-//   k_sc_gather      copies the segments of a u64 read set one after the other (the all-gather of the edges)
 //   k_sc_split       both ends of every edge: the node list is their sorted unique set
 //   k_sc_init        parent = identity over the dense node numbers
 //   k_sc_unite       union-find over them (cc_unite of union_find.cuh, as cluster_kernels.cuh)
 //   k_sc_roots       per node its root, whose node carries the smallest label of the stitched component
 //   k_sc_count       per owned tile record, +1 to its graph node or to its local component
-//   k_sc_sum         element-wise u64 sum of every rank's table (the node counts, peer path)
+//   k_sc_sum         element-wise u64 sum of the tables (the node counts: every rank's, or their NCCL sum)
 //   k_sc_fold        per node, its summed count added to its root
 //   k_sc_output      per tile record, the final label and the whole-map size of its component
 // A header of its own so that tests/host/shard_cluster_host_test.cpp can compile the kernels for the host and simulate
 // several ranks.
 #pragma once
 #include "internal.cuh"
+#include "peer_tables.cuh"
 #include "union_find.cuh"
 
 namespace pclb200 {
@@ -35,23 +35,6 @@ __device__ __forceinline__ int sc_find(const unsigned* __restrict__ a, size_t n,
       hi = mid;
   }
   return lo < n && a[lo] == v ? (int)lo : -1;
-}
-
-// Segments of peer-visible tables read one after the other: segment s holds begin[s + 1] - begin[s] entries at src[s].
-template <typename T>
-struct ScReadSet {
-  int n;
-  const T* src[kMaxRanks];
-  unsigned long long begin[kMaxRanks + 1];
-};
-
-template <typename T>
-__device__ __forceinline__ T sc_read(const ScReadSet<T>& rs, unsigned long long i)
-{
-  int s = 0;
-  while (i >= rs.begin[s + 1])
-    ++s;
-  return __ldcv(rs.src[s] + (i - rs.begin[s]));
 }
 
 // lab_id[i] = local_ids[lab[i]]: cluster_labels labels record i of C_r with the smallest record of its component, and
@@ -85,22 +68,13 @@ k_sc_mark_lower(const unsigned* __restrict__ recv_ids, size_t n, const unsigned*
 // answers are aligned with sent_ids (by destination, each segment in the order this rank wrote it)
 __global__ void __launch_bounds__(256)
 k_sc_edges(const unsigned* __restrict__ sent_ids, size_t n, const unsigned* __restrict__ local_ids, size_t m,
-           const unsigned* __restrict__ lab_id, const ScReadSet<unsigned> answers, unsigned long long* __restrict__ edges)
+           const unsigned* __restrict__ lab_id, const PeerSegments<unsigned> answers, unsigned long long* __restrict__ edges)
 {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const unsigned a = lab_id[sc_find(local_ids, m, sent_ids[i])];
-    const unsigned b = sc_read(answers, i);
+    const unsigned b = peer_segment_read(answers, i);
     edges[i] = a < b ? ((unsigned long long)a << 32) | b : ((unsigned long long)b << 32) | a;
   }
-}
-
-__global__ void __launch_bounds__(256)
-k_sc_gather(const ScReadSet<unsigned long long> rs, unsigned long long* __restrict__ out)
-{
-  const unsigned long long total = rs.begin[rs.n];
-  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < total;
-       i += (unsigned long long)gridDim.x * blockDim.x)
-    out[i] = sc_read(rs, i);
 }
 
 __global__ void __launch_bounds__(256)
@@ -166,12 +140,12 @@ k_sc_count(const float4* __restrict__ pts, size_t np, const unsigned* __restrict
 
 // out[i] = the sum over the tables of word i
 __global__ void __launch_bounds__(256)
-k_sc_sum(const ScReadSet<unsigned long long> tables, size_t n, unsigned long long* __restrict__ out)
+k_sc_sum(const __grid_constant__ PeerTableSet<unsigned long long> tables, size_t n, unsigned long long* __restrict__ out)
 {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     unsigned long long s = 0;
     for (int t = 0; t < tables.n; ++t)
-      s += __ldcv(tables.src[t] + i);
+      s += __ldcv(tables.t[t] + i);
     out[i] = s;
   }
 }

@@ -3,18 +3,19 @@
 // holds every whole-map neighbour of every query, indexes its tile plus that halo as an ordinary index sorted by id, and
 // runs the unchanged single-GPU normals on it (DESIGN.md §5, "Normals of a sharded map").  Clustering a sharded map
 // (shard_cluster.cu) builds its local map here too, with the tile's points as the queries and the tolerance as the radius,
-// and takes a HaloTrace of the exchange so that it can answer every received point back to its sender.
+// and takes a HaloTrace of the exchange so that it can answer every received point back to its sender: the ids it
+// received, and the ids it sent, read from its own table, where its segments are one run.
 //
 //   bound   rho_q^2 = the k-th nearest squared distance of q in this rank's tile (launch_knn_kth; +inf when the tile
 //           holds fewer than k points), or r^2.  The tile is part of the map, so every member of q's whole-map list,
 //           ties at the k-th distance included, lies within rho_q.
 //   boxes   this rank's box = the union of [q - reach(rho_q), q + reach(rho_q)] over its finite queries, rounded outward;
 //           one u64 minimum over every rank's 6 keys (the discipline of icp.cu: union_frame).
-//   halo    every rank counts its tile points inside every other rank's box (one u64 sum of the R x R counts), publishes
-//           them into its peer-mapped table, one segment per destination; a barrier; every rank copies its segments out
-//           of every peer's table; a second barrier, so that no rank rewrites its table while a peer may still read it.
-//           Without the mappings (PCLB200_REDUCE_NCCL) each rank writes its segments at global offsets into a zeroed
-//           table and one u64 sum all-reduce, with one contributor per word, copies them exactly.
+//   halo    every rank counts its tile points inside every other rank's box (one u64 sum of the R x R counts), writes
+//           them into its table of comm_segment_tables, one segment per destination (peer_tables.cuh: the layout);
+//           publish; every rank copies its segments out of every rank's table; release.  The peer path's tables are
+//           peer-mapped and both steps are barriers; under PCLB200_REDUCE_NCCL they lie end to end in one zeroed table
+//           and one u64 sum all-reduce, with one contributor per word, copies them exactly.
 //   map     tile + halo sorted by id, duplicate ids (one point held by two ranks) dropped, indexed with
 //           build_index_from_device: record numbers increase with the id, so the index's (d2, index) tie rule is the
 //           whole map's (d2, id) rule and every list it returns is the whole map's, in the same order.
@@ -26,19 +27,14 @@
 #include <vector>
 
 #include "internal.cuh"
+#include "peer_tables.cuh"
 #include "shard_normals_kernels.cuh"
 
 namespace pclb200 {
 
 bool comm_active(const Ctx& c);
-bool comm_peer_fused(const Ctx& c);
 int comm_nranks(const Ctx& c);
 int comm_rank(const Ctx& c);
-
-static unsigned persistent_blocks(const Ctx& c, size_t n)
-{
-  return (unsigned)std::max<size_t>(1, std::min<size_t>(grid_for(n, 256), (size_t)c.sm_count * 8));
-}
 
 // Steps bound and boxes: every rank's box, on the device (kHaloBoxWords keys per rank, folded over the ranks)
 static void exchange_boxes(Ctx& c, const Index& tile, const float4* d_q, size_t nq, int k, float r2, int R, int me,
@@ -92,15 +88,12 @@ Index* sharded_local_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq
     std::vector<unsigned long long> cnt((size_t)R * R);
     PCLB_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt.p, d_cnt.bytes(), cudaMemcpyDeviceToHost, st));
     check_device_error(c);
-    auto sent = [&](int s, int r) { return s == r ? 0ull : cnt[(size_t)s * R + r]; };  // (s, s) is the tile itself
-    unsigned long long halo = 0, most = 0, all = 0;
+    const std::vector<unsigned long long> n_table = segment_table_sizes(cnt.data(), R);  // (s, s) is the tile itself
+    unsigned long long halo = 0, all = 0;
     for (int s = 0; s < R; ++s) {
-      unsigned long long out = 0;
-      for (int r = 0; r < R; ++r)
-        out += sent(s, r);
-      most = std::max(most, out);
-      all += out;
-      halo += sent(s, me);
+      all += n_table[s];
+      if (s != me)
+        halo += cnt[(size_t)s * R + me];
     }
     const size_t n_tile = cnt[(size_t)me * R + me];
     PCLB_REQUIRE(n_tile == tile.n_valid, PCLB200_ERR_INTERNAL, "sharded normals: the tile's points were miscounted");
@@ -108,91 +101,34 @@ Index* sharded_local_map(Ctx& c, const Index& tile, const float4* d_q, size_t nq
     PCLB_REQUIRE(n_local < (size_t)0x7fffffff, PCLB200_ERR_INVALID,
                  "sharded normals: the tile and its halo exceed 2^31 - 1 points");
     local.alloc(n_local, st);
-    const bool peer = comm_peer_fused(c);
     HaloOut out;
     memset(&out, 0, sizeof(out));
     cursor.alloc(R, st);
     PCLB_CUDA(cudaMemsetAsync(cursor.p, 0, cursor.bytes(), st));
     out.count = cursor.p;
     out.dst[me] = local.p;
-    HaloReadSet rs;
-    memset(&rs, 0, sizeof(rs));
-    OneToOneTables t;
+    PeerTables t;
     if (all) {  // every rank knows every count: all of them take this branch or none
-      // segment (s -> r) at: peer path, s's table, after s's segments for lower r; NCCL path, the global table ordered by
-      // (r, s), so that what rank r receives is one run
-      const size_t words = 2 * (size_t)(peer ? most : all);
-      t = comm_scratch_tables(c, words);
-      float4* mine = reinterpret_cast<float4*>(t.local);
-      if (!t.peer)
-        PCLB_CUDA(cudaMemsetAsync(t.local, 0, words * sizeof(unsigned long long), st));
-      unsigned long long at = 0;
-      for (int r = 0; r < R; ++r)
-        for (int s = t.peer ? me : 0; s < (t.peer ? me + 1 : R); ++s) {
-          if (s == me && r != me)
-            out.dst[r] = mine + at;
-          at += sent(s, r);
-        }
-      if (t.peer) {
-        rs.n = 0;
-        for (int s = 0; s < R; ++s) {
-          if (s == me)
-            continue;
-          unsigned long long off = 0;  // s's segments for the ranks below me
-          for (int r = 0; r < me; ++r)
-            off += sent(s, r);
-          rs.src[rs.n] = reinterpret_cast<const float4*>(t.read[s]) + off;
-          rs.begin[rs.n + 1] = rs.begin[rs.n] + sent(s, me);
-          ++rs.n;
-        }
-      }
-      else {
-        unsigned long long off = 0;  // the runs of the ranks below me
-        for (int r = 0; r < me; ++r)
-          for (int s = 0; s < R; ++s)
-            off += sent(s, r);
-        rs.n = 1;
-        rs.src[0] = reinterpret_cast<const float4*>(t.read[0]) + off;
-        rs.begin[1] = halo;
-      }
+      t = comm_segment_tables(c, n_table.data(), sizeof(float4));
+      segment_writes(reinterpret_cast<float4*>(t.local), cnt.data(), R, me, out.dst);
     }
     k_halo_select<<<persistent_blocks(c, np), 256, 0, st>>>(tile.pts.p, np, boxes.p, R, me, out);
     ++c.launches;
     PCLB_CUDA(cudaGetLastError());
-    if (trace) {
+    if (trace) {  // this rank's segments are the first n_table[me] points of its table, by destination
       trace->cnt = cnt;
-      unsigned long long n_sent = 0;
-      HaloReadSet own;  // this rank's segments, by destination, before any rank rewrites its table
-      memset(&own, 0, sizeof(own));
-      for (int r = 0; r < R; ++r)
-        if (r != me) {
-          own.src[own.n] = out.dst[r];
-          own.begin[own.n + 1] = own.begin[own.n] + sent(me, r);
-          ++own.n;
-          n_sent += sent(me, r);
-        }
-      trace->sent_ids.alloc(n_sent, st);
-      if (n_sent) {
-        DevBuf<float4> copy;
-        copy.alloc(n_sent, st);
-        k_halo_gather<<<persistent_blocks(c, n_sent), 256, 0, st>>>(own, copy.p);
-        k_halo_ids<<<grid_for(n_sent, 256), 256, 0, st>>>(copy.p, n_sent, trace->sent_ids.p);
-        c.launches += 2;
+      trace->sent_ids.alloc(n_table[me], st);
+      if (n_table[me]) {
+        k_halo_ids<<<grid_for(n_table[me], 256), 256, 0, st>>>(reinterpret_cast<const float4*>(t.local), n_table[me],
+                                                               trace->sent_ids.p);
+        ++c.launches;
         PCLB_CUDA(cudaGetLastError());
       }
     }
     if (all) {
-      if (t.peer)
-        comm_barrier(c);
-      else
-        comm_allreduce_u64(c, t.local, const_cast<unsigned long long*>(t.read[0]), 2 * (size_t)all, kU64Sum);
-      if (halo) {
-        k_halo_gather<<<persistent_blocks(c, halo), 256, 0, st>>>(rs, local.p + n_tile);
-        ++c.launches;
-        PCLB_CUDA(cudaGetLastError());
-      }
-      if (t.peer)
-        comm_barrier(c);
+      comm_tables_publish(c, t, kU64Sum);
+      gather_segments(c, segment_reads<float4>(t, cnt.data(), R, me), local.p + n_tile);
+      comm_tables_release(c, t);
     }
   }
 

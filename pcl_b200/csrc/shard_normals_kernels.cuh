@@ -7,8 +7,8 @@
 //   k_halo_select  per tile point and per rank r: inside r's box?  Counts (dst == nullptr) or writes the point, a float4
 //                  whose w is its id, to the rank's segment (warp-aggregated cursors: the order inside a segment is free,
 //                  the local map is sorted by id afterwards)
-//   k_halo_gather  copies this rank's segments out of every peer's table (peer-mapped) or out of their NCCL sum
 //   k_halo_ids     the id of every point (w bits): the sort key of the local map
+// The segments travel through comm_segment_tables and are read back with k_gather_segments (peer_tables.cuh).
 // A header of its own so that tests/host/shard_normals_host_test.cpp can compile the kernels for the host and simulate
 // several ranks.
 #pragma once
@@ -132,27 +132,6 @@ k_halo_select(const float4* __restrict__ pts, size_t n, const unsigned long long
       if (in && out.dst[r])
         out.dst[r][at + __popc(m & ((1u << lane) - 1u))] = p;
     }
-  }
-}
-
-// The halo segments this rank reads: n sources, source s holds count[s] points at src[s]; they land one after the other
-// from out[0] on (begin[s] = the sum of the counts before s).
-struct HaloReadSet {
-  int n;
-  const float4* src[kMaxRanks];
-  unsigned long long begin[kMaxRanks + 1];
-};
-
-__global__ void __launch_bounds__(256)
-k_halo_gather(const HaloReadSet rs, float4* __restrict__ out)
-{
-  const unsigned long long total = rs.begin[rs.n];
-  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < total;
-       i += (unsigned long long)gridDim.x * blockDim.x) {
-    int s = 0;
-    while (i >= rs.begin[s + 1])
-      ++s;
-    out[i] = __ldcv(rs.src[s] + (i - rs.begin[s]));
   }
 }
 

@@ -10,6 +10,7 @@
 // that tests/host/shard_target_host_test.cpp can compile the kernels for the host and simulate several ranks.
 #pragma once
 #include "icp_kernels.cuh"
+#include "peer_tables.cuh"
 
 namespace pclb200 {
 
@@ -135,16 +136,16 @@ k_fitness_keys(const TreeView T, const float4* __restrict__ q, size_t nq, unsign
     atomicExch(d_error, kErrStackOverflow);
 }
 
-// step 2: per slot the smallest key over the read set, then k_fitness's sums (count and sum of d2 <= max_range) in slot
-// order: the same value on every rank
+// step 2: per slot the smallest key over the tables (every rank's, or their NCCL minimum), then k_fitness's sums (count
+// and sum of d2 <= max_range) in slot order: the same value on every rank
 __global__ void __launch_bounds__(256)
-k_fitness_reduce(const ShardReadSet rs, size_t n, double max_range, GridSum sum)
+k_fitness_reduce(const __grid_constant__ PeerTableSet<unsigned long long> keys, size_t n, double max_range, GridSum sum)
 {
   double acc[2] = {0.0, 0.0};
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     unsigned long long best = kNoShardMatch;
-    for (int r = 0; r < rs.n; ++r) {
-      const unsigned long long k = __ldcv(rs.key[r] + i);
+    for (int r = 0; r < keys.n; ++r) {
+      const unsigned long long k = __ldcv(keys.t[r] + i);
       best = k < best ? k : best;
     }
     if (best != kNoShardMatch) {

@@ -97,20 +97,19 @@ static void apply_sharded(World& w, const pclb200_rejector& r, int o2o_mode, dou
     Rank& k = w.ranks[q];
     launch(grid_for(k.n, 256), 256, [&] { k_o2o_min(k.d2.data(), k.tie.data(), k.mt.data(), k.acc.data(), k.n, k.offset, w.tgt_pts.data(), table[q].data()); });
   }
-  O2OReadSet rs;
-  std::memset(&rs, 0, sizeof(rs));
+  PeerTables tabs;
   if (o2o_mode == kPeer) {  // barrier, then every rank reads every table
-    rs.n = R;
-    for (int q = 0; q < R; ++q) rs.t[q] = table[q].data();
+    tabs.n_read = R;
+    for (int q = 0; q < R; ++q) tabs.read[q] = table[q].data();
   }
   else {                    // ncclAllReduce(min) of the tables into recv
     for (size_t t = 0; t < w.n_cloud; ++t) { unsigned long long m = ~0ull; for (int q = 0; q < R; ++q) m = std::min(m, table[q][t]); recv[t] = m; }
-    rs.n = 1;
-    rs.t[0] = recv.data();
+    tabs.n_read = 1;
+    tabs.read[0] = recv.data();
   }
   for (int q = 0; q < R; ++q) {
     Rank& k = w.ranks[q];
-    launch(grid_for(k.n, 256), 256, [&] { k_o2o_keep(k.d2.data(), k.tie.data(), k.mt.data(), k.acc.data(), k.n, k.offset, w.tgt_pts.data(), rs); });
+    launch(grid_for(k.n, 256), 256, [&] { k_o2o_keep(k.d2.data(), k.tie.data(), k.mt.data(), k.acc.data(), k.n, k.offset, w.tgt_pts.data(), peer_table_set(tabs)); });
   }
   for (int q = 0; q < R; ++q) {  // second barrier, sparse reset: the table must be all ~0 again
     Rank& k = w.ranks[q];

@@ -1,8 +1,8 @@
 // shard_cluster_host_test.cpp — Euclidean clustering over a sharded map (pcl_b200/csrc/shard_cluster_kernels.cuh, with the
 // halo kernels of shard_normals_kernels.cuh and the union-find of cluster_kernels.cuh) compiled for the HOST and run in
 // shard_cluster.cu's sequence for R = 1, 2, 3, 5, 8 simulated ranks in one process: this program does the cross-rank steps
-// comm.cu would do (the u64 minimum of the boxes, the peer tables with their barriers, or the NCCL sum of a zeroed global
-// table).  Every rank's labels and sizes are compared with a brute-force connected-components of the whole map (union of
+// comm.cu would do (the u64 minimum of the boxes, the tables of peer_tables_sim.h), and places the segments with the
+// layout functions of peer_tables.cuh that the driver calls.  Every rank's labels and sizes are compared with a brute-force connected-components of the whole map (union of
 // the tiles' ids, d2 < r2 under the library's distance).
 // Scenes: a zig-zag chain crossing every slab boundary many times (a component's pieces on one rank joined only through
 // other ranks), blobs straddling the boundaries, a power-of-two lattice at exactly the tolerance (no edge) and just above
@@ -22,6 +22,7 @@ static inline unsigned long long atomicMin(unsigned long long* p, unsigned long 
 #include "../../pcl_b200/csrc/shard_normals_kernels.cuh"
 #include "../../pcl_b200/csrc/cluster_kernels.cuh"
 #include "../../pcl_b200/csrc/shard_cluster_kernels.cuh"
+#include "peer_tables_sim.h"
 
 static long g_checks = 0, g_fail = 0;
 #define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
@@ -51,8 +52,6 @@ static bool finite3(const float4& p) { return std::isfinite(p.x) && std::isfinit
 static int id_of(const float4& p) { return __float_as_int(p.w); }
 static const float4 kPad = make_float4(INFINITY, INFINITY, INFINITY, __int_as_float(kSentinelIndex));
 
-enum { kPeer = 0, kNccl = 1 };
-
 // per simulated rank: what shard_cluster.cu keeps between the exchanges
 struct Rank {
   std::vector<float4> pts;         // the tile index's point array (finite records, padding between)
@@ -64,45 +63,21 @@ struct Rank {
   std::vector<unsigned long long> edges;
 };
 
-// the u64 tables of one exchange: peer path, one per rank; NCCL path, the sum of every rank's zeroed table
-struct Tables {
-  int mode, R;
-  std::vector<std::vector<unsigned long long>> local;
-  std::vector<unsigned long long> global;
-  Tables(int mode_, int R_, size_t words) : mode(mode_), R(R_), local(R_, std::vector<unsigned long long>(std::max<size_t>(words, 1), mode_ == kPeer ? ~0ull : 0ull)) {}
-  void reduce()  // barrier (peer) or the sum all-reduce (NCCL)
-  {
-    if (mode == kPeer) return;
-    global.assign(local[0].size(), 0ull);
-    for (int s = 0; s < R; ++s) for (size_t i = 0; i < global.size(); ++i) global[i] += local[s][i];
-  }
-  const unsigned long long* read(int r) const { return mode == kPeer ? local[r].data() : global.data(); }
-};
-
 // the all-gather of allgather_u64 over the ranks' arrays
 static std::vector<unsigned long long> allgather(int mode, const std::vector<std::vector<unsigned long long>>& in)
 {
   const int R = (int)in.size();
-  size_t total = 0, most = 0;
-  for (const auto& v : in) { total += v.size(); most = std::max(most, v.size()); }
+  std::vector<unsigned long long> n(R);
+  size_t total = 0;
+  for (int s = 0; s < R; ++s) { n[s] = in[s].size(); total += n[s]; }
   if (!total) return {};
-  Tables t(mode, R, mode == kPeer ? most : total);
-  size_t below = 0;
-  for (int s = 0; s < R; ++s) {
-    ScReadSet<unsigned long long> one;
-    std::memset(&one, 0, sizeof one);
-    one.n = 1; one.src[0] = in[s].data(); one.begin[1] = in[s].size();
-    if (!in[s].empty()) launch(blocks(in[s].size()), 64, [&] { k_sc_gather(one, t.local[s].data() + (mode == kPeer ? 0 : below)); });
-    below += in[s].size();
-  }
-  t.reduce();
+  SimTables t(mode, R, n.data(), sizeof(unsigned long long));
+  for (int s = 0; s < R; ++s)
+    if (n[s]) launch(blocks(n[s]), 64, [&] { k_gather_segments(one_segment(in[s].data(), n[s]), t.local(s)); });
+  const PeerTables view = t.publish();
   std::vector<std::vector<unsigned long long>> out(R, std::vector<unsigned long long>(total));
   for (int r = 0; r < R; ++r) {
-    ScReadSet<unsigned long long> rs;
-    std::memset(&rs, 0, sizeof rs);
-    if (mode == kPeer) { for (int s = 0; s < R; ++s) { rs.src[s] = t.read(s); rs.begin[s + 1] = rs.begin[s] + in[s].size(); } rs.n = R; }
-    else { rs.n = 1; rs.src[0] = t.read(0); rs.begin[1] = total; }
-    launch(blocks(total), 64, [&] { k_sc_gather(rs, out[r].data()); });
+    launch(blocks(total), 64, [&] { k_gather_segments(table_runs<unsigned long long>(view, n.data()), out[r].data()); });
     if (r) CHECK(out[r] == out[0], "allgather: rank %d differs", r);
   }
   return out[0];
@@ -157,16 +132,11 @@ static void run_case(const char* scene, const char* part, const std::vector<std:
     o.count = cnt.data() + (size_t)R * s;
     launch(3, 64, [&] { k_halo_select(rk[s].pts.data(), rk[s].pts.size(), boxes.data(), R, s, o); });
   }
-  auto sent = [&](int s, int r) { return s == r ? 0ull : cnt[(size_t)s * R + r]; };
-  unsigned long long most = 0, all = 0, most_in = 0;
-  for (int s = 0; s < R; ++s) {
-    unsigned long long out = 0, in = 0;
-    for (int r = 0; r < R; ++r) { out += sent(s, r); in += sent(r, s); }
-    most = std::max(most, out);
-    most_in = std::max(most_in, in);
-    all += out;
-  }
-  std::vector<std::vector<float4>> table(R, std::vector<float4>(std::max<unsigned long long>(mode == kPeer ? most : all, 1), make_float4(0.f, 0.f, 0.f, 0.f)));
+  unsigned long long all = 0;
+  for (int s = 0; s < R; ++s)
+    for (int r = 0; r < R; ++r) all += s == r ? 0ull : cnt[(size_t)s * R + r];
+  const std::vector<unsigned long long> n_table = segment_table_sizes(cnt.data(), R);
+  SimTables halo(mode, R, n_table.data(), sizeof(float4));
   for (int s = 0; s < R; ++s) {
     Rank& k = rk[s];
     const size_t n_tile = cnt[(size_t)s * R + s];
@@ -176,57 +146,19 @@ static void run_case(const char* scene, const char* part, const std::vector<std:
     std::memset(&o, 0, sizeof o);
     o.count = cursor.data();
     o.dst[s] = k.local.data();
-    unsigned long long at = 0;
-    for (int r = 0; r < R; ++r)
-      for (int x = mode == kPeer ? s : 0; x < (mode == kPeer ? s + 1 : R); ++x) {
-        if (x == s && r != s) o.dst[r] = table[s].data() + at;
-        at += sent(x, r);
-      }
+    segment_writes(reinterpret_cast<float4*>(halo.local(s)), cnt.data(), R, s, o.dst);
     launch(3, 64, [&] { k_halo_select(k.pts.data(), k.pts.size(), boxes.data(), R, s, o); });
-    // this rank's own segments, by destination (the HaloTrace's sent ids)
-    for (int r = 0; r < R; ++r)
-      if (r != s)
-        for (unsigned long long i = 0; i < sent(s, r); ++i) k.sent_ids.push_back((unsigned)id_of(o.dst[r][i]));
+    // this rank's own segments, one run at the start of its table (the HaloTrace's sent ids)
+    k.sent_ids.assign(n_table[s], 0);
+    if (n_table[s]) launch((unsigned)((n_table[s] + 255) / 256), 256, [&] { k_halo_ids(reinterpret_cast<const float4*>(halo.local(s)), n_table[s], k.sent_ids.data()); });
   }
-  std::vector<float4> global;
-  if (mode == kNccl) {
-    global.assign(table[0].size(), make_float4(0.f, 0.f, 0.f, 0.f));
-    for (int s = 0; s < R; ++s)
-      for (size_t i = 0; i < global.size(); ++i) {
-        unsigned long long a[2], b[2];
-        std::memcpy(a, &global[i], 16);
-        std::memcpy(b, &table[s][i], 16);
-        a[0] += b[0];
-        a[1] += b[1];
-        std::memcpy(&global[i], a, 16);
-      }
-  }
+  const PeerTables halo_view = halo.publish();
   for (int r = 0; r < R; ++r) {
     Rank& k = rk[r];
-    HaloReadSet rs;
-    std::memset(&rs, 0, sizeof rs);
-    unsigned long long halo = 0;
-    for (int s = 0; s < R; ++s) halo += sent(s, r);
-    if (mode == kPeer) {
-      for (int s = 0; s < R; ++s) {
-        if (s == r) continue;
-        unsigned long long off = 0;
-        for (int x = 0; x < r; ++x) off += sent(s, x);
-        rs.src[rs.n] = table[s].data() + off;
-        rs.begin[rs.n + 1] = rs.begin[rs.n] + sent(s, r);
-        ++rs.n;
-      }
-    }
-    else {
-      unsigned long long off = 0;
-      for (int x = 0; x < r; ++x) for (int s = 0; s < R; ++s) off += sent(s, x);
-      rs.n = 1;
-      rs.src[0] = global.data() + off;
-      rs.begin[1] = halo;
-    }
+    const PeerSegments<float4> rs = segment_reads<float4>(halo_view, cnt.data(), R, r);
     const size_t n_tile = k.local.size();
-    k.local.resize(n_tile + halo);
-    if (halo) launch(2, 64, [&] { k_halo_gather(rs, k.local.data() + n_tile); });
+    k.local.resize(n_tile + rs.begin[rs.n]);
+    if (rs.begin[rs.n]) launch(2, 64, [&] { k_gather_segments(rs, k.local.data() + n_tile); });
     for (size_t i = n_tile; i < k.local.size(); ++i) k.recv_ids.push_back((unsigned)id_of(k.local[i]));
     // the local map: sorted by id, each id once, indexed; then the unchanged clustering kernels
     std::map<unsigned, float4> lm;
@@ -249,27 +181,19 @@ static void run_case(const char* scene, const char* part, const std::vector<std:
     launch(blocks(m), 64, [&] { k_sc_label_ids(k.lab.data(), k.local_ids.data(), m, k.lab_id.data()); });
   }
   // ---- stitch: the answers, then the edges ----
-  auto run_of = [&](int r) { unsigned long long off = 0; for (int x = 0; x < r; ++x) for (int s = 0; s < R; ++s) off += sent(s, x); return off; };
+  const std::vector<unsigned long long> ans = segment_answers(cnt, R);
+  const std::vector<unsigned long long> n_ans = segment_table_sizes(ans.data(), R);
   if (all) {
-    Tables t(mode, R, (size_t)((mode == kPeer ? most_in : all) + 1) / 2);
+    SimTables t(mode, R, n_ans.data(), sizeof(unsigned));
     for (int r = 0; r < R; ++r) {
-      unsigned* mine = reinterpret_cast<unsigned*>(t.local[r].data());
+      unsigned* mine = reinterpret_cast<unsigned*>(t.local(r));
       if (!rk[r].recv_ids.empty())
-        launch(blocks(rk[r].recv_ids.size()), 64, [&] { k_sc_answer(rk[r].recv_ids.data(), rk[r].recv_ids.size(), rk[r].local_ids.data(), rk[r].local_ids.size(), rk[r].lab_id.data(), mode == kPeer ? mine : mine + run_of(r)); });
+        launch(blocks(rk[r].recv_ids.size()), 64, [&] { k_sc_answer(rk[r].recv_ids.data(), rk[r].recv_ids.size(), rk[r].local_ids.data(), rk[r].local_ids.size(), rk[r].lab_id.data(), mine); });
     }
-    t.reduce();
+    const PeerTables view = t.publish();
     for (int me = 0; me < R; ++me) {
       Rank& k = rk[me];
-      ScReadSet<unsigned> rs;
-      std::memset(&rs, 0, sizeof rs);
-      for (int r = 0; r < R; ++r) {
-        if (r == me) continue;
-        unsigned long long off = mode == kPeer ? 0 : run_of(r);
-        for (int s = 0; s < me; ++s) off += sent(s, r);
-        rs.src[rs.n] = reinterpret_cast<const unsigned*>(t.read(r)) + off;
-        rs.begin[rs.n + 1] = rs.begin[rs.n] + sent(me, r);
-        ++rs.n;
-      }
+      const PeerSegments<unsigned> rs = segment_reads<unsigned>(view, ans.data(), R, me);
       k.edges.assign(k.sent_ids.size(), 0);
       if (!k.sent_ids.empty())
         launch(blocks(k.sent_ids.size()), 64, [&] { k_sc_edges(k.sent_ids.data(), k.sent_ids.size(), k.local_ids.data(), k.local_ids.size(), k.lab_id.data(), rs, k.edges.data()); });
@@ -299,21 +223,16 @@ static void run_case(const char* scene, const char* part, const std::vector<std:
     const size_t m = k.local_ids.size();
     std::vector<unsigned char> dup(m, 0);
     local_cnt[r].assign(m, 0);
-    unsigned long long lower = 0;
-    for (int s = 0; s < r; ++s) lower += sent(s, r);
+    const unsigned long long lower = segment_start(ans.data(), R, r, r);
     if (lower) launch(blocks(lower), 64, [&] { k_sc_mark_lower(k.recv_ids.data(), lower, k.local_ids.data(), m, dup.data()); });
     launch(blocks(k.pts.size()), 64, [&] { k_sc_count(k.pts.data(), k.pts.size(), k.local_ids.data(), m, k.lab.data(), k.lab_id.data(), dup.data(), nodes.data(), n_nodes, node_cnt[r].data(), local_cnt[r].data()); });
   }
   std::vector<unsigned long long> comp(n_nodes, 0), node_sum(n_nodes, 0);
   if (n_nodes) {
-    Tables t(mode, R, n_nodes);
-    for (int r = 0; r < R; ++r) t.local[r] = node_cnt[r];
-    t.reduce();
-    ScReadSet<unsigned long long> tables;
-    std::memset(&tables, 0, sizeof tables);
-    if (mode == kPeer) { tables.n = R; for (int s = 0; s < R; ++s) tables.src[s] = t.read(s); }
-    else { tables.n = 1; tables.src[0] = t.read(0); }
-    launch(blocks(n_nodes), 64, [&] { k_sc_sum(tables, n_nodes, node_sum.data()); });
+    SimTables t(mode, R, n_nodes);
+    for (int r = 0; r < R; ++r) std::copy(node_cnt[r].begin(), node_cnt[r].end(), t.local(r));
+    const PeerTables view = t.publish();
+    launch(blocks(n_nodes), 64, [&] { k_sc_sum(peer_table_set(view), n_nodes, node_sum.data()); });
     launch(blocks(n_nodes), 64, [&] { k_sc_fold(node_sum.data(), n_nodes, root.data(), comp.data()); });
   }
   long bad = 0;

@@ -1,7 +1,8 @@
 // shard_normals_host_test.cpp — the halo kernels of normal estimation over a sharded map (pcl_b200/csrc/
 // shard_normals_kernels.cuh) compiled for the HOST and run in shard_normals.cu's sequence for R = 1, 2, 3, 5, 8 simulated
 // ranks in one process: this program does the cross-rank steps comm.cu would do (the u64 minimum of the boxes, the sum of
-// the counts, the peer tables or the NCCL sum of the global table).  For every rank it checks
+// the counts, the tables of peer_tables_sim.h), and places the segments with the layout functions of peer_tables.cuh that
+// the driver calls.  For every rank it checks
 //   - the box: the u64 fold of k_halo_box equals a reference fold of the outward-rounded boxes of its finite queries;
 //   - the halo: exactly the points of the other tiles inside that box (a brute-force selection), each once per sender,
 //     under both exchange protocols, and the tile itself is counted whole;
@@ -22,6 +23,8 @@ template <typename T> static inline T __ldcv(const T* p) { return *p; }
 static inline unsigned long long atomicMin(unsigned long long* p, unsigned long long v) { const unsigned long long o = *p; if (v < o) *p = v; return o; }
 
 #include "../../pcl_b200/csrc/shard_normals_kernels.cuh"
+#include "../../pcl_b200/csrc/peer_tables.cuh"
+#include "peer_tables_sim.h"
 
 static long g_checks = 0, g_fail = 0;
 #define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
@@ -86,8 +89,6 @@ static bool in_ref(const RefBox& b, const float4& p)
   return b.any && p.x >= b.lo[0] && p.x <= b.hi[0] && p.y >= b.lo[1] && p.y <= b.hi[1] && p.z >= b.lo[2] && p.z <= b.hi[2];
 }
 
-enum { kPeer = 0, kNccl = 1 };
-
 // One scene, one partition, one neighbourhood (k > 0, or r2): every rank's halo by both protocols, checked.
 static void run_case(const char* name, const std::vector<std::vector<float4>>& tiles,
                      const std::vector<std::vector<float4>>& queries, int k, float r2, int mode, std::mt19937& rng)
@@ -138,17 +139,15 @@ static void run_case(const char* name, const std::vector<std::vector<float4>>& t
     launch(3, 64, [&] { k_halo_select(idx_pts[s].data(), idx_pts[s].size(), boxes.data(), R, s, o); });
   }
   auto sent = [&](int s, int r) { return s == r ? 0ull : cnt[(size_t)s * R + r]; };
-  unsigned long long most = 0, all = 0;
+  unsigned long long all = 0;
   for (int s = 0; s < R; ++s) {
-    unsigned long long out = 0;
-    for (int r = 0; r < R; ++r) out += sent(s, r);
-    most = std::max(most, out);
-    all += out;
+    for (int r = 0; r < R; ++r) all += sent(s, r);
     CHECK(cnt[(size_t)s * R + s] == tiles[s].size(), "%s R=%d rank %d: tile counted %llu of %zu", name, R, s,
           cnt[(size_t)s * R + s], tiles[s].size());
   }
-  // publish: peer tables (segments by destination) or one global table ordered by (destination, source)
-  std::vector<std::vector<float4>> table(R, std::vector<float4>(std::max<unsigned long long>(mode == kPeer ? most : all, 1)));
+  // publish: every rank writes its segments, by destination, into its table of comm_segment_tables
+  const std::vector<unsigned long long> n_table = segment_table_sizes(cnt.data(), R);
+  SimTables t(mode, R, n_table.data(), sizeof(float4));
   std::vector<std::vector<float4>> local(R);
   for (int s = 0; s < R; ++s) {
     local[s].assign(tiles[s].size(), make_float4(0.f, 0.f, 0.f, 0.f));
@@ -157,55 +156,18 @@ static void run_case(const char* name, const std::vector<std::vector<float4>>& t
     std::memset(&o, 0, sizeof o);
     o.count = cursor.data();
     o.dst[s] = local[s].data();
-    unsigned long long at = 0;
-    for (int r = 0; r < R; ++r)
-      for (int x = mode == kPeer ? s : 0; x < (mode == kPeer ? s + 1 : R); ++x) {
-        if (x == s && r != s) o.dst[r] = table[s].data() + at;
-        at += sent(x, r);
-      }
+    segment_writes(reinterpret_cast<float4*>(t.local(s)), cnt.data(), R, s, o.dst);
     launch(3, 64, [&] { k_halo_select(idx_pts[s].data(), idx_pts[s].size(), boxes.data(), R, s, o); });
     for (int r = 0; r < R; ++r)
       CHECK(cursor[r] == (r == s ? tiles[s].size() : sent(s, r)), "%s R=%d rank %d: wrote %llu to rank %d", name, R, s,
             cursor[r], r);
   }
-  std::vector<float4> global;
-  if (mode == kNccl) {  // u64 sum of the tables, each word written by one rank, zero elsewhere
-    global.assign(table[0].size(), make_float4(0.f, 0.f, 0.f, 0.f));
-    for (int s = 0; s < R; ++s)
-      for (size_t i = 0; i < global.size(); ++i) {
-        unsigned long long a[2], b[2];
-        std::memcpy(a, &global[i], 16);
-        std::memcpy(b, &table[s][i], 16);
-        a[0] += b[0];
-        a[1] += b[1];
-        std::memcpy(&global[i], a, 16);
-      }
-  }
+  const PeerTables view = t.publish();
   long bad = 0;
   for (int r = 0; r < R; ++r) {
-    HaloReadSet rs;
-    std::memset(&rs, 0, sizeof rs);
-    unsigned long long halo = 0;
-    for (int s = 0; s < R; ++s) halo += sent(s, r);
-    if (mode == kPeer) {
-      for (int s = 0; s < R; ++s) {
-        if (s == r) continue;
-        unsigned long long off = 0;
-        for (int x = 0; x < r; ++x) off += sent(s, x);
-        rs.src[rs.n] = table[s].data() + off;
-        rs.begin[rs.n + 1] = rs.begin[rs.n] + sent(s, r);
-        ++rs.n;
-      }
-    }
-    else {
-      unsigned long long off = 0;
-      for (int x = 0; x < r; ++x) for (int s = 0; s < R; ++s) off += sent(s, x);
-      rs.n = 1;
-      rs.src[0] = global.data() + off;
-      rs.begin[1] = halo;
-    }
-    local[r].resize(tiles[r].size() + halo);
-    launch(2, 64, [&] { k_halo_gather(rs, local[r].data() + tiles[r].size()); });
+    const PeerSegments<float4> rs = segment_reads<float4>(view, cnt.data(), R, r);
+    local[r].resize(tiles[r].size() + rs.begin[rs.n]);
+    launch(2, 64, [&] { k_gather_segments(rs, local[r].data() + tiles[r].size()); });
     // the tile part: the tile, every point once
     std::multiset<int> got_tile, want_tile;
     for (size_t i = 0; i < tiles[r].size(); ++i) { got_tile.insert(id_of(local[r][i])); want_tile.insert(id_of(tiles[r][i])); }

@@ -153,20 +153,19 @@ static void run_case(const char* name, const std::vector<std::vector<MapPoint>>&
         const Best b = argmin(tiles[r], q[i], -1.f);
         fk[r][i] = b.at < 0 ? kNoShardMatch : (((unsigned long long)__float_as_uint(b.d2) << 32) | (unsigned)b.id);
       }
-    ShardReadSet fs;
-    std::memset(&fs, 0, sizeof fs);
+    PeerTables fs;
     std::vector<unsigned long long> fmin(n);
-    if (mode == kPeer) { fs.n = R; for (int r = 0; r < R; ++r) fs.key[r] = fk[r].data(); }
+    if (mode == kPeer) { fs.n_read = R; for (int r = 0; r < R; ++r) fs.read[r] = fk[r].data(); }
     else {
       for (size_t i = 0; i < n; ++i) { unsigned long long m = ~0ull; for (int r = 0; r < R; ++r) m = std::min(m, fk[r][i]); fmin[i] = m; }
-      fs.n = 1;
-      fs.key[0] = fmin.data();
+      fs.n_read = 1;
+      fs.read[0] = fmin.data();
     }
     const unsigned grid = 3;
     std::vector<double> partials(grid * kAccum, 0.0), accum(kAccum, -1.0);
     unsigned counter = 0;
     const GridSum sum{partials.data(), &counter, accum.data()};
-    launch(grid, 256, [&] { k_fitness_reduce(fs, n, max_range, sum); });
+    launch(grid, 256, [&] { k_fitness_reduce(peer_table_set(fs), n, max_range, sum); });
     double cnt = 0, s = 0;
     for (size_t i = 0; i < n; ++i) {
       const Best t = argmin(whole, q[i], -1.f);

@@ -16,8 +16,9 @@ HOST = os.path.join(ROOT, "tests", "host")
 
 @pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
                     reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
-def test_sharded_cluster_kernels_on_the_host(tmp_path):
-    """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols: every rank's labels and sizes equal a brute-force
+def test_sharded_cluster_kernels_and_layout_on_the_host(tmp_path):
+    """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols, the halo, the answers and the edges placed and read with
+    the layout functions of peer_tables.cuh that the driver calls: every rank's labels and sizes equal a brute-force
     connected-components of the whole map — a zig-zag chain crossing every slab boundary many times, blobs on the
     boundaries, a lattice at and just above the tolerance, duplicated points, non-finite records, ids near 2^31 - 2,
     tolerance 0; slabs, a random partition, overlapping tiles sharing ids and a 1-point tile."""

@@ -15,8 +15,9 @@ HOST = os.path.join(ROOT, "tests", "host")
 
 @pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
                     reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
-def test_sharded_normals_halo_kernels_on_the_host(tmp_path):
-    """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols: every rank's box is the outward-rounded union of its
+def test_sharded_normals_halo_layout_on_the_host(tmp_path):
+    """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols, the segments placed and read with the layout functions
+    of peer_tables.cuh that the driver calls: every rank's box is the outward-rounded union of its
     queries' reaches, its halo is exactly the other tiles' points inside that box, and every whole-map neighbour of every
     query (ties at the k-th distance included; radius: d2 <= r^2) lies in the tile plus the halo — slabs, a random
     partition, overlapping tiles sharing ids, a far tile with fewer than k points, k = 3 / 16 / 40 and a radius."""

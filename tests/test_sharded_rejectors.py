@@ -55,9 +55,9 @@ def test_sharded_rejector_chains_two_gpus_nccl():
 
 @pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
                     reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
-def test_sharded_rejector_kernels_on_the_host(tmp_path):
+def test_sharded_rejector_table_sets_on_the_host(tmp_path):
     """reject_sharded_kernels.cuh compiled for the host, 1 / 2 / 3 / 5 / 8 simulated ranks (the program sums the histograms
-    and min-reduces the one-to-one tables itself, both one-to-one protocols): the union of the survivors equals the oracle's
+    and min-reduces the one-to-one tables itself, both one-to-one protocols, read through peer_table_set): the union of the survivors equals the oracle's
     rejector on the concatenation for every rejector, trimmed with keep = 0, 1, c - 1, c, and four chains; runs of exact
     ties, ranks with no accepted entry, array order unlike slot order."""
     import oracle

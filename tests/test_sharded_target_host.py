@@ -13,10 +13,10 @@ HOST = os.path.join(ROOT, "tests", "host")
 
 @pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
                     reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
-def test_sharded_target_kernels_on_the_host(tmp_path):
+def test_sharded_target_table_sets_on_the_host(tmp_path):
     """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols: the gathered match and record of every query equal the
     brute-force (d2, id) argmin over the whole map — exact ties across ranks, ids near 2^31 - 1, a rank out of reach, a
-    random partition, points held by two ranks — and the fitness reduction counts exactly."""
+    random partition, points held by two ranks — and the fitness reduction, reading the keys through peer_table_set, counts exactly."""
     exe = str(tmp_path / "shard_target_host_test")
     subprocess.check_call(["g++", "-O1", "-std=c++17", "-frounding-math", "-ffp-contract=off", "-fno-fast-math",
                            "-I" + CUDA_INC, "-I" + os.path.join(ROOT, "include"), "-I" + HOST,
