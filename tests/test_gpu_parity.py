@@ -16,6 +16,15 @@ def gpu():
     ctx.close()
 
 
+def _reference(cloud, queries, vp, **kw):
+    """The per-query extended-precision reference of tests/test_normals_reference.py."""
+    import os
+    import sys
+    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+    import test_normals_reference
+    return test_normals_reference.Reference(cloud, queries, vp, **kw)
+
+
 def _clouds(rng):
     yield "uniform", rng.random((20000, 3), dtype=np.float32)
     g = np.stack(np.meshgrid(*[np.arange(13, dtype=np.float32)] * 3, indexing="ij"), -1).reshape(-1, 3)
@@ -82,9 +91,7 @@ def test_knn_and_normals_many_k(gpu, orc):
         g, gd = P.Index(ctx, cloud).normals_knn(cloud, k, viewpoint=(0.5, 0.5, 5), is_dense=False)
         o, od = orc.Index(cloud).normals_knn(cloud, k, viewpoint=(0.5, 0.5, 5), is_dense=False, nthreads=8)
         assert gd == od and np.array_equal(np.isnan(g[:, 0]), np.isnan(o[:, 0]))
-        ok = ~np.isnan(o[:, 0])
-        cosang = (g[ok, :3] * o[ok, :3]).sum(1)
-        assert np.percentile(cosang, 0.5) > 1 - 1e-3 and np.mean(cosang > 1 - 1e-6) > 0.9, (k, walk)
+        _reference(cloud, cloud, (0.5, 0.5, 5), k=k).check(g, f"k={k} {walk}")
 
 
 def test_knn_warp_kernel_mixed_density_every_query(gpu, orc):
@@ -437,9 +444,7 @@ def test_normals_vs_oracle(gpu, orc):
         g, gd = P.Index(ctx, cloud).normals_knn(cloud, k, viewpoint=(0.5, 0.5, 5))
         o, od = orc.Index(cloud).normals_knn(cloud, k, viewpoint=(0.5, 0.5, 5), nthreads=8)
         assert gd == od
-        cosang = (g[:, :3] * o[:, :3]).sum(1)
-        assert np.percentile(cosang, 0.5) > 1 - 1e-3 and np.mean(cosang > 1 - 1e-6) > 0.9, k
-        assert np.allclose(g[:, 3], o[:, 3], atol=5e-3)
+        _reference(cloud, cloud, (0.5, 0.5, 5), k=k).check(g, f"k={k}")  # every normal and curvature
     few = orc.to_xyz1(pts[:2])
     g, gd = P.Index(ctx, few).normals_knn(few, 5)
     assert not gd and np.isnan(g).all()  # < 3 neighbours => NaN, is_dense false (normal_3d.hpp:62-69)
