@@ -171,6 +171,18 @@ int main(int argc, char** argv)
     run_scene("mixed density, k 24", mix, q, 24, 6, 5, 0.02f, 1.0);
   }
   {
+    // map-scale frames: a 200 m map at 1e5 on the 1/128 m grid of its ulp (exact ties), a frame straddling zero (x - lo
+    // rounds), a 1 m cube stretched by one point 1e6 away (every table level holds the cube in one cell)
+    const auto map = cloud(4000 * scale, [&](int, float* p) { p[0] = 1e5f + 200.f * U(rng); p[1] = 1e5f + 200.f * U(rng); p[2] = std::round(256.f * std::sin((p[0] - 1e5f) / 15.f)) / 128.f; });
+    run_scene("map at 1e5", map, self_and_off(map, 96 * scale, 32 * scale), 16, 6, 4, 0.f, 1.0);
+    const auto straddle = cloud(4000 * scale, [&](int, float* p) { p[0] = -3e4f + 6e4f * U(rng); p[1] = 20.f * U(rng); p[2] = 3.f * std::sin(p[0] / 40.f); });
+    run_scene("straddling zero", straddle, self_and_off(straddle, 96 * scale, 32 * scale), 24, 6, 5, 0.f, 1.0);
+    auto outlier = cloud(3000, [&](int, float* p) { p[0] = U(rng); p[1] = U(rng); p[2] = U(rng); });
+    const auto cube = outlier;
+    outlier.insert(outlier.end(), {1e6f, 0.5f, 0.5f});
+    run_scene("one outlier 1e6 away", outlier, self_and_off(cube, 32, 16), 16, 6, 4, 0.f, 1.0);
+  }
+  {
     // exact ties (a lattice) and duplicates: the (d2, index) order decides
     std::vector<float> lat;
     for (int x = 0; x < 14; ++x) for (int y = 0; y < 14; ++y) for (int z = 0; z < 14; ++z) { lat.push_back(0.1f * x); lat.push_back(0.1f * y); lat.push_back(0.1f * z); }

@@ -159,6 +159,15 @@ int main(int argc, char** argv)
     for (int x = 0; x < 13; ++x) for (int y = 0; y < 13; ++y) for (int z = 0; z < 13; ++z) { lat.push_back((float)x); lat.push_back((float)y); lat.push_back((float)z); }
     run_scene("lattice", lat);
   }
+  // map-scale frames: a 200 m map at 1e5 on the 1/128 m grid of its ulp, a frame straddling zero, a 1 m cube stretched by
+  // one point 1e6 away (runs of equal Morton codes far beyond a leaf)
+  run_scene("map at 1e5", cloud(4000 * scale, [&](int, float* p) { p[0] = 1e5f + 200.f * U(rng); p[1] = 1e5f + 200.f * U(rng); p[2] = std::round(256.f * std::sin((p[0] - 1e5f) / 15.f)) / 128.f; }));
+  run_scene("straddling zero", cloud(4000 * scale, [&](int, float* p) { p[0] = -3e4f + 6e4f * U(rng); p[1] = 20.f * U(rng); p[2] = 3.f * std::sin(p[0] / 40.f); }));
+  {
+    auto outlier = cloud(4000 * scale, [&](int, float* p) { p[0] = U(rng); p[1] = U(rng); p[2] = U(rng); });
+    outlier.insert(outlier.end(), {1e6f, 0.5f, 0.5f});
+    run_scene("one outlier 1e6 away", outlier, false);
+  }
   run_scene("collinear", cloud(1777, [&](int i, float* p) { p[0] = p[1] = p[2] = i / 1776.f; }));
   run_scene("planar, zero extent axis", cloud(3000, [&](int, float* p) { p[0] = U(rng); p[1] = 0.25f; p[2] = U(rng); }));
   run_scene("mixed density", cloud(4000 * scale, [&](int i, float* p) { p[0] = 2.f * U(rng); p[1] = 2.f * U(rng); p[2] = (i % 7) ? 1.f + 0.001f * N(rng) : 2.f * U(rng); }));

@@ -175,6 +175,18 @@ int main(int argc, char** argv)
     run_scene("surface, offset frame", cloud(4000 * scale, [&](int, float* p) { p[0] = 1000.f + 3.f * U(rng); p[1] = -500.f + 3.f * U(rng); p[2] = 20.f + 0.01f * N(rng); }),
               cloud(600 * scale, [&](int, float* p) { p[0] = 1000.f + 3.f * U(rng); p[1] = -500.f + 3.f * U(rng); p[2] = 20.f + 0.05f * N(rng); }), no_gate, 5);
   }
+  {  // map-scale frames: a 200 m map at 1e5 on the 1/128 m grid of its ulp (exact ties), a frame straddling zero (x - lo
+     // rounds), a 1 m cube stretched by one point 1e6 away (runs of equal Morton codes far beyond a leaf)
+    const auto map = cloud(4000 * scale, [&](int, float* p) { p[0] = 1e5f + 200.f * U(rng); p[1] = 1e5f + 200.f * U(rng); p[2] = std::round(256.f * std::sin((p[0] - 1e5f) / 15.f)) / 128.f; });
+    run_scene("map at 1e5", map, near_queries(map, 800 * scale, 1.f, 0.05f), no_gate, 6);
+    run_scene("map at 1e5, gate", map, near_queries(map, 400 * scale, 2.f, 0.05f), 9.f, 6);
+    const auto straddle = cloud(4000 * scale, [&](int, float* p) { p[0] = -3e4f + 6e4f * U(rng); p[1] = 20.f * U(rng); p[2] = 3.f * std::sin(p[0] / 40.f); });
+    run_scene("straddling zero", straddle, near_queries(straddle, 800 * scale, 5.f, 0.05f), no_gate, 6);
+    auto outlier = cloud(4000 * scale, [&](int, float* p) { p[0] = U(rng); p[1] = U(rng); p[2] = U(rng); });
+    const auto cube = outlier;
+    outlier.insert(outlier.end(), {1e6f, 0.5f, 0.5f});
+    run_scene("one outlier 1e6 away", outlier, near_queries(cube, 800 * scale, 0.01f, 0.05f), no_gate, 6);
+  }
   {
     std::vector<float> base = cloud(400, [&](int, float* p) { p[0] = U(rng); p[1] = U(rng); p[2] = U(rng); });
     std::vector<float> pts;

@@ -64,52 +64,104 @@ def _valid(cloud):
     return xyz, ids
 
 
-def knn_sets(cloud, queries, k):
+def d2_fp64(q, P):
+    """The squared distance of the same float points in double: what the fp32 rule must not be confused with."""
+    d = P.astype(np.float64) - q.astype(np.float64)[..., None, :]
+    return (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]
+
+
+def knn_sets(cloud, queries, k, return_d2=False, dist=d2_fp32, tie=1):
     """(nq, k) original indices of the k nearest finite points of every query by (fp32 d2, index), -1 past the number
-    of finite points and for non-finite queries.  A kd-tree proposes candidates; the fp32 rule selects them."""
+    of finite points and for non-finite queries; with return_d2 also their d2 as float32 (+inf where the index is -1).
+    A kd-tree proposes candidates; the fp32 rule selects them.  Smaller k are prefixes of the result.
+
+    dist and tie replace the distance rule and the tie order (tie = -1: (d2, -index)); they exist to show that the
+    scenes of tests/test_search_reference.py depend on both."""
     xyz, ids = _valid(cloud)
     q = np.asarray(queries, dtype=np.float32)[:, :3]
     nq = q.shape[0]
     out = np.full((nq, k), -1, dtype=np.int64)
+    od = np.full((nq, k), np.inf, dtype=np.float32)
     keff = min(k, ids.size)
     if keff == 0:
-        return out
+        return (out, od) if return_d2 else out
     tree = cKDTree(xyz[ids].astype(np.float64))
+
+    def take(rows, oi):
+        d2 = dist(q[rows], xyz[oi])
+        order = np.lexsort((tie * oi, d2), axis=-1)
+        oi, d2 = np.take_along_axis(oi, order, 1), np.take_along_axis(d2, order, 1)
+        out[rows, :keff] = oi[:, :keff]
+        od[rows, :keff] = d2[:, :keff]
+
     todo = np.nonzero(np.isfinite(q).all(1))[0]
     m = min(keff + 8, ids.size)
     while todo.size:
-        dist, cand = tree.query(q[todo].astype(np.float64), m)
-        dist, cand = dist.reshape(todo.size, m), cand.reshape(todo.size, m)
-        oi = ids[cand]
-        d2 = d2_fp32(q[todo], xyz[oi])
-        order = np.lexsort((oi, d2), axis=-1)
-        oi, d2 = np.take_along_axis(oi, order, 1), np.take_along_axis(d2, order, 1)
-        # complete when every point outside the candidates is provably farther than the k-th (fp32 d2 is within a
-        # few ulp of the exact squared distance)
-        done = (m == ids.size) | (d2[:, keff - 1].astype(np.float64) < dist[:, -1] ** 2 * (1 - 1e-5))
-        out[todo[done], :keff] = oi[done, :keff]
-        todo = todo[~done]
+        if 4 * m >= ids.size:
+            # the rest against every point (queries far from a compact cloud, where all points are nearly equidistant)
+            for a in range(0, todo.size, max(1, (1 << 22) // ids.size)):
+                rows = todo[a:a + max(1, (1 << 22) // ids.size)]
+                take(rows, np.broadcast_to(ids, (rows.size, ids.size)))
+            break
+        left = []
+        for a in range(0, todo.size, max(1, (1 << 23) // m)):
+            rows = todo[a:a + max(1, (1 << 23) // m)]
+            dst, cand = tree.query(q[rows].astype(np.float64), m, workers=-1)
+            dst, cand = dst.reshape(rows.size, m), cand.reshape(rows.size, m)
+            oi = ids[cand]
+            d2 = dist(q[rows], xyz[oi])
+            # complete when every point outside the candidates is provably farther than the k-th (fp32 d2 is within a
+            # few ulp of the exact squared distance)
+            done = (m == ids.size) | (np.sort(d2, 1)[:, keff - 1].astype(np.float64) < dst[:, -1] ** 2 * (1 - 1e-5))
+            # all m candidates coincide with the query (more than k + 8 exact duplicates): the k-th is at d2 = 0 and
+            # the order among the duplicates is the index order, so gather every point at d2 = 0 and keep the first k
+            dup = ~done & (dst[:, -1] == 0)
+            if done.any():
+                take(rows[done], oi[done])
+            for i in np.nonzero(dup)[0]:
+                z = ids[np.asarray(tree.query_ball_point(q[rows[i]].astype(np.float64), 1e-20), dtype=np.int64)]
+                z = z[dist(q[rows[i]], xyz[z]) == 0]
+                z = np.sort(tie * z) * tie
+                out[rows[i], :keff] = z[:keff]
+                od[rows[i], :keff] = 0
+            left.append(rows[~(done | dup)])
+        todo = np.concatenate(left)
         m = min(2 * m, ids.size)
-    return out
+    return (out, od) if return_d2 else out
+
+
+def radius_csr(cloud, queries, radius, max_nn=0):
+    """Every finite point with fp32 d2 < float(radius * radius) per query, by (d2, index), as CSR (offsets (nq + 1),
+    original indices, d2); max_nn > 0 keeps the max_nn nearest of each row (KdTreeFLANN::radiusSearch)."""
+    xyz, ids = _valid(cloud)
+    q = np.asarray(queries, dtype=np.float32)[:, :3]
+    nq = q.shape[0]
+    r2 = np.float32(radius * radius)
+    tree = cKDTree(xyz[ids].astype(np.float64))
+    fin = np.nonzero(np.isfinite(q).all(1))[0]
+    lists = tree.query_ball_point(q[fin].astype(np.float64), radius * (1 + 1e-5) + 1e-30, workers=-1,
+                                  return_sorted=False) if fin.size else []
+    lens = np.fromiter((len(x) for x in lists), dtype=np.int64, count=len(lists))
+    row = np.repeat(fin, lens)
+    oi = ids[np.concatenate([np.asarray(x, dtype=np.int64) for x in lists]) if lens.sum() else np.zeros(0, np.int64)]
+    d2 = d2_fp32(q[row], xyz[oi][:, None, :])[:, 0] if row.size else np.zeros(0, np.float32)
+    keep = d2 < r2
+    row, oi, d2 = row[keep], oi[keep], d2[keep]
+    order = np.lexsort((oi, d2, row))
+    row, oi, d2 = row[order], oi[order], d2[order]
+    if 0 < max_nn < ids.size:
+        start = np.searchsorted(row, row, side="left")
+        keep = np.arange(row.size) - start < max_nn
+        row, oi, d2 = row[keep], oi[keep], d2[keep]
+    offsets = np.zeros(nq + 1, dtype=np.int64)
+    np.cumsum(np.bincount(row, minlength=nq), out=offsets[1:])
+    return offsets, oi, d2
 
 
 def radius_sets(cloud, queries, radius):
     """Per query, the original indices of every finite point with fp32 d2 < float(radius * radius), by (d2, index)."""
-    xyz, ids = _valid(cloud)
-    q = np.asarray(queries, dtype=np.float32)[:, :3]
-    r2 = np.float32(radius * radius)
-    tree = cKDTree(xyz[ids].astype(np.float64))
-    out = []
-    for i in range(q.shape[0]):
-        if not np.isfinite(q[i]).all():
-            out.append(np.zeros(0, np.int64))
-            continue
-        oi = ids[np.asarray(tree.query_ball_point(q[i].astype(np.float64), radius * (1 + 1e-5) + 1e-30), dtype=np.int64)]
-        d2 = d2_fp32(q[i], xyz[oi])
-        keep = d2 < r2
-        oi, d2 = oi[keep], d2[keep]
-        out.append(oi[np.lexsort((oi, d2))])
-    return out
+    offsets, oi, _ = radius_csr(cloud, queries, radius)
+    return [oi[offsets[i]:offsets[i + 1]] for i in range(offsets.size - 1)]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

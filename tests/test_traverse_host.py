@@ -36,18 +36,20 @@ def _run(tmp_path, source, args=(), defines=(), link=()):
 def test_index_build_kernels_on_the_host(tmp_path):
     """lbvh_kernels.cuh in lbvh.cu's sequence: every point in exactly one leaf slot, leaves of 1..8 points in Morton order,
     child boxes exact, subtree leaf ranges, and the cell table — every occupied cell of every level maps to a subtree that
-    holds all of (and, for a node, only) its points — on twelve clouds incl. duplicates, a lattice, degenerate frames."""
+    holds all of (and, for a node, only) its points — on fifteen clouds incl. duplicates, a lattice, degenerate frames and
+    map-scale frames (a map at 1e5, a frame straddling zero, a cube stretched by one outlier 1e6 away)."""
     out = _run(tmp_path, "lbvh_host_test.cpp", ["2"])
-    assert "cell table levels 1.." in out
+    assert "cell table levels 1.." in out and "map at 1e5" in out and "straddling zero" in out and "one outlier 1e6 away" in out
 
 
 @pytest.mark.parametrize("device_built", [False, True], ids=["reference-index", "device-built-index"])
 def test_device_traversal_header_on_the_host(tmp_path, device_built):
     """traverse.cuh (walk, nearest1, the cell-table look-ups and their conservative bounds, still_nearest): ~7e5 query
-    variants on eleven scene families against brute force — with and without the table, no / the true / a random seed,
+    variants on twelve scene families (map-scale frames among them) against brute force — with and without the table, no / the true / a random seed,
     the TRACK visitor's lower bound — and the temporal-coherence chain of k_search over drifting queries: a skipped walk
     never keeps a match that stopped being the nearest.  Five seeded mutations of the header are caught by this program."""
-    _run(tmp_path, "traverse_host_test.cpp", ["2"], DEVICE_BUILD if device_built else ())
+    out = _run(tmp_path, "traverse_host_test.cpp", ["2"], DEVICE_BUILD if device_built else ())
+    assert "map at 1e5" in out and "straddling zero" in out and "one outlier 1e6 away" in out
 
 
 @pytest.mark.parametrize("device_built", [False, True], ids=["reference-index", "device-built-index"])
@@ -66,7 +68,7 @@ def test_warp_knn_kernel_on_an_emulated_warp(tmp_path, device_built):
     host computePointNormal on the brute-force list, and (reference index) the constructed shared-leaf scene — the bug the
     10 M-row comparison found on the device — passes; it fails on the kernel as it was before the fix."""
     out = _run(tmp_path, "knn_warp_host_test.cpp", ["1"], DEVICE_BUILD if device_built else ())
-    assert "shared leaf, constructed #5" in out
+    assert "shared leaf, constructed #5" in out and "map at 1e5" in out and "straddling zero" in out and "one outlier 1e6 away" in out
 
 
 @pytest.mark.parametrize("device_built", [False, True], ids=["reference-index", "device-built-index"])
