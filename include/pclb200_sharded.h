@@ -22,7 +22,8 @@ extern "C" {
  * records of the cloud an index was built from refuses a labelled index (PCLB200_ERR_INVALID): the normal-based
  * correspondence estimators, normal estimation with k > 32 or a radius, GICP covariances, pclb200_cluster_labels.
  * The normals of a sharded map come from pclb200_normals_knn_sharded / pclb200_normals_radius_sharded, and the clusters
- * of a sharded map come from pclb200_cluster_labels_sharded. */
+ * of a sharded map come from pclb200_cluster_labels_sharded, its k-NN lists and outlier filters from pclb200_knn_sharded,
+ * pclb200_knn_stats_sharded, pclb200_statistical_outlier_sharded and pclb200_radius_outlier_sharded. */
 PCLB200_API int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                         const int32_t* ids, pclb200_index** out);
 
@@ -64,6 +65,49 @@ PCLB200_API int pclb200_normals_radius_sharded(pclb200_ctx* ctx, const pclb200_i
                                                size_t n, size_t stride, const int32_t* indices, size_t n_idx,
                                                int is_dense, double radius, const float viewpoint[3], float* out,
                                                int* is_dense_out);
+
+/* k-NN queries, k-NN statistics and the two outlier filters of a map sharded across the ranks of the context's
+ * communicator.  Collective: every rank passes its tile (built with pclb200_index_build_ids; the whole map is the union
+ * of the tiles' ids) and its OWN queries (any points; typically the tile's records, through an optional indices subset).
+ * Arrays may be host or device memory; a rank with no query still takes part.  Each rank fetches, from the other ranks'
+ * tiles, the points within its queries' k-th nearest distance in its own tile and indexes its tile plus those points:
+ * both are resident at the peak.  An id held by two ranks must name the same point.  PCLB200_ERR_INVALID on every rank,
+ * before any exchange, without an active communicator, for a tile built without ids, and for k <= 0 / mean_k <= 0 /
+ * min_pts < 0 / radius <= 0.
+ *
+ * pclb200_knn_sharded: row i (k entries of out_idx / out_d2) is, byte for byte, what pclb200_knn returns for query i
+ * against one index of the whole map (pclb200_index_build over the map with subset = the union of the ids): the ids, the
+ * d2, the (d2, id) order, the (-1, +inf) padding and the rows of non-finite queries.  *k_eff (nullable) is the whole
+ * map's clamp min(k, number of distinct finite ids), the same on every rank.
+ * pclb200_knn_stats_sharded: out_mean / out_kth (either nullable) are, byte for byte, pclb200_knn_stats on one index of
+ * the whole map. */
+PCLB200_API int pclb200_knn_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* queries, size_t nq,
+                                    size_t stride, int k, int32_t* out_idx, float* out_d2, int* k_eff);
+PCLB200_API int pclb200_knn_stats_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n,
+                                          size_t stride, const int32_t* indices, size_t n_idx, int k, float* out_mean,
+                                          float* out_kth);
+
+/* StatisticalOutlierRemoval (setMeanK(mean_k), setStddevMulThresh(std_mul), setNegative(negative)) over the concatenation
+ * of every rank's queries in rank order.  keep[i] (1 = kept) covers this rank's queries; stats (nullable) receives the
+ * number of finite queries, the mean and the threshold, the same on every rank.  The per-query mean distances are
+ * pclb200_knn_stats's with k = mean_k + 1 on the whole map, bit for bit.  The threshold is not bit for bit: the reference
+ * sums the means one after the other in record order, and here every rank sums its own in a fixed order, the ranks'
+ * partial sums travel exactly and every rank adds them up in rank order.  So every rank holds the same threshold, within
+ * fp64 round-off of one process's, and keep differs from one process's only for a query whose mean lies within that
+ * round-off of the threshold.  The statistics run over the queries as passed: a point two ranks hold under one id counts
+ * once only if just one of them passes it as a query. */
+PCLB200_API int pclb200_statistical_outlier_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts,
+                                                    size_t n, size_t stride, const int32_t* indices, size_t n_idx,
+                                                    int mean_k, double std_mul, int negative, uint8_t* keep,
+                                                    double stats[3]);
+
+/* RadiusOutlierRemoval (setRadiusSearch(radius), setMinNeighborsInRadius(min_pts), setNegative(negative)) of this rank's
+ * queries on the whole map: keep[i] (1 = kept) is, byte for byte, the reference's rule on pclb200_knn_stats with
+ * k = min_pts + 1.  The dense rule (the k-NN comparison) applies when every rank passes is_dense, else the radius rule
+ * (strict d2 < radius^2, non-finite queries removed) applies on every rank. */
+PCLB200_API int pclb200_radius_outlier_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts,
+                                               size_t n, size_t stride, const int32_t* indices, size_t n_idx,
+                                               int is_dense, double radius, int min_pts, int negative, uint8_t* keep);
 
 /* Euclidean clustering of a map sharded across the ranks of the context's communicator (collective: every rank passes its
  * tile, built with pclb200_index_build_ids; the whole map is the union of the tiles' ids).  n_labels is the number of

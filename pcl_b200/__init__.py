@@ -80,7 +80,8 @@ SYMBOLS = [
 # every symbol include/pclb200_sharded.h declares (the sharded-target extension; tests/test_sharded_target_symbols.py)
 SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", "pclb200_fitness_score_sharded",
                    "pclb200_normals_knn_sharded", "pclb200_normals_radius_sharded", "pclb200_cluster_labels_sharded",
-                   "pclb200_comm_allgather_u64"]
+                   "pclb200_comm_allgather_u64", "pclb200_knn_sharded", "pclb200_knn_stats_sharded",
+                   "pclb200_statistical_outlier_sharded", "pclb200_radius_outlier_sharded"]
 
 _lib = None
 
@@ -149,6 +150,10 @@ def lib():
     L.pclb200_cluster_labels.argtypes = [vp, vp, C.c_double, vp, sz]
     L.pclb200_cluster_labels_sharded.argtypes = [vp, vp, C.c_double, vp, vp, sz]
     L.pclb200_comm_allgather_u64.argtypes = [vp, vp, sz, vp, sz, C.POINTER(sz)]
+    L.pclb200_knn_sharded.argtypes = L.pclb200_knn.argtypes
+    L.pclb200_knn_stats_sharded.argtypes = L.pclb200_knn_stats.argtypes
+    L.pclb200_statistical_outlier_sharded.argtypes = [vp, vp, vp, sz, sz, vp, sz, C.c_int, C.c_double, C.c_int, vp, dp]
+    L.pclb200_radius_outlier_sharded.argtypes = [vp, vp, vp, sz, sz, vp, sz, C.c_int, C.c_double, C.c_int, C.c_int, vp]
     L.pclb200_voxelgrid.argtypes = [vp, vp, sz, sz, vp, sz, C.c_int, fp, C.c_uint, vp, C.POINTER(sz)]
     L.pclb200_voxelgrid_tile.argtypes = [vp, vp, sz, sz, fp, fp, C.c_uint, vp, C.POINTER(sz)]
     L.pclb200_voxelgrid_normals.argtypes = [vp, vp, sz, sz, vp, sz, vp, sz, C.c_int, fp, C.c_uint, vp, vp, C.POINTER(sz)]
@@ -673,6 +678,51 @@ class Index:
         """Collective normals_radius over a map sharded across the communicator's ranks (see normals_knn_sharded)."""
         return self._normals_sharded(lib().pclb200_normals_radius_sharded, cloud, float(radius), viewpoint, indices,
                                      is_dense, out)
+
+    def knn_sharded(self, q, k, out_idx=None, out_d2=None):
+        """Collective knn over a map sharded across the communicator's ranks (this index = this rank's tile, built with
+        ids=...; q = this rank's own queries): (ids, d2, k_eff), bit for bit one index of the whole map's answer."""
+        b = _Buf(q)
+        if out_idx is None:
+            out_idx = np.empty((b.rows, max(k, 0)), dtype=np.int32)
+            out_d2 = np.empty((b.rows, max(k, 0)), dtype=np.float32)
+        oi, od = _Buf(out_idx, np.int32), _Buf(out_d2)
+        keff = C.c_int()
+        _check(lib().pclb200_knn_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, k, oi.ptr, od.ptr, C.byref(keff)))
+        return out_idx, out_d2, int(keff.value)
+
+    def knn_stats_sharded(self, cloud, k, indices=None):
+        """Collective knn_stats over a sharded map (see knn_sharded): bit for bit one index of the whole map's answer."""
+        b, ib = _Buf(cloud), _Buf(indices, np.int32)
+        n = ib.rows if indices is not None else b.rows
+        mean, kth = np.empty(n, np.float32), np.empty(n, np.float32)
+        _check(lib().pclb200_knn_stats_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, ib.ptr, ib.rows, k,
+                                               C.c_void_p(mean.ctypes.data), C.c_void_p(kth.ctypes.data)))
+        return mean, kth
+
+    def statistical_outlier_removal_sharded(self, cloud, mean_k, std_mul, negative=False, indices=None):
+        """Collective StatisticalOutlierRemoval over a sharded map, its statistics taken over every rank's queries:
+        (keep mask of this rank's queries as uint8, dict(valid, mean, thr) the same on every rank)."""
+        b, ib = _Buf(cloud), _Buf(indices, np.int32)
+        n = ib.rows if indices is not None else b.rows
+        keep = np.empty(n, np.uint8)
+        stats = np.zeros(3)
+        _check(lib().pclb200_statistical_outlier_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, ib.ptr, ib.rows,
+                                                         int(mean_k), float(std_mul), int(negative),
+                                                         C.c_void_p(keep.ctypes.data),
+                                                         stats.ctypes.data_as(C.POINTER(C.c_double))))
+        return keep, dict(valid=int(stats[0]), mean=float(stats[1]), thr=float(stats[2]))
+
+    def radius_outlier_removal_sharded(self, cloud, radius, min_pts, negative=False, is_dense=True, indices=None):
+        """Collective RadiusOutlierRemoval over a sharded map: the keep mask of this rank's queries as uint8 (the dense
+        rule only when every rank passes is_dense)."""
+        b, ib = _Buf(cloud), _Buf(indices, np.int32)
+        n = ib.rows if indices is not None else b.rows
+        keep = np.empty(n, np.uint8)
+        _check(lib().pclb200_radius_outlier_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, ib.ptr, ib.rows,
+                                                    int(is_dense), float(radius), int(min_pts), int(negative),
+                                                    C.c_void_p(keep.ctypes.data)))
+        return keep
 
 
 def clusters_from_labels(labels, min_size=1, max_size=2 ** 32 - 1):

@@ -36,6 +36,16 @@ double fitness_score_sharded(Ctx& c, const Index& tile, const void* src, size_t 
                              size_t n_idx, const double* T, int scalar_is_double, double max_range);
 void gicp_covariances(Ctx& c, Index& idx, const void* pts, size_t n, size_t stride, int k, double gicp_epsilon,
                       double* out);
+// shard_filter.cu
+int knn_sharded(Ctx& c, const Index& tile, const void* queries, size_t nq, size_t stride, int k, int32_t* d_idx,
+                float* d_d2);
+void knn_stats_sharded(Ctx& c, const Index& tile, const void* pts, size_t n, size_t stride, const int32_t* indices,
+                       size_t n_idx, int k, float* d_mean, float* d_kth);
+void statistical_outlier_sharded(Ctx& c, const Index& tile, const void* pts, size_t n, size_t stride,
+                                 const int32_t* indices, size_t n_idx, int mean_k, double std_mul, int negative,
+                                 unsigned char* d_keep, double* d_stats);
+void radius_outlier_sharded(Ctx& c, const Index& tile, const void* pts, size_t n, size_t stride, const int32_t* indices,
+                            size_t n_idx, int is_dense, double radius, int min_pts, int negative, unsigned char* d_keep);
 // voxel.cu
 size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* indices, size_t n_idx, int is_dense,
                  const float leaf[3], unsigned min_pts, float* out_xyz1, const void* normals, size_t stride_n,
@@ -836,6 +846,77 @@ int pclb200_normals_radius_sharded(pclb200_ctx* ctx, const pclb200_index* idx_ti
                     [&](Index& local, const float4* d_q, size_t nq, float4* d_out, int* d_flag) {
                       launch_normals_radius(c, local, d_q, nq, r2, viewpoint, d_out, d_flag);
                     });
+  });
+}
+
+// ---- k-NN and the outlier filters on a sharded map ---------------------------------------------------------------------------
+int pclb200_knn_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* queries, size_t nq, size_t stride,
+                        int k, int32_t* out_idx, float* out_d2, int* k_eff)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && (!nq || (queries && out_idx && out_d2)), PCLB200_ERR_INVALID,
+                 "NULL argument");
+    const size_t n_out = nq * (size_t)std::max(k, 0);
+    DevBuf<int32_t> ti;
+    DevBuf<float> td;
+    const int keff = knn_sharded(c, *idx_tile->idx, queries, nq, stride, k, out_on_device(c, out_idx, n_out, ti),
+                                 out_on_device(c, out_d2, n_out, td));
+    copy_out(c, out_idx, ti, n_out);
+    copy_out(c, out_d2, td, n_out);
+    check_device_error(c);
+    if (k_eff)
+      *k_eff = keff;
+  });
+}
+
+int pclb200_knn_stats_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n, size_t stride,
+                              const int32_t* indices, size_t n_idx, int k, float* out_mean, float* out_kth)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && (out_mean || out_kth), PCLB200_ERR_INVALID, "NULL argument");
+    const size_t nq = indices ? n_idx : n;
+    DevBuf<float> tm, tk;
+    knn_stats_sharded(c, *idx_tile->idx, pts, n, stride, indices, n_idx, k, out_on_device(c, out_mean, nq, tm),
+                      out_on_device(c, out_kth, nq, tk));
+    copy_out(c, out_mean, tm, nq);
+    copy_out(c, out_kth, tk, nq);
+    check_device_error(c);
+  });
+}
+
+int pclb200_statistical_outlier_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n,
+                                        size_t stride, const int32_t* indices, size_t n_idx, int mean_k, double std_mul,
+                                        int negative, uint8_t* keep, double stats[3])
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const size_t nq = indices ? n_idx : n;
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && (keep || !nq), PCLB200_ERR_INVALID, "NULL argument");
+    DevBuf<unsigned char> tk;
+    DevBuf<double> d_stats;
+    d_stats.alloc(3, c.stream);
+    statistical_outlier_sharded(c, *idx_tile->idx, pts, n, stride, indices, n_idx, mean_k, std_mul, negative,
+                                out_on_device(c, keep, nq, tk), d_stats.p);
+    copy_out(c, keep, tk, nq);
+    double h[3];
+    PCLB_CUDA(cudaMemcpyAsync(h, d_stats.p, sizeof(h), cudaMemcpyDeviceToHost, c.stream));
+    check_device_error(c);
+    if (stats)
+      std::copy(h, h + 3, stats);
+  });
+}
+
+int pclb200_radius_outlier_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n,
+                                   size_t stride, const int32_t* indices, size_t n_idx, int is_dense, double radius,
+                                   int min_pts, int negative, uint8_t* keep)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const size_t nq = indices ? n_idx : n;
+    PCLB_REQUIRE(idx_tile && idx_tile->idx && (keep || !nq), PCLB200_ERR_INVALID, "NULL argument");
+    DevBuf<unsigned char> tk;
+    radius_outlier_sharded(c, *idx_tile->idx, pts, n, stride, indices, n_idx, is_dense, radius, min_pts, negative,
+                           out_on_device(c, keep, nq, tk));
+    copy_out(c, keep, tk, nq);
+    check_device_error(c);
   });
 }
 

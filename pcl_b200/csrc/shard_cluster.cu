@@ -37,9 +37,9 @@ namespace pclb200 {
 int comm_nranks(const Ctx& c);
 int comm_rank(const Ctx& c);
 
-// sorted unique copy of keys[0..n) (u32 or u64) into out; returns how many
+// sorted unique copy of keys[0..n) (u32 or u64) into out; returns how many (shard_filter.cu counts a map's ids with it)
 template <typename K>
-static size_t sort_unique(Ctx& c, const K* keys, size_t n, DevBuf<K>& out)
+size_t sort_unique(Ctx& c, const K* keys, size_t n, DevBuf<K>& out)
 {
   cudaStream_t st = c.stream;
   out.alloc(n, st);
@@ -62,6 +62,7 @@ static size_t sort_unique(Ctx& c, const K* keys, size_t n, DevBuf<K>& out)
   PCLB_CUDA(cudaStreamSynchronize(st));
   return (size_t)m;
 }
+template size_t sort_unique<unsigned long long>(Ctx&, const unsigned long long*, size_t, DevBuf<unsigned long long>&);
 
 void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t* d_labels, int64_t* d_sizes)
 {
