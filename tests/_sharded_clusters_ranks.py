@@ -1,7 +1,7 @@
 """Helper for tests/test_gpu_sharded_clusters.py (launched under torchrun, gloo): Euclidean clusters of a map sharded
 across ranks (pclb200_cluster_labels_sharded).
 
-Ranks on cuda:0 with the peer exchange bootstrapped over gloo (comm_export / _import), or, with SHARDED_CLUSTERS_NCCL=1,
+Ranks on cuda:0 with the peer exchange bootstrapped over gloo (comm_export / _import), or, with PCLB_SHARDED_NCCL=1,
 one GPU per rank with pclb200_comm_init and PCLB200_REDUCE_NCCL.  Scenes: a zig-zag chain crossing every slab boundary
 many times, blobs straddling the boundaries with duplicated points and non-finite records, a lattice at exactly the
 tolerance and just above it, tolerance 0, and a 1 M-point sheet with holes.  Partitions: slabs, random, and "special"
@@ -10,33 +10,14 @@ byte-equal to one process's cluster_labels on the whole map at the tile's ids, i
 equal to a bincount of those labels; euclidean_clusters_sharded's parts, gathered over the ranks, equal
 clusters_from_labels of the reference.  Last, the refusals (ERR_INVALID on every rank), after which the communicator
 still works."""
-import os
-import sys
-
 import numpy as np
 import torch
-import torch.distributed as dist
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import pcl_b200 as P  # noqa: E402
+import _sharded as S
+import pcl_b200 as P
 
-NCCL = os.environ.get("SHARDED_CLUSTERS_NCCL") == "1"
-rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-dev = rank if NCCL else 0
-torch.cuda.set_device(dev)
-dist.init_process_group("gloo")
-ctx = P.Context(dev)
-if NCCL:
-    uid = [P.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(uid, src=0)
-    ctx.comm_init(rank, world, uid[0])
-    ctx.comm_set_mode(P.REDUCE_NCCL)
-else:
-    handles = [None] * world
-    dist.all_gather_object(handles, ctx.comm_export())
-    ctx.comm_import(rank, world, handles)
-ref_ctx = P.Context(dev)  # no communicator: one process on the whole map
+me = S.join()
+rank, world, dev, ctx, ref_ctx = me.rank, me.world, me.device, me.ctx, me.ref
 
 rng = np.random.default_rng(29)
 
@@ -91,12 +72,6 @@ def partitions(whole):
     yield "special", special
 
 
-def gathered(obj):
-    out = [None] * world
-    dist.all_gather_object(out, obj)
-    return out
-
-
 checked = 0
 for sname, whole, tols in SCENES:
     ref_index = P.Index(ref_ctx, whole)
@@ -119,14 +94,14 @@ for sname, whole, tols in SCENES:
             assert dl.cpu().numpy().tobytes() == labels.tobytes() and np.array_equal(ds.cpu().numpy(), sizes)
             # an id held by two ranks: one label everywhere
             seen = {}
-            for r_ids, r_lab in gathered((ids, labels)):
+            for r_ids, r_lab in S.gathered((ids, labels)):
                 for i, l in zip(r_ids.tolist(), r_lab.tolist()):
                     assert seen.setdefault(i, l) == l, (sname, pname, tol, "shared id", i)
             checked += 1
         tol = tols[0]
         for lo, hi in ((1, 2 ** 32 - 1), (3, 500)):
             parts_here = tindex.euclidean_clusters_sharded(tol, ids, lo, hi)
-            every = gathered(parts_here)
+            every = S.gathered(parts_here)
             assert len(set(len(e) for e in every)) == 1, (sname, pname, "lengths")
             union = [np.unique(np.concatenate([e[k] for e in every])).astype(np.int32) for k in range(len(every[0]))]
             want_cl = P.clusters_from_labels(ref_index.cluster_labels(tol), lo, hi)
@@ -137,15 +112,6 @@ for sname, whole, tols in SCENES:
 
 
 # ---- refusals: ERR_INVALID on every rank, and the communicator still works -------------------------------------------------
-def refused(fn, word):
-    try:
-        fn()
-    except P.Pclb200Error as e:
-        assert e.code == P.ERR_INVALID and word in str(e), e
-        return
-    raise SystemExit(f"accepted: {word}")
-
-
 whole = SCENES[1][1]
 ids = np.ascontiguousarray(next(partitions(whole))[1][rank], dtype=np.int32)
 tile = np.ascontiguousarray(whole[ids])
@@ -153,16 +119,13 @@ tindex = P.Index(ctx, tile, ids=ids)
 plain = P.Index(ctx, tile)
 lone = P.Index(ref_ctx, tile, ids=ids)
 short = np.empty(len(ids) - 1, np.int32)
-refused(lambda: tindex.cluster_labels_sharded(-0.01), "negative cluster tolerance")
-refused(lambda: plain.cluster_labels_sharded(0.01), "pclb200_index_build_ids")
-refused(lambda: lone.cluster_labels_sharded(0.01), "communicator")
-refused(lambda: P._check(P.lib().pclb200_cluster_labels_sharded(ctx.h, tindex.h, 0.01, short.ctypes.data, None,
+S.refused(lambda: tindex.cluster_labels_sharded(-0.01), "negative cluster tolerance")
+S.refused(lambda: plain.cluster_labels_sharded(0.01), "pclb200_index_build_ids")
+S.refused(lambda: lone.cluster_labels_sharded(0.01), "communicator")
+S.refused(lambda: P._check(P.lib().pclb200_cluster_labels_sharded(ctx.h, tindex.h, 0.01, short.ctypes.data, None,
                                                                     len(short))), "one entry per record")
-refused(lambda: P._check(P.lib().pclb200_cluster_labels(ctx.h, tindex.h, 0.01, short.ctypes.data, len(ids))),
+S.refused(lambda: P._check(P.lib().pclb200_cluster_labels(ctx.h, tindex.h, 0.01, short.ctypes.data, len(ids))),
         "no cloud to size the labels by")  # the single-GPU call still refuses a tile
 want = P.Index(ref_ctx, whole).cluster_labels(0.01)
 assert tindex.cluster_labels_sharded(0.01)[0].tobytes() == np.ascontiguousarray(want[ids]).tobytes()
-dist.barrier()
-print(f"SHARDED_CLUSTERS_OK {'nccl' if NCCL else 'export'} {world} checks={checked}", flush=True)
-dist.barrier()
-dist.destroy_process_group()
+me.finish("SHARDED_CLUSTERS", checks=checked)

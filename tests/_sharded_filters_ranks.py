@@ -2,7 +2,7 @@
 outlier filters of a map sharded across ranks (pclb200_knn_sharded, pclb200_knn_stats_sharded,
 pclb200_statistical_outlier_sharded, pclb200_radius_outlier_sharded).
 
-Ranks on cuda:0 with the peer exchange bootstrapped over gloo (comm_export / _import), or, with SHARDED_FILTERS_NCCL=1, one
+Ranks on cuda:0 with the peer exchange bootstrapped over gloo (comm_export / _import), or, with PCLB_SHARDED_NCCL=1, one
 GPU per rank with pclb200_comm_init and PCLB200_REDUCE_NCCL.  Two maps (a surface and a volume cloud, both with an
 exact-tie lattice, non-finite rows and duplicated points under other ids), four partitions (spatial slabs; a random
 partition; slabs whose points near a cut are held by both neighbours under one id; slabs plus a far tile of 2 points).
@@ -12,47 +12,18 @@ whole map; the ROR masks byte-equal (dense and not, negative both ways); the SOR
 within 1e-12 relative of the sequential threshold over one process's means, no query within that band of it, and the
 SOR masks byte-equal; both masks equal the CPU oracle's.  Last, the refusals (ERR_INVALID on every rank), after which the
 communicator still works."""
-import os
-import sys
-
 import numpy as np
 import torch
-import torch.distributed as dist
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import oracle  # noqa: E402
-import pcl_b200 as P  # noqa: E402
+import _sharded as S
+import oracle
+import pcl_b200 as P
 
-NCCL = os.environ.get("SHARDED_FILTERS_NCCL") == "1"
-rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-dev = rank if NCCL else 0
-torch.cuda.set_device(dev)
-dist.init_process_group("gloo")
-ctx = P.Context(dev)
-if NCCL:
-    uid = [P.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(uid, src=0)
-    ctx.comm_init(rank, world, uid[0])
-    ctx.comm_set_mode(P.REDUCE_NCCL)
-else:
-    handles = [None] * world
-    dist.all_gather_object(handles, ctx.comm_export())
-    ctx.comm_import(rank, world, handles)
-ref_ctx = P.Context(dev)  # no communicator: one process on the whole map
+me = S.join()
+rank, world, dev, ctx, ref_ctx = me.rank, me.world, me.device, me.ctx, me.ref
 
 rng = np.random.default_rng(23)
 REL = 1e-12
-
-
-def surface(n):
-    xy = rng.random((n, 2), dtype=np.float32) * 4
-    z = (0.3 * np.sin(xy[:, 0]) * np.cos(xy[:, 1])).astype(np.float32)
-    return np.c_[xy, z]
-
-
-def volume(n):
-    return rng.random((n, 3), dtype=np.float32) * np.float32(0.6)
 
 
 def lattice(origin, n, step):
@@ -60,74 +31,17 @@ def lattice(origin, n, step):
     return np.c_[g, np.zeros(len(g), np.float32)] + np.asarray(origin, np.float32)
 
 
-def with_extras(xyz):
-    """xyz1 rows, some non-finite, some points repeated under other ids (exact ties)"""
-    w = P.xyz1(np.concatenate([xyz, xyz[rng.choice(len(xyz), 200, replace=False)]]))
-    w[rng.choice(len(w), 30, replace=False), 1] = np.nan
-    return w
-
-
-SCENES = [("surface", with_extras(np.concatenate([surface(150000), lattice((0.5, 0.5, 1.0), 64, 1 / 32)]))),
-          ("volume", with_extras(np.concatenate([volume(80000), lattice((0.0, 0.0, 0.3), 32, 1 / 64)])))]
-
-
-def partitions(whole):
-    """Tiles as id arrays; every id of the map is held by some rank"""
-    ids = np.arange(len(whole))
-    x = np.nan_to_num(whole[:, 0], nan=0.0)
-    span = x.max() + 1e-6
-    slab = np.minimum((x / span * world).astype(int), world - 1)
-    yield "slabs", [ids[slab == r] for r in range(world)]
-    perm = rng.permutation(len(whole))
-    yield "random", [np.sort(perm[r::world]) for r in range(world)]
-    frac = x / span * world - slab
-    yield "shared ids", [np.r_[ids[slab == r], ids[(slab == r + 1) & (frac < 0.1)]] for r in range(world)]
-    far = [ids[slab == r] for r in range(world)]
-    far[-2] = np.r_[far[-2], far[-1]]
-    far[-1] = np.array([], np.int64)
-    yield "far tile", far
-
-
-def ror_rule(kth, finite, is_dense, radius, negative):
-    """RadiusOutlierRemoval::applyFilterIndices (radius_outlier_removal.hpp:86-150) on the k-th squared distances"""
-    kth = kth.astype(np.float64)
-    if is_dense:
-        fin = np.isfinite(kth)
-        removed = np.where(fin, (radius * radius >= kth) if negative else (radius * radius < kth), not negative)
-    else:
-        enough = kth.astype(np.float32) < np.float32(radius * radius)
-        removed = ~finite | (enough if negative else ~enough)
-    return (~removed).astype(np.uint8)
-
-
-def sequential_sor(means, finite, std_mul):
-    """statistical_outlier_removal.hpp:100-112: sums in record order (np.cumsum is sequential), d * d in float"""
-    valid = float(finite.sum())
-    s = np.cumsum(means.astype(np.float64))[-1] if len(means) else 0.0
-    sq = np.cumsum((means * means).astype(np.float64))[-1] if len(means) else 0.0
-    mean = s / valid
-    var = (sq - s * s / valid) / (valid - 1)
-    return valid, mean, mean + std_mul * np.sqrt(var)
-
-
-def finite_rows(a):
-    return np.isfinite(a[:, :3]).all(1)
-
+SCENES = [("surface", S.with_extras(rng, np.concatenate([S.surface(rng, 150000), lattice((0.5, 0.5, 1.0), 64, 1 / 32)]))),
+          ("volume", S.with_extras(rng, np.concatenate([S.volume(rng, 80000), lattice((0.0, 0.0, 0.3), 32, 1 / 64)])))]
 
 checked = 0
 for sname, whole0 in SCENES:
     orc_index = None
-    for pname, parts in partitions(whole0):
-        whole = whole0
-        if pname == "far tile":  # two far points of their own, held by the last rank only
-            whole = np.concatenate([whole0, P.xyz1(np.array([[50, 50, 50], [50, 50.02, 50]], np.float32))])
-            parts[-1] = np.array([len(whole0), len(whole0) + 1])
+    for pname, parts, whole in S.partitions(rng, whole0, world):
         ref_index = P.Index(ref_ctx, whole)
         tile = np.ascontiguousarray(whole[parts[rank]])
         tindex = P.Index(ctx, tile, ids=np.ascontiguousarray(parts[rank], dtype=np.int32))
-        q_any = P.xyz1(np.concatenate([whole[rng.choice(len(whole), 3000), :3] + np.float32(0.004),
-                                       np.array([[np.nan, 0, 0], [100, 100, 100]], np.float32)]))
-        sub = np.sort(rng.choice(len(q_any), 1500, replace=False)).astype(np.int32)
+        q_any, sub = S.arbitrary_queries(rng, whole)
         for k in (2, 16, 51):
             for q in (tile, q_any[sub]):
                 got, want = tindex.knn_sharded(q, k), ref_index.knn(q, k)
@@ -147,43 +61,39 @@ for sname, whole0 in SCENES:
                 for is_dense in (True, False):
                     for negative in (False, True):
                         got = tindex.radius_outlier_removal_sharded(q, radius, min_pts, negative, is_dense, indices=ind)
-                        want = ror_rule(kth, finite_rows(rows), is_dense, radius, negative)
+                        want = S.ror_rule(kth, S.finite_rows(rows), is_dense, radius, negative)
                         assert got.tobytes() == want.tobytes(), (sname, pname, "ror", min_pts, is_dense, negative, rank)
                         checked += 1
         # one rank not dense: the radius rule on every rank
         got = tindex.radius_outlier_removal_sharded(tile, 0.02, 3, False, is_dense=rank != world - 1)
         _, kth = ref_index.knn_stats(tile, 4)
-        assert got.tobytes() == ror_rule(kth, finite_rows(tile), False, 0.02, False).tobytes(), (sname, pname, "ror mixed")
+        assert got.tobytes() == S.ror_rule(kth, S.finite_rows(tile), False, 0.02).tobytes(), (sname, pname, "ror mixed")
         # StatisticalOutlierRemoval over the concatenation of every rank's queries in rank order
         every = np.concatenate(parts).astype(np.int32)
         at = int(sum(len(p) for p in parts[:rank]))
         for mean_k, std_mul in ((8, 1.0), (50, 0.5)):
             means, _ = ref_index.knn_stats(whole, mean_k + 1, indices=every)
-            valid, mean, thr = sequential_sor(means, finite_rows(whole[every]), std_mul)
-            band = REL * abs(thr)
-            assert not (np.abs(means.astype(np.float64) - thr) <= band).any(), (sname, pname, "a mean in the band")
             for negative in (False, True):
+                want, (valid, mean, thr) = S.sor_rule(means, S.finite_rows(whole[every]), std_mul, negative)
+                band = REL * abs(thr)
+                assert not (np.abs(means.astype(np.float64) - thr) <= band).any(), (sname, pname, "a mean in the band")
                 keep, st = tindex.statistical_outlier_removal_sharded(tile, mean_k, std_mul, negative)
                 assert st["valid"] == valid and abs(st["thr"] - thr) <= band and abs(st["mean"] - mean) <= REL * abs(mean), \
                     (sname, pname, "sor stats", st, (valid, mean, thr))
-                every_thr = [None] * world
-                dist.all_gather_object(every_thr, st["thr"])
+                every_thr = S.gathered(st["thr"])
                 assert len(set(every_thr)) == 1, (sname, pname, "thr differs between ranks", every_thr)
-                m = means[at:at + len(parts[rank])].astype(np.float64)
-                want = (~((m <= thr) if negative else (m > thr))).astype(np.uint8)
-                assert keep.tobytes() == want.tobytes(), (sname, pname, "sor", mean_k, negative, rank)
+                assert keep.tobytes() == want[at:at + len(parts[rank])].tobytes(), (sname, pname, "sor", mean_k, negative, rank)
                 checked += 1
         # an indices subset of arbitrary queries: each rank its own slice
         mine = sub[rank::world]
         keep, st = tindex.statistical_outlier_removal_sharded(q_any, 8, 1.0, False, indices=mine)
         allq = np.concatenate([sub[r::world] for r in range(world)])
         means, _ = ref_index.knn_stats(q_any, 9, indices=allq)
-        valid, mean, thr = sequential_sor(means, finite_rows(q_any[allq]), 1.0)
+        want, (valid, mean, thr) = S.sor_rule(means, S.finite_rows(q_any[allq]), 1.0)
         assert st["valid"] == valid and abs(st["thr"] - thr) <= REL * abs(thr), (sname, pname, "sor subset", st, thr)
         off = int(sum(len(sub[r::world]) for r in range(rank)))
-        m = means[off:off + len(mine)].astype(np.float64)
         assert not (np.abs(means.astype(np.float64) - thr) <= REL * abs(thr)).any()
-        assert keep.tobytes() == (m <= thr).astype(np.uint8).tobytes(), (sname, pname, "sor subset", rank)
+        assert keep.tobytes() == want[off:off + len(mine)].tobytes(), (sname, pname, "sor subset", rank)
         checked += 1
         # the CPU oracle (PCL's own arithmetic): the slab partition of each scene, the tile's records as queries
         if pname == "slabs":
@@ -215,7 +125,7 @@ checked += 1
 
 # ---- device arrays in and out --------------------------------------------------------------------------------------------
 whole = SCENES[0][1]
-parts = next(partitions(whole))[1]
+parts = next(S.partitions(rng, whole, world))[1]
 tile = np.ascontiguousarray(whole[parts[rank]])
 tindex = P.Index(ctx, tile, ids=np.ascontiguousarray(parts[rank], dtype=np.int32))
 ref_index = P.Index(ref_ctx, whole)
@@ -229,33 +139,21 @@ checked += 1
 
 
 # ---- refusals: ERR_INVALID on every rank, and the communicator still works -------------------------------------------------
-def refused(fn, word):
-    try:
-        fn()
-    except P.Pclb200Error as e:
-        assert e.code == P.ERR_INVALID and word in str(e), e
-        return
-    raise SystemExit(f"accepted: {word}")
-
-
 plain = P.Index(ctx, tile)
 lone = P.Index(ref_ctx, tile, ids=np.ascontiguousarray(parts[rank], dtype=np.int32))
-refused(lambda: tindex.knn_sharded(tile, 0), "k must be positive")
-refused(lambda: tindex.knn_stats_sharded(tile, 0), "k must be positive")
-refused(lambda: tindex.statistical_outlier_removal_sharded(tile, 0, 1.0), "mean_k must be positive")
-refused(lambda: tindex.radius_outlier_removal_sharded(tile, 0.0, 3), "radius must be positive")
-refused(lambda: tindex.radius_outlier_removal_sharded(tile, 0.02, -1), "min_pts must not be negative")
-refused(lambda: plain.knn_sharded(tile, 8), "pclb200_index_build_ids")
-refused(lambda: plain.knn_stats_sharded(tile, 8), "pclb200_index_build_ids")
-refused(lambda: plain.statistical_outlier_removal_sharded(tile, 8, 1.0), "pclb200_index_build_ids")
-refused(lambda: plain.radius_outlier_removal_sharded(tile, 0.02, 3), "pclb200_index_build_ids")
-refused(lambda: lone.knn_sharded(tile, 8), "communicator")
-refused(lambda: lone.knn_stats_sharded(tile, 8), "communicator")
-refused(lambda: lone.statistical_outlier_removal_sharded(tile, 8, 1.0), "communicator")
-refused(lambda: lone.radius_outlier_removal_sharded(tile, 0.02, 3), "communicator")
+S.refused(lambda: tindex.knn_sharded(tile, 0), "k must be positive")
+S.refused(lambda: tindex.knn_stats_sharded(tile, 0), "k must be positive")
+S.refused(lambda: tindex.statistical_outlier_removal_sharded(tile, 0, 1.0), "mean_k must be positive")
+S.refused(lambda: tindex.radius_outlier_removal_sharded(tile, 0.0, 3), "radius must be positive")
+S.refused(lambda: tindex.radius_outlier_removal_sharded(tile, 0.02, -1), "min_pts must not be negative")
+S.refused(lambda: plain.knn_sharded(tile, 8), "pclb200_index_build_ids")
+S.refused(lambda: plain.knn_stats_sharded(tile, 8), "pclb200_index_build_ids")
+S.refused(lambda: plain.statistical_outlier_removal_sharded(tile, 8, 1.0), "pclb200_index_build_ids")
+S.refused(lambda: plain.radius_outlier_removal_sharded(tile, 0.02, 3), "pclb200_index_build_ids")
+S.refused(lambda: lone.knn_sharded(tile, 8), "communicator")
+S.refused(lambda: lone.knn_stats_sharded(tile, 8), "communicator")
+S.refused(lambda: lone.statistical_outlier_removal_sharded(tile, 8, 1.0), "communicator")
+S.refused(lambda: lone.radius_outlier_removal_sharded(tile, 0.02, 3), "communicator")
 got = tindex.knn_sharded(tile, 16)
 assert got[0].tobytes() == want[0].tobytes() and got[1].tobytes() == want[1].tobytes()
-dist.barrier()
-print(f"SHARDED_FILTERS_OK {'nccl' if NCCL else 'export'} {world} checks={checked}", flush=True)
-dist.barrier()
-dist.destroy_process_group()
+me.finish("SHARDED_FILTERS", checks=checked)

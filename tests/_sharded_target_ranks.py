@@ -1,39 +1,19 @@
 """Helper for tests/test_gpu_sharded_target.py (launched under torchrun, gloo): a map sharded across ranks, the whole source
 on every rank (pclb200_index_build_ids + pclb200_icp_set_target_sharded).
 
-Ranks on cuda:0 with the peer exchange bootstrapped over gloo (comm_export / _import), or, with SHARDED_TARGET_NCCL=1, one
+Ranks on cuda:0 with the peer exchange bootstrapped over gloo (comm_export / _import), or, with PCLB_SHARDED_NCCL=1, one
 GPU per rank with pclb200_comm_init and PCLB200_REDUCE_NCCL.  The map is a 200 k-point surface cut three ways (spatial
 slabs; a random partition; slabs plus duplicated map points given to another rank under other ids and a far 1-point tile
 no source point reaches within the gate).  For every estimator, Scalar and tracking mode, stepping one iteration at a
 time and running whole, every iteration's correspondences, the final stats and the aligned cloud must be byte-equal to
 one process on the whole map, on every rank.  Fitness agrees to 1e-12; every refusal is ERR_INVALID on every rank."""
-import os
-import sys
-
 import numpy as np
-import torch
-import torch.distributed as dist
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import pcl_b200 as P  # noqa: E402
+import _sharded as S
+import pcl_b200 as P
 
-NCCL = os.environ.get("SHARDED_TARGET_NCCL") == "1"
-rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-dev = rank if NCCL else 0
-torch.cuda.set_device(dev)
-dist.init_process_group("gloo")
-ctx = P.Context(dev)
-if NCCL:
-    uid = [P.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(uid, src=0)
-    ctx.comm_init(rank, world, uid[0])
-    ctx.comm_set_mode(P.REDUCE_NCCL)
-else:
-    handles = [None] * world
-    dist.all_gather_object(handles, ctx.comm_export())
-    ctx.comm_import(rank, world, handles)
-ref_ctx = P.Context(dev)  # no communicator: one process on the whole map
+me = S.join()
+rank, world, ctx, ref_ctx = me.rank, me.world, me.ctx, me.ref
 
 # ---- the map: a smooth surface, analytic normals; ids = row numbers of `whole` -------------------------------------------
 rng = np.random.default_rng(11)
@@ -84,7 +64,7 @@ src[rng.choice(ns, 50, replace=False), 0] = np.nan                    # non-fini
 
 ESTIMATORS = [("svd", P.EST_SVD, 0), ("svd_correlation", P.EST_SVD, 1), ("point_to_plane", P.EST_POINT_TO_PLANE_LLS, 0),
               ("symmetric", P.EST_SYMMETRIC_POINT_TO_PLANE_LLS, 0)]
-if NCCL:
+if me.nccl:
     ESTIMATORS = ESTIMATORS[2:3]
 
 
@@ -150,23 +130,13 @@ for pname, parts in partitions():
     for max_range in (np.finfo(np.float64).max, 0.01):
         f = tindex.fitness_score_sharded(src, T, max_range=max_range)
         f1 = ref_index.fitness_score(src, T, max_range=max_range)
-        allf = [None] * world
-        dist.all_gather_object(allf, f)
+        allf = S.gathered(f)
         assert all(x == allf[0] for x in allf), (pname, allf)
         assert abs(f - f1) <= 1e-12 * abs(f1), (pname, f, f1)
     print(f"rank {rank}: {pname} ok ({checked} runs)", flush=True)
 
 
 # ---- refusals: ERR_INVALID on every rank ---------------------------------------------------------------------------------
-def refused(fn, word):
-    try:
-        fn()
-    except P.Pclb200Error as e:
-        assert e.code == P.ERR_INVALID and word in str(e), e
-        return
-    raise SystemExit(f"accepted: {word}")
-
-
 ids = np.ascontiguousarray(np.arange(rank, N, world), dtype=np.int32)
 tile = np.ascontiguousarray(whole[ids])
 tindex = P.Index(ctx, tile, ids=ids)
@@ -183,9 +153,9 @@ def with_source(icp, s=src):
     icp.iterate()
 
 
-refused(lambda: with_source(session(use_reciprocal=1)), "reciprocal")
-refused(lambda: with_source(session(correspondence_kind=P.CORR_NORMAL_SHOOTING)), "normal-shooting")
-refused(lambda: with_source(session(correspondence_kind=P.CORR_BACK_PROJECTION)), "back-projection")
+S.refused(lambda: with_source(session(use_reciprocal=1)), "reciprocal")
+S.refused(lambda: with_source(session(correspondence_kind=P.CORR_NORMAL_SHOOTING)), "normal-shooting")
+S.refused(lambda: with_source(session(correspondence_kind=P.CORR_BACK_PROJECTION)), "back-projection")
 
 
 def with_rejector():
@@ -194,15 +164,12 @@ def with_rejector():
     with_source(icp)
 
 
-refused(with_rejector, "rejector")
+S.refused(with_rejector, "rejector")
 short = np.ascontiguousarray(src[:ns - rank])  # rank 0 passes one point more than the others
-refused(lambda: with_source(session(), short), "same whole source")
+S.refused(lambda: with_source(session(), short), "same whole source")
 lone = P.Index(ref_ctx, tile, ids=ids)
-refused(lambda: P.Icp(ref_ctx).set_target_sharded(lone), "communicator")
-refused(lambda: lone.fitness_score_sharded(src, np.eye(4)), "communicator")
+S.refused(lambda: P.Icp(ref_ctx).set_target_sharded(lone), "communicator")
+S.refused(lambda: lone.fitness_score_sharded(src, np.eye(4)), "communicator")
 # the session still works after the refusals
 with_source(session())
-dist.barrier()
-print(f"SHARDED_TARGET_OK {'nccl' if NCCL else 'export'} {world} runs={checked}", flush=True)
-dist.barrier()
-dist.destroy_process_group()
+me.finish("SHARDED_TARGET", runs=checked)

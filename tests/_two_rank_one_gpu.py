@@ -5,24 +5,14 @@ the caller bootstraps with pclb200_comm_export / _import over gloo).  Each rank 
 one half of the source; every iteration's 40 accumulators cross between the two processes through the peer-mapped
 exchange block inside the iteration kernel (comm.cu + peer_exchange.cuh).  The sharded result must equal the
 single-process result on the whole cloud: same correspondence counts, same iterations, transform within 1e-6."""
-import os
-import sys
-
 import numpy as np
-import torch
 import torch.distributed as dist
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import pcl_b200 as P  # noqa: E402
+import _sharded as S
+import pcl_b200 as P
 
-rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-torch.cuda.set_device(0)
-dist.init_process_group("gloo")
-ctx = P.Context(0)
-handles = [None] * world
-dist.all_gather_object(handles, ctx.comm_export())
-ctx.comm_import(rank, world, handles)
+me = S.join()
+rank, world, ctx = me.rank, me.world, me.ctx
 
 rng = np.random.default_rng(5)
 n = 120000
@@ -45,8 +35,7 @@ for name, est in (("svd", P.EST_SVD), ("lls", P.EST_POINT_TO_PLANE_LLS)):
     r = P.icp_align(ctx, shard, idx, tgt_normals=nrm if est != P.EST_SVD else None,
                     src_normals=P.Field(shard, 4) if est != P.EST_SVD else None, **kw)
     results[name] = r
-    got = [None] * world
-    dist.all_gather_object(got, r["final"].tobytes())
+    got = S.gathered(r["final"].tobytes())
     assert all(g == got[0] for g in got), "ranks disagree on the transform (the fused fold is rank-ordered: must be bitwise equal)"
     # reciprocal correspondences need the whole source on every rank: refused, not silently different
     try:
@@ -56,7 +45,7 @@ for name, est in (("svd", P.EST_SVD), ("lls", P.EST_POINT_TO_PLANE_LLS)):
         assert "reciprocal" in str(e), e
 dist.barrier()
 if rank == 0:
-    ctx1 = P.Context(0)  # no communicator: the whole cloud in one process
+    ctx1 = me.ref  # no communicator: the whole cloud in one process
     idx1 = P.Index(ctx1, tgt)
     for name, est in (("svd", P.EST_SVD), ("lls", P.EST_POINT_TO_PLANE_LLS)):
         kw = dict(max_iterations=12, max_correspondence_distance=0.2, estimator=est, mse_threshold_absolute=0.0,

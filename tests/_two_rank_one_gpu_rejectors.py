@@ -2,23 +2,18 @@
 sharded source.
 
 Every process holds a replica of the target index and one uneven contiguous range of the source (rank r holds the r-th
-range, so global position = input order).  Bootstrap: `export` = two or three processes on cuda:0, the peer exchange made
-with pclb200_comm_export / _import over gloo; `nccl` = one process per GPU, pclb200_comm_init + PCLB200_REDUCE_NCCL.
+range, so global position = input order).  Bootstrap: two or three processes on cuda:0, the peer exchange made with
+pclb200_comm_export / _import over gloo; with PCLB_SHARDED_NCCL=1, one process per GPU, pclb200_comm_init +
+PCLB200_REDUCE_NCCL.
   * iteration 1, exact: the correspondences of every rank (query indices shifted by the shard offset), concatenated in
     rank order, equal the single-process list with the same chain, as arrays — on a smooth surface with outliers and on
     a lattice scene full of exact distance ties across shard boundaries (median, trimmed and one-to-one tie rules);
   * full align: every rank ends with the bitwise same transform; against the single process the same iterations,
     n_correspondences and total_correspondences, transforms within 1e-6 (the fp64 sums fold in another order)."""
-import os
-import sys
-
 import numpy as np
-import torch
-import torch.distributed as dist
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import pcl_b200 as P  # noqa: E402
+import _sharded as S
+import pcl_b200 as P
 
 CHAIN4 = [(P.REJ_MEDIAN, 3.0, 0), (P.REJ_ONE_TO_ONE, 0.0, 0), (P.REJ_TRIMMED, 0.9, 100), (P.REJ_DISTANCE, 0.2, 0)]
 SVD, LLS = P.EST_SVD, P.EST_POINT_TO_PLANE_LLS
@@ -88,8 +83,8 @@ def run_case(ctx, idx, tgt, src, lo, hi, chain, est, max_iterations):
     return st, corr
 
 
-def main(ctx, rank, world, tag):
-    single = P.Context(0 if tag == "export" else int(os.environ["LOCAL_RANK"]))  # no communicator: the whole cloud
+def main(me):
+    ctx, rank, world, single = me.ctx, me.rank, me.world, me.ref  # single: no communicator, the whole cloud
     for name, tgt, src, full in scenes(ctx):
         idx = P.Index(ctx, tgt)
         idx1 = P.Index(single, tgt) if rank == 0 else None
@@ -97,8 +92,7 @@ def main(ctx, rank, world, tag):
         for case, chain, est in CASES:
             # iteration 1: bit-identical inputs, so the lists must be equal
             st, corr = run_case(ctx, idx, tgt, src, lo, hi, chain, est, 1)
-            got = [None] * world
-            dist.all_gather_object(got, corr.tobytes())
+            got = S.gathered(corr.tobytes())
             if rank == 0:
                 st1, corr1 = run_case(single, idx1, tgt, src, 0, src.shape[0], chain, est, 1)
                 cat = np.frombuffer(b"".join(got), dtype=P.CORR_DTYPE)
@@ -108,8 +102,7 @@ def main(ctx, rank, world, tag):
             if not full:
                 continue
             st, _ = run_case(ctx, idx, tgt, src, lo, hi, chain, est, 30)
-            got = [None] * world
-            dist.all_gather_object(got, st["final"].tobytes())
+            got = S.gathered(st["final"].tobytes())
             assert all(g == got[0] for g in got), (name, case, "ranks disagree on the transform")
             if rank == 0:
                 st1, _ = run_case(single, idx1, tgt, src, 0, src.shape[0], chain, est, 30)
@@ -126,26 +119,6 @@ def main(ctx, rank, world, tag):
 
 
 if __name__ == "__main__":
-    tag = sys.argv[1] if len(sys.argv) > 1 else "export"
-    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-    if tag == "export":
-        torch.cuda.set_device(0)
-        dist.init_process_group("gloo")
-        ctx = P.Context(0)
-        handles = [None] * world
-        dist.all_gather_object(handles, ctx.comm_export())
-        ctx.comm_import(rank, world, handles)
-    else:
-        local = int(os.environ["LOCAL_RANK"])
-        torch.cuda.set_device(local)
-        dist.init_process_group("gloo")
-        ctx = P.Context(local)
-        uid = [P.comm_unique_id() if rank == 0 else None]
-        dist.broadcast_object_list(uid, src=0)
-        ctx.comm_init(rank, world, uid[0])
-        ctx.comm_set_mode(P.REDUCE_NCCL)
-    main(ctx, rank, world, tag)
-    dist.barrier()
-    if rank == 0:
-        print(f"SHARDED_REJECTORS_OK {tag} {world}")
-    dist.destroy_process_group()
+    me = S.join()
+    main(me)
+    me.finish("SHARDED_REJECTORS")

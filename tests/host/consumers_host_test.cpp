@@ -6,8 +6,8 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 
 #include <cfloat>
 
@@ -38,15 +38,6 @@ size_t orc_reject_surface_normal(const pclb200_corr* in, size_t n, const float* 
 }
 
 // the fixed seed of the committed test, or PCLB_TEST_SEED for a fuzz run (tools/dev/fuzz_host_tests.sh)
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
 static float gate_from_max_dist(double max_dist)   // icp.cu: the largest float not above max_dist^2
 {
   const double m2 = max_dist * max_dist;

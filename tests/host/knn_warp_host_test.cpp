@@ -7,8 +7,8 @@
 // cells (the case that hid a pruning bug on the device until every one of 10 M rows was compared).
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 
 #include "../../pcl_b200/csrc/knn_warp.cuh"
 
@@ -16,15 +16,6 @@
 #include <pcl/point_types.h>
 
 // the fixed seed of the committed test, or PCLB_TEST_SEED for a fuzz run (tools/dev/fuzz_host_tests.sh)
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
 static void brute_knn(const std::vector<float>& xyz, const float q[3], int k, std::vector<int>& idx, std::vector<float>& d2)
 {
   const int n = static_cast<int>(xyz.size() / 3);

@@ -11,22 +11,13 @@
 #define PCLB_HOST_EMULATION 1
 #define PCLB_TEST_DEVICE_BUILD 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 
 #include <map>
 #include <set>
 
 // the fixed seed of the committed test, or PCLB_TEST_SEED for a fuzz run (tools/dev/fuzz_host_tests.sh)
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
 struct Sub { std::vector<int> points; float lo[3], hi[3]; int first_leaf, n_leaves; };
 
 static Sub collect(const HostIndex& I, int ref, int& bad_boxes, int& bad_ranges)

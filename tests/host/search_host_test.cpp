@@ -6,8 +6,8 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 
 static inline unsigned __float_as_uint(float f) { unsigned u; std::memcpy(&u, &f, 4); return u; }
 
@@ -17,15 +17,6 @@ static inline unsigned __float_as_uint(float f) { unsigned u; std::memcpy(&u, &f
 #include <pcl/point_types.h>
 
 // the fixed seed of the committed test, or PCLB_TEST_SEED for a fuzz run (tools/dev/fuzz_host_tests.sh)
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
 static void brute_all(const std::vector<float>& xyz, const float q[3], std::vector<std::pair<float, int>>& all)
 {
   const int n = static_cast<int>(xyz.size() / 3);

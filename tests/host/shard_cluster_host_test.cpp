@@ -1,7 +1,7 @@
 // shard_cluster_host_test.cpp — Euclidean clustering over a sharded map (pcl_b200/csrc/shard_cluster_kernels.cuh, with the
 // halo kernels of shard_normals_kernels.cuh and the union-find of cluster_kernels.cuh) compiled for the HOST and run in
 // shard_cluster.cu's sequence for R = 1, 2, 3, 5, 8 simulated ranks in one process: this program does the cross-rank steps
-// comm.cu would do (the u64 minimum of the boxes, the tables of peer_tables_sim.h), and places the segments with the
+// comm.cu would do (the u64 minimum of the boxes, the tables of shard_sim.h), and places the segments with the
 // layout functions of peer_tables.cuh that the driver calls.  Every rank's labels and sizes are compared with a brute-force connected-components of the whole map (union of
 // the tiles' ids, d2 < r2 under the library's distance).
 // Scenes: a zig-zag chain crossing every slab boundary many times (a component's pieces on one rank joined only through
@@ -11,46 +11,17 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 #include <map>
 #include <set>
 
-template <typename T> static inline T __ldcv(const T* p) { return *p; }
-static inline unsigned long long atomicMin(unsigned long long* p, unsigned long long v) { const unsigned long long o = *p; if (v < o) *p = v; return o; }
-
+#include "shard_sim.h"
 #include "../../pcl_b200/csrc/shard_normals_kernels.cuh"
 #include "../../pcl_b200/csrc/cluster_kernels.cuh"
 #include "../../pcl_b200/csrc/shard_cluster_kernels.cuh"
-#include "peer_tables_sim.h"
 
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
-template <typename F> static void launch(unsigned grid, int block, F kernel)
-{
-  blockDim.x = block;
-  gridDim.x = grid ? grid : 1;
-  for (unsigned b = 0; b < gridDim.x; ++b) { blockIdx_storage.x = b; warp_emu::run_block(block, kernel); }
-  blockIdx_storage.x = 0;
-  gridDim.x = 1;
-}
 static unsigned blocks(size_t n) { return (unsigned)std::min<size_t>(3, (n + 63) / 64); }  // a grid-stride loop over n
-
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static float d2_of(const float4& q, const float4& p)
-{
-  const float dx = __fsub_rn(q.x, p.x), dy = __fsub_rn(q.y, p.y), dz = __fsub_rn(q.z, p.z);
-  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
-static bool finite3(const float4& p) { return std::isfinite(p.x) && std::isfinite(p.y) && std::isfinite(p.z); }
-static int id_of(const float4& p) { return __float_as_int(p.w); }
-static const float4 kPad = make_float4(INFINITY, INFINITY, INFINITY, __int_as_float(kSentinelIndex));
 
 // per simulated rank: what shard_cluster.cu keeps between the exchanges
 struct Rank {

@@ -1,6 +1,6 @@
 // shard_filter_host_test.cpp — the kernels of k-NN queries and outlier filters over a sharded map (pcl_b200/csrc/
 // shard_filter_kernels.cuh) compiled for the HOST and run in shard_filter.cu's sequence for R = 1, 2, 3, 5, 8 simulated
-// ranks in one process, under both exchange protocols (peer_tables_sim.h: every rank's table read directly, or the tables
+// ranks in one process, under both exchange protocols (shard_sim.h: every rank's table read directly, or the tables
 // end to end in one zeroed table summed over the ranks).  It checks
 //   - the id mapping: every record number of a k-NN row becomes the local map's id of that record, padding -1 stays;
 //     a tile's ids come out of its Morton array with the padding's sentinel;
@@ -12,33 +12,10 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
-
-template <typename T> static inline T __ldcv(const T* p) { return *p; }
-
+#include "shard_sim.h"
 #include "../../pcl_b200/csrc/shard_filter_kernels.cuh"
-#include "peer_tables_sim.h"
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
-template <typename F> static void launch(unsigned grid, int block, F kernel)
-{
-  blockDim.x = block;
-  gridDim.x = grid ? grid : 1;
-  for (unsigned b = 0; b < gridDim.x; ++b) { blockIdx_storage.x = b; warp_emu::run_block(block, kernel); }
-  blockIdx_storage.x = 0;
-  gridDim.x = 1;
-}
-
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static bool finite3(const float4& p) { return std::isfinite(p.x) && std::isfinite(p.y) && std::isfinite(p.z); }
 
 // the facade's StatisticalOutlierRemoval::classify arithmetic over one process's distances (outlier_removal.h)
 static void facade_sor(const std::vector<float>& d, long long valid, double std_mul, double out[3])

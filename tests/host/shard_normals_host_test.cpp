@@ -1,7 +1,7 @@
 // shard_normals_host_test.cpp — the halo kernels of normal estimation over a sharded map (pcl_b200/csrc/
 // shard_normals_kernels.cuh) compiled for the HOST and run in shard_normals.cu's sequence for R = 1, 2, 3, 5, 8 simulated
 // ranks in one process: this program does the cross-rank steps comm.cu would do (the u64 minimum of the boxes, the sum of
-// the counts, the tables of peer_tables_sim.h), and places the segments with the layout functions of peer_tables.cuh that
+// the counts, the tables of shard_sim.h), and places the segments with the layout functions of peer_tables.cuh that
 // the driver calls.  For every rank it checks
 //   - the box: the u64 fold of k_halo_box equals a reference fold of the outward-rounded boxes of its finite queries;
 //   - the halo: exactly the points of the other tiles inside that box (a brute-force selection), each once per sender,
@@ -14,44 +14,13 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 #include <map>
 #include <set>
 
-template <typename T> static inline T __ldcv(const T* p) { return *p; }
-static inline unsigned long long atomicMin(unsigned long long* p, unsigned long long v) { const unsigned long long o = *p; if (v < o) *p = v; return o; }
-
+#include "shard_sim.h"
 #include "../../pcl_b200/csrc/shard_normals_kernels.cuh"
-#include "../../pcl_b200/csrc/peer_tables.cuh"
-#include "peer_tables_sim.h"
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
-template <typename F> static void launch(unsigned grid, int block, F kernel)
-{
-  blockDim.x = block;
-  gridDim.x = grid ? grid : 1;
-  for (unsigned b = 0; b < gridDim.x; ++b) { blockIdx_storage.x = b; warp_emu::run_block(block, kernel); }
-  blockIdx_storage.x = 0;
-  gridDim.x = 1;
-}
-
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-// the library's squared distance: ((dx*dx) + dy*dy) + dz*dz, fp32, no fma
-static float d2_of(const float4& q, const float4& p)
-{
-  const float dx = __fsub_rn(q.x, p.x), dy = __fsub_rn(q.y, p.y), dz = __fsub_rn(q.z, p.z);
-  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
-static bool finite3(const float4& p) { return std::isfinite(p.x) && std::isfinite(p.y) && std::isfinite(p.z); }
-static int id_of(const float4& p) { return __float_as_int(p.w); }
 
 // k-th smallest d2 from q over pts (+inf when fewer than k): what launch_knn_stats returns on an index of pts
 static float kth_d2(const std::vector<float4>& pts, const float4& q, int k)
@@ -108,9 +77,9 @@ static void run_case(const char* name, const std::vector<std::vector<float4>>& t
     std::shuffle(t.begin(), t.end(), rng);
     for (size_t i = 0; i < t.size(); ++i) {
       idx_pts[r].push_back(t[i]);
-      if (i % 5 == 2) idx_pts[r].push_back(make_float4(INFINITY, INFINITY, INFINITY, __int_as_float(kSentinelIndex)));
+      if (i % 5 == 2) idx_pts[r].push_back(kPad);
     }
-    for (int j = 0; j < 3; ++j) idx_pts[r].push_back(make_float4(INFINITY, INFINITY, INFINITY, __int_as_float(kSentinelIndex)));
+    for (int j = 0; j < 3; ++j) idx_pts[r].push_back(kPad);
   }
   // bound + boxes
   std::vector<unsigned long long> boxes((size_t)kHaloBoxWords * R, kNoHaloBox);

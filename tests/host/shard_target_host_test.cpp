@@ -10,40 +10,15 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
-
-#include <cstdlib>
+#include "check.h"
 
 static inline unsigned __float_as_uint(float f) { unsigned u; std::memcpy(&u, &f, 4); return u; }
-template <typename T> static inline T __ldcv(const T* p) { return *p; }
 
+#include "shard_sim.h"
 #include "../../pcl_b200/csrc/shard_target_kernels.cuh"
 
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
-template <typename F> static void launch(unsigned grid, int block, F kernel)
-{
-  blockDim.x = block;
-  gridDim.x = grid ? grid : 1;
-  for (unsigned b = 0; b < gridDim.x; ++b) { blockIdx_storage.x = b; warp_emu::run_block(block, kernel); }
-  blockIdx_storage.x = 0;
-  gridDim.x = 1;
-}
 static unsigned blocks(size_t n) { return (unsigned)((n + 255) / 256); }
 
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-// the library's squared distance: ((dx*dx) + dy*dy) + dz*dz, fp32, no fma
-static float d2_of(const float4& q, const float4& p)
-{
-  const float dx = __fsub_rn(q.x, p.x), dy = __fsub_rn(q.y, p.y), dz = __fsub_rn(q.z, p.z);
-  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
-static bool finite3(const float4& p) { return std::isfinite(p.x) && std::isfinite(p.y) && std::isfinite(p.z); }
 static bool same_bits(const float4& a, const float4& b) { return std::memcmp(&a, &b, sizeof(float4)) == 0; }
 
 struct MapPoint { float4 p, n; };  // p.w = id bits
@@ -61,8 +36,6 @@ static Best argmin(const std::vector<MapPoint>& pts, const float4& q, float gate
   }
   return b;
 }
-
-enum { kPeer = 0, kNccl = 1 };
 
 static void run_case(const char* name, const std::vector<std::vector<MapPoint>>& tiles, const std::vector<float4>& q,
                      float gate, bool with_normals, int mode)

@@ -13,19 +13,10 @@
 // gate; TRACK's lower bound never exceeds the true second-nearest distance.  Scenes: uniform volume, a thin surface,
 // duplicates beyond a leaf, a lattice full of exact ties, a degenerate line, far-away queries, tiny clouds.
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 
 // the fixed seed of the committed test, or PCLB_TEST_SEED for a fuzz run (tools/dev/fuzz_host_tests.sh)
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
 static void run_scene(const char* name, const std::vector<float>& xyz, const std::vector<float>& queries, float gate, int bmax)
 {
   const bool quiet = std::strncmp(name, "small cloud", 11) == 0;

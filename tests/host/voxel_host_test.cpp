@@ -5,8 +5,8 @@
 #define PCLB_HOST_EXTRA_SHIMS "warp_emu.h"
 #define PCLB_HOST_EMULATION 1
 #include "host_index.h"
+#include "check.h"
 
-#include <cstdlib>
 
 #include <numeric>
 
@@ -19,15 +19,6 @@ extern "C" long long orc_voxelgrid_normals(const float* pts, size_t n, size_t st
                                            const float leaf[3], unsigned min_pts, float* out, long normal_off, float* out_nc);
 
 // the fixed seed of the committed test, or PCLB_TEST_SEED for a fuzz run (tools/dev/fuzz_host_tests.sh)
-static unsigned test_seed(unsigned fixed)
-{
-  const char* e = std::getenv("PCLB_TEST_SEED");
-  return e && *e ? fixed ^ (2654435761u * static_cast<unsigned>(std::strtoul(e, nullptr, 10))) : fixed;
-}
-
-static long g_checks = 0, g_fail = 0;
-#define CHECK(c, ...) do { ++g_checks; if (!(c)) { if (++g_fail <= 20) { std::printf("FAIL %s:%d %s  ", __FILE__, __LINE__, #c); std::printf(__VA_ARGS__); std::printf("\n"); } } } while (0)
-
 template <typename F> static void launch(std::size_t n, int block, F kernel)
 {
   const unsigned grid = static_cast<unsigned>((n + block - 1) / block);

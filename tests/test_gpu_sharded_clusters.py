@@ -1,31 +1,9 @@
 """Euclidean clusters of a map sharded across ranks (pclb200_cluster_labels_sharded) under torchrun
 (tests/_sharded_clusters_ranks.py): labels byte-equal to one process's cluster_labels on the whole map, sizes equal to its
 component sizes, and euclidean_clusters_sharded's parts equal to the whole map's clusters."""
-import os
-import socket
-import subprocess
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _torchrun(nproc, env=None):
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={nproc}",
-                        "--master-addr", "127.0.0.1", "--master-port", str(_free_port()),
-                        os.path.join(ROOT, "tests", "_sharded_clusters_ranks.py")],
-                       capture_output=True, text=True, timeout=1500, env=dict(os.environ, **(env or {})))
-    print(r.stdout[-4000:], r.stderr[-4000:])
-    return r
+import _sharded as S
 
 
 @pytest.mark.gpu
@@ -35,7 +13,7 @@ def test_sharded_clusters_share_one_gpu(nproc):
     duplicates and non-finite records, a lattice at and just above the tolerance, tolerance 0 and a 1 M-point holed sheet;
     slabs, a random partition and shared ids with a 1-point tile: labels and sizes into host and device buffers, one label
     per shared id, the cluster lists, and every refusal on every rank."""
-    r = _torchrun(nproc)
+    r = S.torchrun("_sharded_clusters_ranks.py", nproc)
     assert r.returncode == 0 and f"SHARDED_CLUSTERS_OK export {nproc}" in r.stdout
 
 
@@ -46,5 +24,5 @@ def test_sharded_clusters_two_gpus_nccl():
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs (VISIBLE SKIP: the peer-mapped path runs on one GPU in test_sharded_clusters_share_one_gpu)")
-    r = _torchrun(2, {"SHARDED_CLUSTERS_NCCL": "1"})
+    r = S.torchrun("_sharded_clusters_ranks.py", 2, nccl=True)
     assert r.returncode == 0 and "SHARDED_CLUSTERS_OK nccl 2" in r.stdout

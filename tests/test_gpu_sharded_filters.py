@@ -2,31 +2,9 @@
 pclb200_knn_stats_sharded, pclb200_statistical_outlier_sharded, pclb200_radius_outlier_sharded) under torchrun
 (tests/_sharded_filters_ranks.py): byte-equal to one process on an index of the whole map, the SOR threshold within fp64
 round-off of one process's sequential threshold and the same on every rank."""
-import os
-import socket
-import subprocess
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _torchrun(nproc, env=None):
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={nproc}",
-                        "--master-addr", "127.0.0.1", "--master-port", str(_free_port()),
-                        os.path.join(ROOT, "tests", "_sharded_filters_ranks.py")],
-                       capture_output=True, text=True, timeout=1500, env=dict(os.environ, **(env or {})))
-    print(r.stdout[-4000:], r.stderr[-4000:])
-    return r
+import _sharded as S
 
 
 @pytest.mark.gpu
@@ -37,7 +15,7 @@ def test_sharded_filters_share_one_gpu(nproc):
     indices subset: k-NN rows, k_eff, mean and kth byte-equal to one process on the whole map; ROR masks byte-equal (dense
     and not, negative both ways); the SOR threshold equal on every rank and within 1e-12 of the sequential one, its masks
     byte-equal; both masks equal the CPU oracle's; a map smaller than k; device arrays; every refusal on every rank."""
-    r = _torchrun(nproc)
+    r = S.torchrun("_sharded_filters_ranks.py", nproc)
     assert r.returncode == 0 and f"SHARDED_FILTERS_OK export {nproc}" in r.stdout
 
 
@@ -48,5 +26,5 @@ def test_sharded_filters_two_gpus_nccl():
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs (VISIBLE SKIP: the peer-mapped path runs on one GPU in test_sharded_filters_share_one_gpu)")
-    r = _torchrun(2, {"SHARDED_FILTERS_NCCL": "1"})
+    r = S.torchrun("_sharded_filters_ranks.py", 2, nccl=True)
     assert r.returncode == 0 and "SHARDED_FILTERS_OK nccl 2" in r.stdout

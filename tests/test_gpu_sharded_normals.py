@@ -1,31 +1,9 @@
 """Normals of a map sharded across ranks (pclb200_normals_knn_sharded / pclb200_normals_radius_sharded) under torchrun
 (tests/_sharded_normals_ranks.py): byte-equal to one process's normals on an index of the whole map, and, fed to
 set_target_sharded, point-to-plane and symmetric aligns byte-equal to one process that used the whole map's normals."""
-import os
-import socket
-import subprocess
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _torchrun(nproc, env=None):
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={nproc}",
-                        "--master-addr", "127.0.0.1", "--master-port", str(_free_port()),
-                        os.path.join(ROOT, "tests", "_sharded_normals_ranks.py")],
-                       capture_output=True, text=True, timeout=1500, env=dict(os.environ, **(env or {})))
-    print(r.stdout[-4000:], r.stderr[-4000:])
-    return r
+import _sharded as S
 
 
 @pytest.mark.gpu
@@ -35,7 +13,7 @@ def test_sharded_normals_share_one_gpu(nproc):
     partition, tiles sharing ids and a far tile of 2 points, k = 3 / 16 / 40 and a radius, the tiles' own records and an
     arbitrary query subset: out and is_dense byte-equal to one process on the whole map; the normals drive sharded
     point-to-plane and symmetric aligns byte-equal to one process; every refusal on every rank."""
-    r = _torchrun(nproc)
+    r = S.torchrun("_sharded_normals_ranks.py", nproc)
     assert r.returncode == 0 and f"SHARDED_NORMALS_OK export {nproc}" in r.stdout
 
 
@@ -46,5 +24,5 @@ def test_sharded_normals_two_gpus_nccl():
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs (VISIBLE SKIP: the peer-mapped path runs on one GPU in test_sharded_normals_share_one_gpu)")
-    r = _torchrun(2, {"SHARDED_NORMALS_NCCL": "1"})
+    r = S.torchrun("_sharded_normals_ranks.py", 2, nccl=True)
     assert r.returncode == 0 and "SHARDED_NORMALS_OK nccl 2" in r.stdout

@@ -1,33 +1,10 @@
 """A target map sharded across ranks: the labelled index (pclb200_index_build_ids) on one GPU, and the sharded-target ICP
 session and fitness (pclb200_icp_set_target_sharded, pclb200_fitness_score_sharded) under torchrun
 (tests/_sharded_target_ranks.py): byte-equal to one process on the whole map."""
-import os
-import socket
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _torchrun(nproc, env=None):
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={nproc}",
-                        "--master-addr", "127.0.0.1", "--master-port", str(_free_port()),
-                        os.path.join(ROOT, "tests", "_sharded_target_ranks.py")],
-                       capture_output=True, text=True, timeout=1500, env=dict(os.environ, **(env or {})))
-    print(r.stdout[-4000:], r.stderr[-4000:])
-    return r
+import _sharded as S
 
 
 @pytest.mark.gpu
@@ -77,7 +54,7 @@ def test_sharded_target_share_one_gpu(nproc):
     points and a far 1-point tile; SVD (Umeyama and correlation), point-to-plane and symmetric, float and double, tracking
     off / on / auto, stepping and whole: every iteration's correspondences, the final stats and the aligned cloud
     byte-equal to one process on the whole map; fitness to 1e-12; every refusal on every rank."""
-    r = _torchrun(nproc)
+    r = S.torchrun("_sharded_target_ranks.py", nproc)
     assert r.returncode == 0 and f"SHARDED_TARGET_OK export {nproc}" in r.stdout
 
 
@@ -88,5 +65,5 @@ def test_sharded_target_two_gpus_nccl():
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs (VISIBLE SKIP: the peer-mapped path runs on one GPU in test_sharded_target_share_one_gpu)")
-    r = _torchrun(2, {"SHARDED_TARGET_NCCL": "1"})
+    r = S.torchrun("_sharded_target_ranks.py", 2, nccl=True)
     assert r.returncode == 0 and "SHARDED_TARGET_OK nccl 2" in r.stdout

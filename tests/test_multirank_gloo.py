@@ -5,7 +5,6 @@ origin-shifted fp64 sums of ITS source shard, the 40 doubles are all-reduced (su
 identical 3x3 / 6x6 system.  These tests run that algebra over a real torch.distributed all_reduce and compare with
 the oracle's single-process estimator on the whole cloud, and exercise the unique-id broadcast plumbing bench.py uses."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -13,15 +12,7 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+import _sharded as S
 
 
 def _svd_accumulators(p, q, o):
@@ -55,8 +46,6 @@ def _solve_svd(a, o):
 def _worker(rank, world, port, q):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
-    import sys
-    sys.path.insert(0, ROOT)
     import bench
     # 1. unique-id plumbing: rank 0's 128 bytes reach every rank unchanged
     uid = [bytes(range(128)) if rank == 0 else None]
@@ -91,7 +80,7 @@ def _worker(rank, world, port, q):
 def test_sharded_accumulators_match_whole_cloud(orc):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = S.free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
@@ -109,13 +98,7 @@ def test_two_gpu_icp_matches_single_gpu():
     """Needs 2 GPUs: the sharded ICP (NCCL all-reduce per iteration) reaches the single-GPU transform."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs (VISIBLE SKIP: the same product path runs on one GPU in test_two_ranks_share_one_gpu)")
-    import subprocess
-    import sys
-    script = os.path.join(ROOT, "tests", "_two_gpu_icp.py")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", str(_free_port()), script],
-                       capture_output=True, text=True, timeout=600)
-    print(r.stdout[-2000:], r.stderr[-2000:])
+    r = S.torchrun("_two_gpu_icp.py", 2, timeout=600)
     assert r.returncode == 0 and "TWO_GPU_OK" in r.stdout
 
 
@@ -124,11 +107,5 @@ def test_two_ranks_share_one_gpu():
     """The N > 1 product path on ANY box with one GPU: two processes on cuda:0, the peer exchange bootstrapped over gloo
     (pclb200_comm_export / _import), 40 accumulators per iteration crossing between the processes inside the iteration
     kernel.  Sharded == whole-cloud result; reciprocal + communicator is refused (tests/_two_rank_one_gpu.py)."""
-    import subprocess
-    import sys
-    script = os.path.join(ROOT, "tests", "_two_rank_one_gpu.py")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", str(_free_port()), script],
-                       capture_output=True, text=True, timeout=600)
-    print(r.stdout[-3000:], r.stderr[-3000:])
+    r = S.torchrun("_two_rank_one_gpu.py", 2, timeout=600)
     assert r.returncode == 0 and "TWO_RANK_ONE_GPU_OK" in r.stdout

@@ -2,57 +2,31 @@
 shard_cluster_kernels.cuh, driven by shard_cluster.cu) compiled for the host, and the exactness argument restated on the
 CPU oracle: per-rank clusters of tile plus halo, joined by the edges of the points the halo shares, are the whole map's
 clusters."""
-import os
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-HOST = os.path.join(ROOT, "tests", "host")
+import _sharded as S
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
-                    reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
+@S.needs_host_compiler
 def test_sharded_cluster_kernels_and_layout_on_the_host(tmp_path):
     """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols, the halo, the answers and the edges placed and read with
     the layout functions of peer_tables.cuh that the driver calls: every rank's labels and sizes equal a brute-force
     connected-components of the whole map — a zig-zag chain crossing every slab boundary many times, blobs on the
     boundaries, a lattice at and just above the tolerance, duplicated points, non-finite records, ids near 2^31 - 2,
     tolerance 0; slabs, a random partition, overlapping tiles sharing ids and a 1-point tile."""
-    exe = str(tmp_path / "shard_cluster_host_test")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-frounding-math", "-ffp-contract=off", "-fno-fast-math",
-                           "-I" + CUDA_INC, "-I" + os.path.join(ROOT, "include"), "-I" + HOST,
-                           os.path.join(HOST, "shard_cluster_host_test.cpp"), "-o", exe])
-    r = subprocess.run([exe], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and "PASSED" in r.stdout, r.stdout[-3000:] + r.stderr[-1000:]
-    lines = r.stdout.splitlines()
+    out = S.host_program(tmp_path, "shard_cluster_host_test.cpp", timeout=900)
+    lines = out.splitlines()
     for want in ("zig-zag chain          slabs        R=8 nccl", "1-point tile R=8 peer", "overlapping  R=5 nccl",
                  "lattice above", "blobs, tolerance 0"):
         assert any(want in l for l in lines), want
-    assert "DIFFERS" not in r.stdout
+    assert "DIFFERS" not in out
 
 
 def _local_ids(whole, parts, r, tol):
-    """Rank r's local map as ids, selected in numpy: its tile, and every point of the other tiles inside the box of its
-    tile's finite points widened by the reach of r2, rounded outward by a float step."""
+    """Rank r's local map as ids: the box of its tile's finite points widened by the reach of r2, over every tile."""
     r2 = np.float32(np.float64(np.float32(tol)) ** 2)
-    tile = whole[parts[r], :3]
-    q = tile[np.isfinite(tile).all(1)].astype(np.float64)
-    h = np.sqrt(np.float64(r2)) * (1 + 2.0 ** -20) + 2.0 ** -60
-    lo = np.nextafter((q - h).min(0).astype(np.float32), np.float32(-np.inf))
-    hi = np.nextafter((q + h).max(0).astype(np.float32), np.float32(np.inf))
-    pts = whole[:, :3]
-    with np.errstate(invalid="ignore"):
-        inside = (pts >= lo).all(1) & (pts <= hi).all(1)
-    sel = np.zeros(len(whole), bool)
-    for s, p in enumerate(parts):
-        if s != r:
-            sel[p] |= inside[p]
-    sel[parts[r]] = True
-    return np.nonzero(sel)[0]  # ascending: the id order
+    return S.local_ids(whole, parts, r, *S.halo_box(whole[parts[r]], r2))
 
 
 def _stitched_labels(orc, whole, parts, tol):

@@ -2,56 +2,28 @@
 oracle (k-NN rows and statistics over one rank's tile plus its halo, indexed in id order, equal the whole map's bit for
 bit, and the filters' rules applied to the ranks' concatenated statistics give the whole map's masks), and the kernels of
 pcl_b200/csrc/shard_filter_kernels.cuh (driven by shard_filter.cu) compiled for the host."""
-import os
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-HOST = os.path.join(ROOT, "tests", "host")
+import _sharded as S
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
-                    reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
+@S.needs_host_compiler
 def test_sharded_filter_kernels_on_the_host(tmp_path):
     """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols: the id mapping of k-NN rows, the SOR partial sums, their
     exchange and the rank-order fold (every rank the same threshold, within 1e-12 of the sequential one), and both mask
     rules against the facade's."""
-    exe = str(tmp_path / "shard_filter_host_test")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-frounding-math", "-ffp-contract=off", "-fno-fast-math",
-                           "-I" + CUDA_INC, "-I" + os.path.join(ROOT, "include"), "-I" + HOST,
-                           os.path.join(HOST, "shard_filter_host_test.cpp"), "-o", exe])
-    r = subprocess.run([exe], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and "PASSED" in r.stdout, r.stdout[-3000:] + r.stderr[-1000:]
-    assert any(l.startswith("random, one rank empty") and "R=8 nccl" in l for l in r.stdout.splitlines())
-    assert "DIFFERS" not in r.stdout
+    out = S.host_program(tmp_path, "shard_filter_host_test.cpp", timeout=900)
+    assert any(l.startswith("random, one rank empty") and "R=8 nccl" in l for l in out.splitlines())
+    assert "DIFFERS" not in out
 
 
 def _halo_ids(orc, whole, parts, r, queries, k, radius):
-    """Rank r's local map as ids, selected in numpy: the box of its queries widened by their reach (the k-th nearest
-    distance in its own tile, or the radius), rounded outward by a float step, over every tile."""
-    tile = whole[parts[r]]
-    fin = np.isfinite(queries[:, :3]).all(1)
-    q = queries[fin, :3].astype(np.float64)
-    if k:
-        _, kth = orc.Index(tile).knn_stats(queries[fin], k)
-        rho = np.sqrt(kth.astype(np.float64))
-    else:
-        rho = np.full(len(q), radius * radius, np.float32).astype(np.float64) ** 0.5
-    h = rho * (1 + 2.0 ** -20) + 2.0 ** -60
-    lo = np.nextafter((q - h[:, None]).min(0).astype(np.float32), np.float32(-np.inf))
-    hi = np.nextafter((q + h[:, None]).max(0).astype(np.float32), np.float32(np.inf))
-    pts = whole[:, :3]
-    inside = (pts >= lo).all(1) & (pts <= hi).all(1)
-    sel = np.zeros(len(whole), bool)
-    for s, p in enumerate(parts):
-        if s != r:
-            sel[p] |= inside[p]
-    sel[parts[r]] = True
-    return np.nonzero(sel)[0]  # ascending: the id order
+    """Rank r's local map as ids: the box of its queries widened by their reach (the k-th nearest distance in its own
+    tile, or the radius) over every tile."""
+    q = queries[S.finite_rows(queries)]
+    rho2 = orc.Index(whole[parts[r]]).knn_stats(q, k)[1] if k else np.float32(radius * radius)
+    return S.local_ids(whole, parts, r, *S.halo_box(q, rho2))
 
 
 def _layouts(whole, R, rng):
@@ -68,22 +40,6 @@ def _layouts(whole, R, rng):
     parts[-2] = np.r_[parts[-2], parts[-1]]
     parts[-1] = np.array([len(whole), len(whole) + 1])
     yield "a far tile of 2 points", parts, far
-
-
-def _sor_rule(means, finite, mean_k_std_mul):
-    """statistical_outlier_removal.hpp:100-135 in record order (np.cumsum is sequential), d * d in float"""
-    s = np.cumsum(means.astype(np.float64))[-1]
-    sq = np.cumsum((means * means).astype(np.float64))[-1]
-    valid = float(finite.sum())
-    thr = s / valid + mean_k_std_mul * np.sqrt((sq - s * s / valid) / (valid - 1))
-    return (means.astype(np.float64) <= thr).astype(np.uint8)
-
-
-def _ror_rule(kth, finite, is_dense, radius):
-    """radius_outlier_removal.hpp:86-150, negative = false"""
-    if is_dense:
-        return (np.isfinite(kth) & ~(radius * radius < kth.astype(np.float64))).astype(np.uint8)
-    return (finite & (kth < np.float32(radius * radius))).astype(np.uint8)
 
 
 def _mask(kept, n):
@@ -130,10 +86,10 @@ def test_oracle_knn_and_filters_over_tile_and_halo_equal_the_whole_map(orc, layo
             if k in (2, 9):  # ROR with min_pts = k - 1
                 for is_dense in (True, False):
                     want = _mask(ref_index.radius_outlier_removal(queries, 0.02, k - 1, is_dense=is_dense), len(queries))
-                    assert _ror_rule(gk, fin_all[parts[r]], is_dense, 0.02).tobytes() == want.tobytes(), (layout, r, k)
+                    assert S.ror_rule(gk, fin_all[parts[r]], is_dense, 0.02).tobytes() == want.tobytes(), (layout, r, k)
             assert len(local) < len(whole) or layout == "random" or (layout.startswith("a far") and r == R - 1), \
                 (layout, r, k, len(local))
         if k in (9, 51):  # SOR with mean_k = k - 1 over the concatenation of the ranks' queries in rank order
             every = np.concatenate(parts)
             want = _mask(ref_index.statistical_outlier_removal(np.ascontiguousarray(whole[every]), k - 1, 1.0), len(every))
-            assert _sor_rule(np.concatenate(means), fin_all[every], 1.0).tobytes() == want.tobytes(), (layout, k)
+            assert S.sor_rule(np.concatenate(means), fin_all[every], 1.0)[0].tobytes() == want.tobytes(), (layout, k)

@@ -1,58 +1,30 @@
 """Normals of a map sharded across ranks without a GPU: the halo kernels (pcl_b200/csrc/shard_normals_kernels.cuh, driven
 by shard_normals.cu) compiled for the host, and the exactness argument checked on the CPU oracle: the normals of the
 whole map equal, bit for bit, the normals over one rank's tile plus its halo, indexed in id order."""
-import os
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-HOST = os.path.join(ROOT, "tests", "host")
+import _sharded as S
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
-                    reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
+@S.needs_host_compiler
 def test_sharded_normals_halo_layout_on_the_host(tmp_path):
     """1 / 2 / 3 / 5 / 8 simulated ranks, both exchange protocols, the segments placed and read with the layout functions
     of peer_tables.cuh that the driver calls: every rank's box is the outward-rounded union of its
     queries' reaches, its halo is exactly the other tiles' points inside that box, and every whole-map neighbour of every
     query (ties at the k-th distance included; radius: d2 <= r^2) lies in the tile plus the halo — slabs, a random
     partition, overlapping tiles sharing ids, a far tile with fewer than k points, k = 3 / 16 / 40 and a radius."""
-    exe = str(tmp_path / "shard_normals_host_test")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-frounding-math", "-ffp-contract=off", "-fno-fast-math",
-                           "-I" + CUDA_INC, "-I" + os.path.join(ROOT, "include"), "-I" + HOST,
-                           os.path.join(HOST, "shard_normals_host_test.cpp"), "-o", exe])
-    r = subprocess.run([exe], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and "PASSED" in r.stdout, r.stdout[-3000:] + r.stderr[-1000:]
-    assert any(l.startswith("a far tile of 2 points") and "R=8 nccl" in l for l in r.stdout.splitlines())
-    assert "DIFFERS" not in r.stdout
+    out = S.host_program(tmp_path, "shard_normals_host_test.cpp", timeout=900)
+    assert any(l.startswith("a far tile of 2 points") and "R=8 nccl" in l for l in out.splitlines())
+    assert "DIFFERS" not in out
 
 
 def _halo_ids(orc, whole, parts, r, queries, k, radius):
-    """Rank r's local map as ids, selected in numpy: the box of its queries widened by their reach (the k-th nearest
-    distance in its own tile, or the radius), rounded outward by a float step, over every tile."""
-    tile = whole[parts[r]]
-    fin = np.isfinite(queries[:, :3]).all(1)
-    q = queries[fin, :3].astype(np.float64)
-    if k:
-        _, kth = orc.Index(tile).knn_stats(queries[fin], k)
-        rho = np.sqrt(kth.astype(np.float64))
-    else:
-        rho = np.full(len(q), radius * radius, np.float32).astype(np.float64) ** 0.5
-    h = rho * (1 + 2.0 ** -20) + 2.0 ** -60
-    lo = np.nextafter((q - h[:, None]).min(0).astype(np.float32), np.float32(-np.inf))
-    hi = np.nextafter((q + h[:, None]).max(0).astype(np.float32), np.float32(np.inf))
-    pts = whole[:, :3]
-    inside = (pts >= lo).all(1) & (pts <= hi).all(1)
-    sel = np.zeros(len(whole), bool)
-    for s, p in enumerate(parts):
-        if s != r:
-            sel[p] |= inside[p]
-    sel[parts[r]] = True
-    return np.nonzero(sel)[0]  # ascending: the id order
+    """Rank r's local map as ids: the box of its queries widened by their reach (the k-th nearest distance in its own
+    tile, or the radius) over every tile."""
+    q = queries[S.finite_rows(queries)]
+    rho2 = orc.Index(whole[parts[r]]).knn_stats(q, k)[1] if k else np.float32(radius * radius)
+    return S.local_ids(whole, parts, r, *S.halo_box(q, rho2))
 
 
 @pytest.mark.parametrize("layout", ["slabs", "random"])

@@ -8,29 +8,14 @@ under the library's own distance expression and tie rule, against the facade's h
 CPU oracle.  The search programs run twice: on an index built by a small reference builder (tests/host/host_index.h) and on
 the index the REAL build kernels produce (tests/host/device_build.h replays lbvh.cu's sequence)."""
 import os
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = "/usr/local/cuda/include"
-HOST = os.path.join(ROOT, "tests", "host")
+from _sharded import ROOT, host_program, needs_host_compiler
 
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")) or shutil.which("g++") is None,
-                                reason="needs g++ and the CUDA headers (vector types only; nothing is run on a device)")
+pytestmark = needs_host_compiler
 
 DEVICE_BUILD = ["-DPCLB_TEST_DEVICE_BUILD", "-DPCLB_HOST_EMULATION", '-DPCLB_HOST_EXTRA_SHIMS="warp_emu.h"']
-
-
-def _run(tmp_path, source, args=(), defines=(), link=()):
-    exe = str(tmp_path / (os.path.splitext(source)[0] + ("_dev" if defines else "")))
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-frounding-math", "-ffp-contract=off", "-fno-fast-math", *defines,
-                           "-I" + CUDA_INC, "-I" + os.path.join(ROOT, "include"), "-I" + HOST,
-                           "-I" + os.path.join(ROOT, "pcl_b200", "pcl_compat"), os.path.join(HOST, source), "-o", exe, *link])
-    r = subprocess.run([exe, *args], capture_output=True, text=True)
-    assert r.returncode == 0 and "PASSED" in r.stdout, r.stdout[-3000:] + r.stderr[-1000:]
-    return r.stdout
 
 
 def test_index_build_kernels_on_the_host(tmp_path):
@@ -38,7 +23,7 @@ def test_index_build_kernels_on_the_host(tmp_path):
     child boxes exact, subtree leaf ranges, and the cell table — every occupied cell of every level maps to a subtree that
     holds all of (and, for a node, only) its points — on fifteen clouds incl. duplicates, a lattice, degenerate frames and
     map-scale frames (a map at 1e5, a frame straddling zero, a cube stretched by one outlier 1e6 away)."""
-    out = _run(tmp_path, "lbvh_host_test.cpp", ["2"])
+    out = host_program(tmp_path, "lbvh_host_test.cpp", ["2"])
     assert "cell table levels 1.." in out and "map at 1e5" in out and "straddling zero" in out and "one outlier 1e6 away" in out
 
 
@@ -48,7 +33,7 @@ def test_device_traversal_header_on_the_host(tmp_path, device_built):
     variants on twelve scene families (map-scale frames among them) against brute force — with and without the table, no / the true / a random seed,
     the TRACK visitor's lower bound — and the temporal-coherence chain of k_search over drifting queries: a skipped walk
     never keeps a match that stopped being the nearest.  Five seeded mutations of the header are caught by this program."""
-    out = _run(tmp_path, "traverse_host_test.cpp", ["2"], DEVICE_BUILD if device_built else ())
+    out = host_program(tmp_path, "traverse_host_test.cpp", ["2"], DEVICE_BUILD if device_built else ())
     assert "map at 1e5" in out and "straddling zero" in out and "one outlier 1e6 away" in out
 
 
@@ -58,7 +43,7 @@ def test_per_thread_search_kernels_on_the_host(tmp_path, device_built):
     k_normals<K>, and the list-based forms k_stats_from_lists / k_normals_from_lists (k > 32) / k_normals_from_csr (radius
     normals) — block by block against brute force (lists bit for bit, ties and duplicates included) and, for the normals,
     against the host computePointNormal."""
-    _run(tmp_path, "search_host_test.cpp", ["2"], DEVICE_BUILD if device_built else ())
+    host_program(tmp_path, "search_host_test.cpp", ["2"], DEVICE_BUILD if device_built else ())
 
 
 @pytest.mark.parametrize("device_built", [False, True], ids=["reference-index", "device-built-index"])
@@ -67,7 +52,7 @@ def test_warp_knn_kernel_on_an_emulated_warp(tmp_path, device_built):
     the normals epilogue) on an emulated warp: every certified row equals brute force bit for bit, every normal equals the
     host computePointNormal on the brute-force list, and (reference index) the constructed shared-leaf scene — the bug the
     10 M-row comparison found on the device — passes; it fails on the kernel as it was before the fix."""
-    out = _run(tmp_path, "knn_warp_host_test.cpp", ["1"], DEVICE_BUILD if device_built else ())
+    out = host_program(tmp_path, "knn_warp_host_test.cpp", ["1"], DEVICE_BUILD if device_built else ())
     assert "shared leaf, constructed #5" in out and "map at 1e5" in out and "straddling zero" in out and "one outlier 1e6 away" in out
 
 
@@ -85,7 +70,7 @@ def test_whole_icp_iterations_about_the_svd_origin_on_an_emulated_block(tmp_path
     import oracle
     oracle.build()
     odir = os.path.join(ROOT, "oracle")
-    out = _run(tmp_path, "icp_host_test.cpp", (), DEVICE_BUILD if device_built else (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
+    out = host_program(tmp_path, "icp_host_test.cpp", (), DEVICE_BUILD if device_built else (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
     assert "tracking automatic" in out and "point-to-plane LLS double" in out and "reciprocal" in out and "trimmed rejectors" in out and "back-projection" in out and "500 m out" in out
 
 
@@ -97,7 +82,7 @@ def test_voxelgrid_kernels_on_the_host(tmp_path):
     import oracle
     oracle.build()
     odir = os.path.join(ROOT, "oracle")
-    out = _run(tmp_path, "voxel_host_test.cpp", ["2"], (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
+    out = host_program(tmp_path, "voxel_host_test.cpp", ["2"], (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
     assert "overflow guard" in out and "PointNormal, min 2 points" in out
 
 
@@ -108,7 +93,7 @@ def test_rejector_kernels_on_the_host(tmp_path):
     import oracle
     oracle.build()
     odir = os.path.join(ROOT, "oracle")
-    out = _run(tmp_path, "reject_host_test.cpp", ["2"], (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
+    out = host_program(tmp_path, "reject_host_test.cpp", ["2"], (), ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
     assert "every distance equal" in out and "DIFFERS" not in out
 
 
@@ -122,5 +107,5 @@ def test_searcher_consumer_kernels_on_the_host(tmp_path):
     import oracle
     oracle.build()
     odir = os.path.join(ROOT, "oracle")
-    out = _run(tmp_path, "consumers_host_test.cpp", (), DEVICE_BUILD, ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
+    out = host_program(tmp_path, "consumers_host_test.cpp", (), DEVICE_BUILD, ["-L" + odir, "-lpcl_oracle", "-Wl,-rpath," + odir])
     assert "reciprocal, index subset" in out and "GICP covariances" in out and "back projection" in out and "Euclidean clustering" in out

@@ -28,7 +28,8 @@ import torch
 import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+import _sharded as S  # noqa: E402
 import pcl_b200 as P  # noqa: E402
 
 STAGES = ("sharded_cluster_halo", "sharded_cluster_local", "sharded_cluster_stitch", "sharded_cluster_labels")
@@ -70,18 +71,6 @@ def card():
         return "unknown"
 
 
-def halo_points(whole, tile_ids, tol):
-    """points of the other tiles inside this rank's box (the tile widened by the reach of r2, rounded outward)"""
-    r2 = np.float32(np.float64(np.float32(tol)) ** 2)
-    q = whole[tile_ids, :3]
-    h = np.sqrt(np.float64(r2)) * (1 + 2.0 ** -20) + 2.0 ** -60
-    lo = np.nextafter((q.min(0) - h).astype(np.float32), np.float32(-np.inf))
-    hi = np.nextafter((q.max(0) + h).astype(np.float32), np.float32(np.inf))
-    inside = ((whole[:, :3] >= lo) & (whole[:, :3] <= hi)).all(1)
-    inside[tile_ids] = False
-    return int(inside.sum())
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--points", type=int, default=20_000_000)
@@ -92,11 +81,9 @@ def main():
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     shared = torch.cuda.device_count() < world
     dev = 0 if shared else rank
-    torch.cuda.set_device(dev)
-    dist.init_process_group("gloo")
     whole = scene(a.points)
     ref_ms, ref_labels, n_clusters = None, None, None
-    if rank == 0:  # the reference, while the other ranks wait
+    if rank == 0:  # the reference, before the communicator
         rctx = P.Context(dev)
         d_whole = torch.from_numpy(whole).to(f"cuda:{dev}")
         rindex = P.Index(rctx, d_whole)
@@ -112,11 +99,7 @@ def main():
         n_clusters = int(len(np.unique(ref_labels[ref_labels >= 0])))
         del rindex, d_whole, out
         rctx.close()
-    dist.barrier()
-    ctx = P.Context(dev)
-    handles = [None] * world
-    dist.all_gather_object(handles, ctx.comm_export())
-    ctx.comm_import(rank, world, handles)
+    ctx = S.join(nccl=False, device=dev).ctx  # the other ranks wait here while rank 0 takes its reference
     ids_all = np.arange(a.points)
     slab = np.minimum((whole[:, 0] / 30.0 * world).astype(np.int64), world - 1)  # R = 2: cut at x = 15 m, through objects
     perm = np.random.default_rng(5).permutation(a.points)
@@ -148,13 +131,12 @@ def main():
         exact = None
         if rank == 0:
             exact = lab.tobytes() == np.ascontiguousarray(ref_labels[ids]).tobytes()
-        halo = halo_points(whole, ids, a.tolerance)
+        r2 = np.float32(np.float64(np.float32(a.tolerance)) ** 2)  # the tile widened by the reach of r2
+        halo = S.halo_points(whole, ids, *S.halo_box(whole[ids], r2))
         mine = dict(rank=rank, tile_points=int(len(ids)), halo_points=halo, halo_fraction=round(halo / len(ids), 5),
                     stage_ms=stage, wall_ms=round(wall_ms, 3))
-        allr = [None] * world
-        dist.all_gather_object(allr, mine)
-        labs = [None] * world
-        dist.all_gather_object(labs, np.unique(lab))
+        allr = S.gathered(mine)
+        labs = S.gathered(np.unique(lab))
         if rank == 0:
             seen = np.concatenate(labs)
             _, times = np.unique(seen, return_counts=True)

@@ -26,7 +26,8 @@ import torch
 import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+import _sharded as S  # noqa: E402
 import pcl_b200 as P  # noqa: E402
 
 STAGES = ("sharded_filter_bound", "sharded_filter_halo", "sharded_filter_build", "sharded_filter_stats", "sharded_filter_sor")
@@ -50,25 +51,6 @@ def card():
         return "unknown"
 
 
-def halo_points(whole, tile_ids, kth):
-    """points of the other tiles inside this rank's box (the bound of shard_normals.cu: sharded_local_map, rounded outward by a float step)"""
-    q = whole[tile_ids, :3].astype(np.float64)
-    h = np.sqrt(kth.astype(np.float64)) * (1 + 2.0 ** -20) + 2.0 ** -60
-    lo = np.nextafter((q - h[:, None]).min(0).astype(np.float32), np.float32(-np.inf))
-    hi = np.nextafter((q + h[:, None]).max(0).astype(np.float32), np.float32(np.inf))
-    inside = ((whole[:, :3] >= lo) & (whole[:, :3] <= hi)).all(1)
-    inside[tile_ids] = False
-    return int(inside.sum())
-
-
-def sequential_thr(means, std_mul):
-    """statistical_outlier_removal.hpp:100-112 in record order (np.cumsum is sequential; every point is finite)"""
-    s = np.cumsum(means.astype(np.float64))[-1]
-    sq = np.cumsum((means * means).astype(np.float64))[-1]
-    n = float(len(means))
-    return s / n + std_mul * np.sqrt((sq - s * s / n) / (n - 1))
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--points", type=int, default=20_000_000)
@@ -81,11 +63,9 @@ def main():
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     shared = torch.cuda.device_count() < world
     dev = 0 if shared else rank
-    torch.cuda.set_device(dev)
-    dist.init_process_group("gloo")
     whole = cfg3_surface(a.points)
     ref_ms, ref_means = None, None
-    if rank == 0:  # the reference, while the other ranks wait
+    if rank == 0:  # the reference, before the communicator
         rctx = P.Context(dev)
         d_whole = torch.from_numpy(whole).to(f"cuda:{dev}")
         rindex = P.Index(rctx, d_whole)
@@ -99,11 +79,7 @@ def main():
         rctx.profile(False)
         del rindex, d_whole
         rctx.close()
-    dist.barrier()
-    ctx = P.Context(dev)
-    handles = [None] * world
-    dist.all_gather_object(handles, ctx.comm_export())
-    ctx.comm_import(rank, world, handles)
+    ctx = S.join(nccl=False, device=dev).ctx  # the other ranks wait here while rank 0 takes its reference
     ids_all = np.arange(a.points)
     slab = np.minimum((whole[:, 0] / 10.0 * world).astype(np.int64), world - 1)
     perm = np.random.default_rng(5).permutation(a.points)
@@ -128,16 +104,16 @@ def main():
         if rank == 0:
             means, _ = tindex.knn_stats_sharded(d_tile, k)
             mean_exact = means.tobytes() == np.ascontiguousarray(ref_means[ids]).tobytes()
-            thr = sequential_thr(ref_means[np.concatenate(parts)], a.std_mul)
+            every = np.concatenate(parts)
+            _, (_, _, thr) = S.sor_rule(ref_means[every], S.finite_rows(whole[every]), a.std_mul)
             thr_rel = abs(st["thr"] - thr) / abs(thr)
         else:
             tindex.knn_stats_sharded(d_tile, k)
         _, kth = tindex.knn_stats(d_tile, k)
-        halo = halo_points(whole, ids, kth)
+        halo = S.halo_points(whole, ids, *S.halo_box(whole[ids], kth))
         mine = dict(rank=rank, tile_points=int(len(ids)), halo_points=halo, halo_fraction=round(halo / len(ids), 5),
                     stage_ms=stage, wall_ms=round(wall_ms, 3), kept=int(keep.sum()), thr=st["thr"])
-        allr = [None] * world
-        dist.all_gather_object(allr, mine)
+        allr = S.gathered(mine)
         if rank == 0:
             rec = dict(workload="sharded_sor_cfg3_surface", partition=pname, ranks=world, gpus_shared=shared,
                        map_points=a.points, mean_k=a.mean_k, std_mul=a.std_mul, reps=a.reps,

@@ -21,7 +21,8 @@ import torch
 import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+import _sharded as S  # noqa: E402
 import pcl_b200 as P  # noqa: E402
 
 
@@ -53,13 +54,7 @@ def main():
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     shared = torch.cuda.device_count() < world
     dev = 0 if shared else rank
-    torch.cuda.set_device(dev)
-    dist.init_process_group("gloo")
-    ctx = P.Context(dev)
-    if world > 1:
-        handles = [None] * world
-        dist.all_gather_object(handles, ctx.comm_export())
-        ctx.comm_import(rank, world, handles)
+    ctx = S.join(nccl=False, device=dev).ctx
     extent = 100.0
     whole = surface(a.map_points, 1, extent)
     cut = np.minimum((whole[:, 0] / extent * world).astype(np.int64), world - 1)
@@ -105,8 +100,7 @@ def main():
                 per_scope[s] += ctx.profile_get(s)[0] / a.aligns
             iters = st["iterations"]
     ctx.profile(False)
-    finals = [None] * world
-    dist.all_gather_object(finals, st["final"].tobytes())
+    finals = S.gathered(st["final"].tobytes())
     assert all(f == finals[0] for f in finals), "ranks disagree on the transform"
     per_pt_index = stats["bytes"] / max(len(ids), 1)
     per_pt_peak = (free0 - free1) / max(len(ids), 1)

@@ -13,7 +13,8 @@ import torch
 import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+import _sharded as S  # noqa: E402
 import pcl_b200 as P  # noqa: E402
 
 CHAIN4 = [(P.REJ_MEDIAN, 3.0, 0), (P.REJ_ONE_TO_ONE, 0.0, 0), (P.REJ_TRIMMED, 0.9, 100), (P.REJ_DISTANCE, 0.2, 0)]
@@ -50,22 +51,16 @@ def reject_ms(ctx, idx, src):
 
 def main():
     out = sys.argv[1] if len(sys.argv) > 1 else None
-    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-    torch.cuda.set_device(0)
-    dist.init_process_group("gloo")
-    ctx = P.Context(0)
-    handles = [None] * world
-    dist.all_gather_object(handles, ctx.comm_export())
-    ctx.comm_import(rank, world, handles)
+    me = S.join(nccl=False, device=0)
+    rank, world, ctx = me.rank, me.world, me.ctx
     tgt, src = cloud()
     idx = P.Index(ctx, tgt)
     lo, hi = rank * N // world, (rank + 1) * N // world
     ms, n, st = reject_ms(ctx, idx, np.ascontiguousarray(src[lo:hi]))
-    got = [None] * world
-    dist.all_gather_object(got, (ms, n))
+    got = S.gathered((ms, n))
     dist.barrier()
     if rank == 0:
-        single = P.Context(0)
+        single = me.ref
         ms1, n1, st1 = reject_ms(single, P.Index(single, tgt), src)
         props = torch.cuda.get_device_properties(0)
         power = os.popen("nvidia-smi --query-gpu=power.limit --format=csv,noheader -i 0").read().strip()
