@@ -23,7 +23,8 @@ extern "C" {
  * correspondence estimators, normal estimation with k > 32 or a radius, GICP covariances, pclb200_cluster_labels.
  * The normals of a sharded map come from pclb200_normals_knn_sharded / pclb200_normals_radius_sharded, and the clusters
  * of a sharded map come from pclb200_cluster_labels_sharded, its k-NN lists and outlier filters from pclb200_knn_sharded,
- * pclb200_knn_stats_sharded, pclb200_statistical_outlier_sharded and pclb200_radius_outlier_sharded. */
+ * pclb200_knn_stats_sharded, pclb200_statistical_outlier_sharded and pclb200_radius_outlier_sharded, its VoxelGrid from
+ * pclb200_voxelgrid_sharded. */
 PCLB200_API int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                         const int32_t* ids, pclb200_index** out);
 
@@ -122,6 +123,30 @@ PCLB200_API int pclb200_radius_outlier_sharded(pclb200_ctx* ctx, const pclb200_i
  * communicator, for a tile built without ids, for a negative tolerance and for n_labels other than the tile's records. */
 PCLB200_API int pclb200_cluster_labels_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, double tolerance,
                                                int32_t* out_labels, int64_t* out_sizes, size_t n_labels);
+
+/* VoxelGrid of a map sharded across the ranks of the context's communicator.  Collective: every rank passes its own
+ * records pts[0..n) and their ids (the map is the union of the ids; on one rank they are distinct and lie in
+ * [0, 2^31 - 2]; an id held by two ranks must name the same record, and it counts once).  The output is pclb200_voxelgrid
+ * (pclb200_voxelgrid_normals when normals is given) of the whole map with indices = the union of the ids in ascending
+ * order, byte for byte, split across the ranks:
+ * - each voxel of that output is returned by exactly one rank;
+ * - each rank returns its voxels ordered by voxel linear index;
+ * - out_voxel[i] is the linear index of row i (ijk . (1, div_b0, div_b0 div_b1) on the whole map's grid).
+ * Stable-sorting the concatenation of every rank's rows by out_voxel gives the whole output.  Every voxel a rank returns
+ * holds at least one of its own finite records, so *n_out <= n and a capacity of n rows always suffices.
+ * Arrays may be host or device memory; normals and out_normal_curv (both or neither) use the layouts of
+ * pclb200_voxelgrid_normals.  A rank with no finite record still takes part; when no rank has one, *n_out = 0 everywhere.
+ * Each rank receives, from the other ranks, every record whose voxel lies in the voxel range of its own records' box, and
+ * sorts its records plus those: both are resident at the peak (on a random partition that is nearly the whole map).
+ * PCLB200_ERR_INVALID on every rank, before any record moves, without an active communicator, for a NULL argument, a leaf
+ * <= 0 or non-finite, invalid ids on any rank, ranks that disagree on leaf or min_points_per_voxel, and normals given on
+ * some ranks and not on others.  PCLB200_ERR_LEAF_TOO_SMALL on every rank exactly when the whole map's grid trips
+ * pclb200_voxelgrid's integer guard. */
+PCLB200_API int pclb200_voxelgrid_sharded(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
+                                          const int32_t* ids, const void* normals /*nullable*/, size_t stride_n,
+                                          const float leaf[3], unsigned min_points_per_voxel,
+                                          float* out_xyz1, float* out_normal_curv /*nullable*/,
+                                          uint32_t* out_voxel, size_t* n_out);
 
 /* Collective over the context's communicator: every rank's send[0..n) concatenated in rank order, the same on every
  * rank.  *n_total is the total; recv (host or device, nullable) receives it when capacity >= *n_total, else nothing is

@@ -81,7 +81,7 @@ SYMBOLS = [
 SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", "pclb200_fitness_score_sharded",
                    "pclb200_normals_knn_sharded", "pclb200_normals_radius_sharded", "pclb200_cluster_labels_sharded",
                    "pclb200_comm_allgather_u64", "pclb200_knn_sharded", "pclb200_knn_stats_sharded",
-                   "pclb200_statistical_outlier_sharded", "pclb200_radius_outlier_sharded"]
+                   "pclb200_statistical_outlier_sharded", "pclb200_radius_outlier_sharded", "pclb200_voxelgrid_sharded"]
 
 _lib = None
 
@@ -157,6 +157,7 @@ def lib():
     L.pclb200_voxelgrid.argtypes = [vp, vp, sz, sz, vp, sz, C.c_int, fp, C.c_uint, vp, C.POINTER(sz)]
     L.pclb200_voxelgrid_tile.argtypes = [vp, vp, sz, sz, fp, fp, C.c_uint, vp, C.POINTER(sz)]
     L.pclb200_voxelgrid_normals.argtypes = [vp, vp, sz, sz, vp, sz, vp, sz, C.c_int, fp, C.c_uint, vp, vp, C.POINTER(sz)]
+    L.pclb200_voxelgrid_sharded.argtypes = [vp, vp, sz, sz, vp, vp, sz, fp, C.c_uint, vp, vp, vp, C.POINTER(sz)]
     L.pclb200_validate_transformation.argtypes = [vp, vp, vp, sz, sz, dp, C.c_int, C.c_double, dp]
     L.pclb200_inliers.argtypes = [vp, vp, vp, sz, sz, dp, C.c_float, vp, C.POINTER(sz)]
     L.pclb200_gicp_covariances.argtypes = [vp, vp, vp, sz, sz, C.c_int, C.c_double, vp]
@@ -353,6 +354,27 @@ class Context:
                                                int(is_dense), leaf, int(min_points_per_voxel),
                                                C.c_void_p(out.ctypes.data), C.c_void_p(nc.ctypes.data), C.byref(m)))
         return out[:m.value].copy(), nc[:m.value].copy()
+
+    def voxelgrid_sharded(self, cloud, ids, leaf, min_points_per_voxel=0, normal_offset=None):
+        """Collective VoxelGrid of a map sharded across the communicator's ranks: this rank's records and their ids in,
+        this rank's share of the whole map's output out, as (xyz1 rows, uint32 voxel indices) or, with the normal at float
+        normal_offset of each record (PointNormal: 4), (xyz1 rows, voxel indices, {nx,ny,nz,n4,curvature,0,0,0} rows).
+        Stable-sorting every rank's rows by voxel index gives pclb200_voxelgrid(_normals) of the whole map."""
+        b = _Buf(cloud)
+        ib = _Buf(ids, np.int32)
+        nb = _Buf(Field(cloud, normal_offset) if normal_offset is not None else None)
+        n = max(b.rows, 1)
+        leaf = (C.c_float * 3)(*[float(x) for x in np.broadcast_to(np.asarray(leaf, dtype=np.float32), (3,))])
+        out = np.empty((n, 4), dtype=np.float32)
+        vox = np.empty(n, dtype=np.uint32)
+        nc = np.empty((n, 8), dtype=np.float32) if normal_offset is not None else None
+        m = C.c_size_t()
+        _check(lib().pclb200_voxelgrid_sharded(self.h, b.ptr, b.rows, b.stride, ib.ptr, nb.ptr, nb.stride, leaf,
+                                               int(min_points_per_voxel), C.c_void_p(out.ctypes.data),
+                                               None if nc is None else C.c_void_p(nc.ctypes.data),
+                                               C.c_void_p(vox.ctypes.data), C.byref(m)))
+        got = (out[:m.value].copy(), vox[:m.value].copy())
+        return got if nc is None else got + (nc[:m.value].copy(),)
 
     def reject(self, corr, kind, p=0.0, min_correspondences=0):
         """One correspondence rejector (getRemainingCorrespondences); returns (remaining, median)."""

@@ -50,6 +50,10 @@ void radius_outlier_sharded(Ctx& c, const Index& tile, const void* pts, size_t n
 size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* indices, size_t n_idx, int is_dense,
                  const float leaf[3], unsigned min_pts, float* out_xyz1, const void* normals, size_t stride_n,
                  float* out_normal_curv, const float* grid_bounds = nullptr);
+// shard_voxel.cu
+size_t voxelgrid_sharded(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* ids, const void* normals,
+                         size_t stride_n, const float leaf[3], unsigned min_pts, float* out_xyz1, float* out_normal_curv,
+                         uint32_t* out_voxel, size_t* n_out);
 // comm.cu
 void comm_unique_id(void* out128);
 void comm_export(Ctx& c, void* out64);
@@ -1010,6 +1014,16 @@ int pclb200_voxelgrid_normals(pclb200_ctx* ctx, const void* pts, size_t n, size_
     ProfScope ps(c, "voxelgrid");
     *n_out = voxelgrid(c, pts, n, stride, indices, n_idx, is_dense, leaf, min_points_per_voxel, out_xyz1, normals,
                        stride_n, out_normal_curv);
+  });
+}
+
+int pclb200_voxelgrid_sharded(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride, const int32_t* ids,
+                              const void* normals, size_t stride_n, const float leaf[3], unsigned min_points_per_voxel,
+                              float* out_xyz1, float* out_normal_curv, uint32_t* out_voxel, size_t* n_out)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    voxelgrid_sharded(c, pts, n, stride, ids, normals, stride_n, leaf, min_points_per_voxel, out_xyz1, out_normal_curv,
+                      out_voxel, n_out);
   });
 }
 

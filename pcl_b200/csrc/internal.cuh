@@ -258,6 +258,9 @@ struct Index {
 Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* subset, size_t n_subset);
 // point i labelled ids[i] (non-negative, distinct, < 2^31 - 1) instead of i: one tile of a map sharded across ranks
 Index* build_index_ids(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* ids);
+// the faults of the caller's ids d_ids[0..n) (device): kIdOutOfRange (outside [0, 2^31 - 2]) | kIdRepeated; synchronises
+enum { kIdOutOfRange = 1, kIdRepeated = 2 };
+int id_faults(Ctx& c, const int32_t* d_ids, size_t n);
 // device-resident source already dense float4 (w ignored): used for the reciprocal source tree (rebuilt every iteration:
 // no cell table) and for the local map of a sharded map (shard_normals.cu: with the cell table)
 Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig /*nullable*/,
@@ -347,6 +350,19 @@ size_t correspondences_by_normals(Ctx& c, Index& tgt, int kind, const void* src,
 size_t reject_surface_normal(Ctx& c, const pclb200_corr* in, size_t n, const void* src_normals, size_t n_src,
                              size_t stride_sn, const void* tgt_normals, size_t n_tgt, size_t stride_tn,
                              double threshold, pclb200_corr* out);
+
+// The launches of the VoxelGrid kernels voxelgrid() and the VoxelGrid of a sharded map share (voxel.cu defines the kernels
+// of voxel_kernels.cuh, shard_voxel.cu runs them through these).  vg_minmax: the min / max / count of k_vg_minmax over n
+// dense points, synchronised.  vg_load_normals: the normal planes (k_vg_load_nc) of n records of a host-or-device array,
+// or of its records indices[0..n_idx).  vg_runs: k_vg_runs.  vg_reduce: k_vg_centroids, and k_vg_normals when nc is given.
+struct MinMaxAcc;
+struct RunRef;
+MinMaxAcc vg_minmax(Ctx& c, const float4* d_pts, size_t n);
+void vg_load_normals(Ctx& c, const void* normals, size_t n, size_t stride_n, const int32_t* indices, size_t n_idx,
+                     float4* d_nc);
+void vg_runs(Ctx& c, const unsigned* starts, size_t n_runs, size_t n_valid, RunRef* runs);
+void vg_reduce(Ctx& c, const float4* pts, const float4* nc, const int32_t* vals, const RunRef* runs, size_t n_runs,
+               float4* out, float4* out_nc);
 
 // connected components of the d2 < tolerance^2 graph over the indexed points (cluster.cu)
 void cluster_labels(Ctx& c, const Index& idx, double tolerance, int32_t* d_labels /* idx.n_cloud */);

@@ -314,7 +314,7 @@ Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int3
 }
 
 // ---- labelled index: one tile of a map, its points carrying the caller's ids -------------------------------------
-// sorted ids: bit 0 = an id outside [0, 2^31 - 2] (2^31 - 1 marks padding), bit 1 = two equal ids
+// sorted ids: kIdOutOfRange = an id outside [0, 2^31 - 2] (2^31 - 1 marks padding), kIdRepeated = two equal ids
 __global__ void k_check_sorted_ids(const int32_t* __restrict__ sorted, size_t n, int* __restrict__ flag)
 {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
@@ -322,9 +322,33 @@ __global__ void k_check_sorted_ids(const int32_t* __restrict__ sorted, size_t n,
     return;
   const int32_t v = sorted[i];
   if (v < 0 || v == kSentinelIndex)
-    atomicOr(flag, 1);
+    atomicOr(flag, kIdOutOfRange);
   if (i > 0 && sorted[i - 1] == v)
-    atomicOr(flag, 2);
+    atomicOr(flag, kIdRepeated);
+}
+
+int id_faults(Ctx& c, const int32_t* d_ids, size_t n)
+{
+  cudaStream_t s = c.stream;
+  if (!n)
+    return 0;
+  DevBuf<int32_t> sorted;
+  sorted.alloc(n, s);
+  size_t tb = 0;
+  PCLB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_ids, sorted.p, (int)n, 0, 32, s));
+  DevBuf<unsigned char> tmp;
+  tmp.alloc(tb, s);
+  PCLB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tb, d_ids, sorted.p, (int)n, 0, 32, s));
+  c.launches += 5;
+  DevBuf<int> flag;
+  flag.alloc(1, s);
+  PCLB_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(int), s));
+  k_check_sorted_ids<<<grid_for(n, 256), 256, 0, s>>>(sorted.p, n, flag.p);
+  ++c.launches;
+  int h = 0;
+  PCLB_CUDA(cudaMemcpyAsync(&h, flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  PCLB_CUDA(cudaStreamSynchronize(s));
+  return h;
 }
 
 // w = record number (as built) -> w = ids[record], the record number kept in slot_of_pos
@@ -352,28 +376,12 @@ Index* build_index_ids(Ctx& c, const void* pts, size_t n, size_t stride, const i
   PCLB_REQUIRE(pts != nullptr && n > 0, PCLB200_ERR_EMPTY, "cannot index an empty cloud (kdtree_flann.hpp:118-129)");
   PCLB_REQUIRE(ids != nullptr, PCLB200_ERR_INVALID, "index_build_ids: NULL ids");
   PCLB_REQUIRE(n < (size_t)0x7fffffff, PCLB200_ERR_INVALID, "cloud too large for int32 indices");
-  DevBuf<int32_t> d_ids, sorted;
+  DevBuf<int32_t> d_ids;
   d_ids.alloc(n, s);
-  sorted.alloc(n, s);
   PCLB_CUDA(cudaMemcpyAsync(d_ids.p, ids, n * sizeof(int32_t), cudaMemcpyDefault, s));
-  {
-    size_t tb = 0;
-    PCLB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_ids.p, sorted.p, (int)n, 0, 32, s));
-    DevBuf<unsigned char> tmp;
-    tmp.alloc(tb, s);
-    PCLB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tb, d_ids.p, sorted.p, (int)n, 0, 32, s));
-    c.launches += 5;
-    DevBuf<int> flag;
-    flag.alloc(1, s);
-    PCLB_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(int), s));
-    k_check_sorted_ids<<<grid_for(n, 256), 256, 0, s>>>(sorted.p, n, flag.p);
-    ++c.launches;
-    int h = 0;
-    PCLB_CUDA(cudaMemcpyAsync(&h, flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    PCLB_CUDA(cudaStreamSynchronize(s));
-    PCLB_REQUIRE(!(h & 1), PCLB200_ERR_INVALID, "index_build_ids: every id must lie in [0, 2^31 - 2]");
-    PCLB_REQUIRE(!(h & 2), PCLB200_ERR_INVALID, "index_build_ids: two points of the cloud carry the same id");
-  }
+  const int h = id_faults(c, d_ids.p, n);
+  PCLB_REQUIRE(!(h & kIdOutOfRange), PCLB200_ERR_INVALID, "index_build_ids: every id must lie in [0, 2^31 - 2]");
+  PCLB_REQUIRE(!(h & kIdRepeated), PCLB200_ERR_INVALID, "index_build_ids: two points of the cloud carry the same id");
   DevBuf<float4> dense;
   dense.alloc(n, s);
   load_xyz_as_float4(c, pts, n, stride, nullptr, 0, dense.p, s);

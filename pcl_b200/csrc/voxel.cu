@@ -23,6 +23,62 @@ struct IsSet {
   __host__ __device__ bool operator()(unsigned char v) const { return v != 0; }
 };
 
+MinMaxAcc vg_minmax(Ctx& c, const float4* d_pts, size_t n)
+{
+  cudaStream_t st = c.stream;
+  MinMaxAcc h;
+  for (int d = 0; d < 3; ++d) {
+    h.lo[d] = 0x7fffffff;
+    h.hi[d] = (int)0x80000000;
+  }
+  h.count = 0;
+  if (!n)
+    return h;
+  DevBuf<MinMaxAcc> acc;
+  acc.alloc(1, st);
+  PCLB_CUDA(cudaMemcpyAsync(acc.p, &h, sizeof(h), cudaMemcpyHostToDevice, st));
+  unsigned g = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)c.sm_count * 8);
+  k_vg_minmax<<<g, 256, 0, st>>>(d_pts, n, acc.p);
+  ++c.launches;
+  PCLB_CUDA(cudaMemcpyAsync(&h, acc.p, sizeof(h), cudaMemcpyDeviceToHost, st));
+  PCLB_CUDA(cudaStreamSynchronize(st));
+  return h;
+}
+
+void vg_load_normals(Ctx& c, const void* normals, size_t n, size_t stride_n, const int32_t* indices, size_t n_idx,
+                     float4* d_nc)
+{
+  // the remaining fields of a PointNormal / Normal record; the upload stops at the last byte of the last record's fields
+  // (as in strided_to_float4).  The staging buffers go back to the stream's cache after the launch: stream-ordered.
+  DevBuf<unsigned char> staged;
+  DevBuf<int32_t> staged_sub;
+  const unsigned char* d_src = on_device(c, static_cast<const unsigned char*>(normals), (n - 1) * stride_n + 20, staged);
+  const int32_t* d_sub = on_device(c, indices, n_idx, staged_sub);
+  const size_t cnt = indices ? n_idx : n;
+  k_vg_load_nc<<<grid_for(cnt, 256), 256, 0, c.stream>>>(d_src, stride_n, d_sub, cnt, d_nc);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
+void vg_runs(Ctx& c, const unsigned* starts, size_t n_runs, size_t n_valid, RunRef* runs)
+{
+  k_vg_runs<<<grid_for(n_runs, 256), 256, 0, c.stream>>>(starts, n_runs, n_valid, runs);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
+void vg_reduce(Ctx& c, const float4* pts, const float4* nc, const int32_t* vals, const RunRef* runs, size_t n_runs,
+               float4* out, float4* out_nc)
+{
+  k_vg_centroids<<<grid_for(n_runs, 128), 128, 0, c.stream>>>(pts, vals, runs, n_runs, out);
+  ++c.launches;
+  if (nc) {
+    k_vg_normals<<<grid_for(n_runs, 128), 128, 0, c.stream>>>(nc, vals, runs, n_runs, out_nc);
+    ++c.launches;
+  }
+  PCLB_CUDA(cudaGetLastError());
+}
+
 size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* indices, size_t n_idx, int is_dense,
                  const float leaf[3], unsigned min_pts, float* out_xyz1, const void* normals, size_t stride_n,
                  float* out_normal_curv, const float* grid_bounds)
@@ -37,29 +93,14 @@ size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t
   dense.alloc(cnt, st);
   load_xyz_as_float4(c, pts, n, stride, indices, n_idx, dense.p, st);
   // pass 1: min/max
-  DevBuf<MinMaxAcc> acc;
-  acc.alloc(1, st);
-  MinMaxAcc init;
-  for (int d = 0; d < 3; ++d) {
-    init.lo[d] = 0x7fffffff;
-    init.hi[d] = (int)0x80000000;
-  }
-  init.count = 0;
-  PCLB_CUDA(cudaMemcpyAsync(acc.p, &init, sizeof(init), cudaMemcpyHostToDevice, st));
-  unsigned g = (unsigned)std::min<size_t>((cnt + 255) / 256, (size_t)c.sm_count * 8);
-  k_vg_minmax<<<g, 256, 0, st>>>(dense.p, cnt, acc.p);
-  ++c.launches;
-  MinMaxAcc h;
-  PCLB_CUDA(cudaMemcpyAsync(&h, acc.p, sizeof(h), cudaMemcpyDeviceToHost, st));
-  PCLB_CUDA(cudaStreamSynchronize(st));
+  const MinMaxAcc h = vg_minmax(c, dense.p, cnt);
   const size_t n_valid = (size_t)h.count;
   if (n_valid == 0)
     return 0;
-  float mn[3], mx[3], inv[3];
+  float mn[3], mx[3];
   for (int d = 0; d < 3; ++d) {
     mn[d] = vord2f(h.lo[d]);
     mx[d] = vord2f(h.hi[d]);
-    inv[d] = 1.0f / leaf[d];  // inverse_leaf_size_ = 1 / leaf_size_ (voxel_grid.h:266,282)
   }
   if (grid_bounds) {
     // a spatial tile of a larger cloud: the grid (min_b, div_b) is the WHOLE cloud's, so that the tiles' voxels are the
@@ -71,25 +112,9 @@ size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t
       mx[d] = grid_bounds[3 + d];
     }
   }
-  // guard, in the reference's float arithmetic (voxel_grid.hpp:620-629)
-  volatile float e0 = (mx[0] - mn[0]) * inv[0], e1 = (mx[1] - mn[1]) * inv[1], e2 = (mx[2] - mn[2]) * inv[2];
-  const int64_t dx = (int64_t)e0 + 1, dy = (int64_t)e1 + 1, dz = (int64_t)e2 + 1;
-  if (dx * dy * dz > (int64_t)std::numeric_limits<int32_t>::max())
-    throw Error(PCLB200_ERR_LEAF_TOO_SMALL,
-                "VoxelGrid: leaf size is too small for the input dataset, integer indices would overflow "
-                "(voxel_grid.hpp:620-629)");
   VgParams gp;
-  int max_b[3], div_b[3];
-  for (int d = 0; d < 3; ++d) {
-    volatile float lo_s = mn[d] * inv[d], hi_s = mx[d] * inv[d];
-    gp.inv[d] = inv[d];
-    gp.min_b[d] = (int)std::floor(lo_s);
-    max_b[d] = (int)std::floor(hi_s);
-    div_b[d] = max_b[d] - gp.min_b[d] + 1;
-  }
-  gp.mul[0] = 1;
-  gp.mul[1] = div_b[0];
-  gp.mul[2] = div_b[0] * div_b[1];
+  if (!vg_grid(mn, mx, leaf, gp))
+    throw Error(PCLB200_ERR_LEAF_TOO_SMALL, kVgLeafTooSmall);
   // pass 2: keys ; pass 3: stable radix sort
   DevBuf<unsigned> keys_in, keys;
   DevBuf<int32_t> vals_in, vals;
@@ -126,8 +151,7 @@ size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t
   PCLB_CUDA(cudaStreamSynchronize(st));
   DevBuf<RunRef> runs_all, runs;
   runs_all.alloc(n_runs, st);
-  k_vg_runs<<<grid_for(n_runs, 256), 256, 0, st>>>(starts.p, n_runs, n_valid, runs_all.p);
-  ++c.launches;
+  vg_runs(c, starts.p, n_runs, n_valid, runs_all.p);
   size_t n_out = n_runs;
   const RunRef* d_runs = runs_all.p;
   if (min_pts > 1) {
@@ -147,33 +171,21 @@ size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t
   }
   if (n_out == 0)
     return 0;
-  // pass 5: centroids
-  DevBuf<float4> out;
-  float4* const caller_out = reinterpret_cast<float4*>(out_xyz1);
-  k_vg_centroids<<<grid_for(n_out, 128), 128, 0, st>>>(dense.p, vals.p, d_runs, n_out, out_on_device(c, caller_out, n_out, out));
-  ++c.launches;
-  PCLB_CUDA(cudaGetLastError());
-  copy_out(c, caller_out, out, n_out);
-  if (normals && out_normal_curv) {
-    // the remaining fields of a PointNormal / Normal record, averaged over the same runs in the same order
+  // pass 5: centroids, and with normals the remaining fields averaged over the same runs in the same order
+  const bool with_nc = normals && out_normal_curv;
+  DevBuf<float4> nc, out, nout;
+  if (with_nc) {
     PCLB_REQUIRE(stride_n >= 20 && stride_n % 4 == 0, PCLB200_ERR_INVALID, "normal stride must be a multiple of 4 and >= 20");
-    // the upload stops at the last byte of the last record's fields (as in strided_to_float4)
-    DevBuf<unsigned char> staged;
-    DevBuf<int32_t> staged_sub;
-    const unsigned char* d_src = on_device(c, static_cast<const unsigned char*>(normals), (n - 1) * stride_n + 20, staged);
-    const int32_t* d_sub = on_device(c, indices, n_idx, staged_sub);
-    DevBuf<float4> nc, nout;
     nc.alloc(2 * cnt, st);
-    k_vg_load_nc<<<grid_for(cnt, 256), 256, 0, st>>>(d_src, stride_n, d_sub, cnt, nc.p);
-    float4* const caller_nout = reinterpret_cast<float4*>(out_normal_curv);
-    k_vg_normals<<<grid_for(n_out, 128), 128, 0, st>>>(nc.p, vals.p, d_runs, n_out,
-                                                       out_on_device(c, caller_nout, 2 * n_out, nout));
-    c.launches += 2;
-    PCLB_CUDA(cudaGetLastError());
-    copy_out(c, caller_nout, nout, 2 * n_out);
-    PCLB_CUDA(cudaStreamSynchronize(st));
-    return n_out;
+    vg_load_normals(c, normals, n, stride_n, indices, n_idx, nc.p);
   }
+  float4* const caller_out = reinterpret_cast<float4*>(out_xyz1);
+  float4* const caller_nout = reinterpret_cast<float4*>(out_normal_curv);
+  vg_reduce(c, dense.p, with_nc ? nc.p : nullptr, vals.p, d_runs, n_out, out_on_device(c, caller_out, n_out, out),
+            with_nc ? out_on_device(c, caller_nout, 2 * n_out, nout) : nullptr);
+  copy_out(c, caller_out, out, n_out);
+  if (with_nc)
+    copy_out(c, caller_nout, nout, 2 * n_out);
   PCLB_CUDA(cudaStreamSynchronize(st));
   return n_out;
 }

@@ -3,28 +3,9 @@
 // A header so that voxel.cu stays the host-side driver (CUB sort / select between the kernels) and
 // tests/host/voxel_host_test.cpp can compile the SAME kernels for the host and compare with the oracle bit for bit.
 #pragma once
-#include "internal.cuh"
+#include "voxel_grid.cuh"
 
 namespace pclb200 {
-
-struct MinMaxAcc {
-  int lo[3];
-  int hi[3];
-  unsigned long long count;
-};
-
-__device__ __forceinline__ int vf2ord(float f)
-{
-  int i = __float_as_int(f);
-  return i >= 0 ? i : i ^ 0x7fffffff;
-}
-static inline float vord2f(int i)
-{
-  int j = i >= 0 ? i : i ^ 0x7fffffff;
-  float f;
-  memcpy(&f, &j, 4);
-  return f;
-}
 
 __global__ void k_vg_minmax(const float4* __restrict__ p, size_t n, MinMaxAcc* acc)
 {
@@ -58,12 +39,6 @@ __global__ void k_vg_minmax(const float4* __restrict__ p, size_t n, MinMaxAcc* a
   }
 }
 
-struct VgParams {
-  float inv[3];
-  int min_b[3];
-  int mul[3];
-};
-
 __global__ void k_vg_keys(const float4* __restrict__ p, size_t n, VgParams g, unsigned* __restrict__ keys,
                           int32_t* __restrict__ vals)
 {
@@ -72,12 +47,8 @@ __global__ void k_vg_keys(const float4* __restrict__ p, size_t n, VgParams g, un
     return;
   float4 v = __ldg(p + i);
   unsigned key = 0xffffffffu;  // non-finite points sort to the tail and are cut off
-  if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
-    int ijk0 = (int)(floorf(__fmul_rn(v.x, g.inv[0])) - (float)g.min_b[0]);
-    int ijk1 = (int)(floorf(__fmul_rn(v.y, g.inv[1])) - (float)g.min_b[1]);
-    int ijk2 = (int)(floorf(__fmul_rn(v.z, g.inv[2])) - (float)g.min_b[2]);
-    key = (unsigned)(ijk0 * g.mul[0] + ijk1 * g.mul[1] + ijk2 * g.mul[2]);
-  }
+  if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z))
+    key = vg_linear(vg_ijk(v.x, g.inv[0], g.min_b[0]), vg_ijk(v.y, g.inv[1], g.min_b[1]), vg_ijk(v.z, g.inv[2], g.min_b[2]), g);
   keys[i] = key;
   vals[i] = (int32_t)i;
 }
@@ -99,10 +70,6 @@ __global__ void k_vg_keep(const unsigned* __restrict__ starts, size_t n_runs, si
   size_t b = starts[m], e = (m + 1 < n_runs) ? starts[m + 1] : n_valid;
   keep[m] = (e - b) >= min_pts ? 1 : 0;
 }
-
-struct RunRef {
-  unsigned begin, end;
-};
 
 __global__ void k_vg_runs(const unsigned* __restrict__ starts, size_t n_runs, size_t n_valid, RunRef* __restrict__ runs)
 {
