@@ -926,7 +926,10 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     a.ctrl = s.ctrl.p;
     a.track_sel = track_mode == PCLB200_TRACK_AUTO;  // the search runs only in the flavour of the device's decision
     const unsigned grid = persistent_blocks(c, s.n_q);
-    const unsigned wgrid = persistent_blocks(c, s.n_q, 256, 18);
+    // the search: 72 blocks per SM over the 5 that are resident, so a block walks only a few warp rounds and the SMs run
+    // out of work together (18 left the last blocks walking alone; a block per warp round pays for every launch that a
+    // finished loop or the unwanted tracking flavour returns from at once)
+    const unsigned wgrid = persistent_blocks(c, s.n_q, 256, 72);
     const unsigned agrid = std::min(persistent_blocks(c, s.n_q, 256, kAccumBlocksPerSM), s.red.max_blocks);
     const int n_enq = std::min(max_steps, std::max(1, s.P.max_iterations - s.loop.iterations));
     // sharded target: the accumulate kernels read the gathered records and the global matches
