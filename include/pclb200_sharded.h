@@ -24,7 +24,9 @@ extern "C" {
  * The normals of a sharded map come from pclb200_normals_knn_sharded / pclb200_normals_radius_sharded, and the clusters
  * of a sharded map come from pclb200_cluster_labels_sharded, its k-NN lists and outlier filters from pclb200_knn_sharded,
  * pclb200_knn_stats_sharded, pclb200_statistical_outlier_sharded and pclb200_radius_outlier_sharded, its VoxelGrid from
- * pclb200_voxelgrid_sharded. */
+ * pclb200_voxelgrid_sharded, its nearest and reciprocal correspondences, validation and inliers from
+ * pclb200_correspondences_sharded, pclb200_correspondences_normals_sharded, pclb200_validate_transformation_sharded
+ * and pclb200_inliers_sharded. */
 PCLB200_API int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                         const int32_t* ids, pclb200_index** out);
 
@@ -44,12 +46,70 @@ PCLB200_API int pclb200_icp_set_target_sharded(pclb200_icp* icp, const pclb200_i
 /* The same score over a target sharded across the ranks of the context's communicator (collective: every rank passes its
  * tile, built with pclb200_index_build_ids, and the same source).  Every rank returns the same value; the count of points
  * within max_range is one process's count on the whole map, the score agrees with one process's to fp64 round-off (the
- * sum runs in another order). */
+ * sum runs in another order).  Arguments one rank refuses (a tile without ids, a source count other ranks do not pass)
+ * are PCLB200_ERR_INVALID on every rank. */
 PCLB200_API int pclb200_fitness_score_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile,
                                               const void* src, size_t n, size_t stride,
                                               const int32_t* src_indices, size_t n_idx, int is_dense,
                                               const double T[16], int scalar_is_double, double max_range,
                                               double* score);
+
+/* The stand-alone consumers of the 1-NN search over a target sharded across the ranks of the context's communicator, so
+ * that any registration loop of correspondence estimation, pclb200_reject chains and pclb200_estimate_* runs against a map
+ * larger than one GPU.  Collective, in the layout of pclb200_icp_set_target_sharded and pclb200_fitness_score_sharded:
+ * every rank passes its tile (built with pclb200_index_build_ids; the map is the union of the ids, an id held by two ranks
+ * names the same point and normal) and the SAME whole source (array, src_indices, is_dense, transform), and every rank
+ * returns the same result.  "One index of the whole map" below is pclb200_index_build over the map with subset = the
+ * union of the ids; index_match holds map ids.  Arrays may be host or device memory.
+ *
+ * pclb200_correspondences_sharded: the list pclb200_correspondences returns on one index of the whole map, byte for
+ * byte.  idx_src != NULL selects the reciprocal variant; it is an ordinary index (pclb200_index_build) each rank builds
+ * over the same source.  out_xyz1 (nullable) receives one {x, y, z, 1} row per output correspondence, the matched map
+ * point; out_normals (nullable, needs tgt_normals: one record per record of the tile, stride stride_tn) receives its
+ * {nx, ny, nz, 0}.  Rows have a stride of 16 bytes (device rows 16-byte aligned), so they pass straight to
+ * pclb200_estimate_* with corr = NULL.
+ * pclb200_validate_transformation_sharded: pclb200_validate_transformation's score on one index of the whole map, as
+ * pclb200_fitness_score_sharded states it: the same value on every rank, the count exact, the score within fp64
+ * round-off of one process's (the sum runs in another order).
+ * pclb200_correspondences_normals_sharded: the list pclb200_correspondences_normals returns on one index of the whole
+ * map, byte for byte, with the same record outputs; k is clamped to the whole map's number of distinct finite ids, as
+ * pclb200_knn_sharded clamps k_eff.  tgt_normals (back projection, out_normals) has one record per record of the tile.
+ * Each rank's k nearest of its tile (as keys) are merged per source point into the whole map's row: every member of the
+ * whole map's k nearest that lies in a tile is among that tile's k nearest.  Every rank scores the candidates its tile
+ * holds; one u64 minimum of the n_q x k_eff score table gives every rank every score.  Memory per rank at the peak: its
+ * published rows (n_q k_eff 8 B), the other ranks' rows where they must be resident to merge (none on the peer path,
+ * which reads them in place; (R - 1) n_q k_eff 8 B under NCCL, an all-gather), the merged rows and the score table
+ * (2 n_q k_eff 8 B).
+ * pclb200_inliers_sharded: the inlier list of pclb200_inliers (float transform, strict d2 < threshold^2) on one index of
+ * the whole map, byte for byte; out_xyz1 as above.
+ *
+ * Each rank searches its tile; per source point the smallest key (d2 bits << 32 | id) over the ranks is the whole map's
+ * nearest neighbour (one u64-minimum exchange of n_q keys, 2 n_q for the reciprocal variant: the second key carries the
+ * verdict of the reverse search of whichever rank holds the winning point).  The record rows take a second exchange of
+ * n_q keys and n_q (n_q more with normals) 16-byte records, the one the sharded ICP session runs every iteration; both
+ * exchanges of a call draw one scratch table of the larger size, and under NCCL each reduces only its own words.
+ * PCLB200_ERR_INVALID on every rank, before any exchange, without an active communicator, and when any rank passes a
+ * tile built without ids, a NULL argument (a NULL tile included), k < 0, an unknown kind, missing source normals, back
+ * projection without target normals, a labelled idx_src, out_normals without tgt_normals, misaligned device rows, a query
+ * count other ranks do not pass, or a different choice of variant, kind, k and rows. */
+PCLB200_API int pclb200_correspondences_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile,
+                                                const pclb200_index* idx_src /*nullable*/, const void* src, size_t n,
+                                                size_t stride, const int32_t* src_indices, size_t n_idx, int is_dense,
+                                                double max_dist, const void* tgt_normals /*nullable*/, size_t stride_tn,
+                                                pclb200_corr* out, float* out_xyz1 /*nullable*/,
+                                                float* out_normals /*nullable*/, size_t* n_out);
+PCLB200_API int pclb200_correspondences_normals_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, int kind,
+                                                        const void* src, size_t n, size_t stride, const void* src_normals,
+                                                        size_t stride_sn, const void* tgt_normals /*nullable*/,
+                                                        size_t stride_tn, const int32_t* src_indices, size_t n_idx, int k,
+                                                        double max_dist, pclb200_corr* out, float* out_xyz1 /*nullable*/,
+                                                        float* out_normals /*nullable*/, size_t* n_out);
+PCLB200_API int pclb200_validate_transformation_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* src,
+                                                        size_t n, size_t stride, const double T[16], int scalar_is_double,
+                                                        double max_range, double* score);
+PCLB200_API int pclb200_inliers_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* src, size_t n,
+                                        size_t stride, const double T[16], float inlier_threshold, pclb200_corr* out,
+                                        float* out_xyz1 /*nullable*/, size_t* n_out);
 
 /* Collective over the context's communicator: every rank passes its tile (built with pclb200_index_build_ids) and its
  * OWN queries (any points; typically the tile's records).  out[i] is, bit for bit, what pclb200_normals_knn /

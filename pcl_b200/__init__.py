@@ -81,7 +81,9 @@ SYMBOLS = [
 SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", "pclb200_fitness_score_sharded",
                    "pclb200_normals_knn_sharded", "pclb200_normals_radius_sharded", "pclb200_cluster_labels_sharded",
                    "pclb200_comm_allgather_u64", "pclb200_knn_sharded", "pclb200_knn_stats_sharded",
-                   "pclb200_statistical_outlier_sharded", "pclb200_radius_outlier_sharded", "pclb200_voxelgrid_sharded"]
+                   "pclb200_statistical_outlier_sharded", "pclb200_radius_outlier_sharded", "pclb200_voxelgrid_sharded",
+                   "pclb200_correspondences_sharded", "pclb200_correspondences_normals_sharded",
+                   "pclb200_validate_transformation_sharded", "pclb200_inliers_sharded"]
 
 _lib = None
 
@@ -160,6 +162,12 @@ def lib():
     L.pclb200_voxelgrid_sharded.argtypes = [vp, vp, sz, sz, vp, vp, sz, fp, C.c_uint, vp, vp, vp, C.POINTER(sz)]
     L.pclb200_validate_transformation.argtypes = [vp, vp, vp, sz, sz, dp, C.c_int, C.c_double, dp]
     L.pclb200_inliers.argtypes = [vp, vp, vp, sz, sz, dp, C.c_float, vp, C.POINTER(sz)]
+    L.pclb200_correspondences_sharded.argtypes = [vp, vp, vp, vp, sz, sz, vp, sz, C.c_int, C.c_double, vp, sz, vp, vp, vp,
+                                                  C.POINTER(sz)]
+    L.pclb200_correspondences_normals_sharded.argtypes = [vp, vp, C.c_int, vp, sz, sz, vp, sz, vp, sz, vp, sz, C.c_int,
+                                                          C.c_double, vp, vp, vp, C.POINTER(sz)]
+    L.pclb200_validate_transformation_sharded.argtypes = L.pclb200_validate_transformation.argtypes
+    L.pclb200_inliers_sharded.argtypes = [vp, vp, vp, sz, sz, dp, C.c_float, vp, vp, C.POINTER(sz)]
     L.pclb200_gicp_covariances.argtypes = [vp, vp, vp, sz, sz, C.c_int, C.c_double, vp]
     L.pclb200_radius_into.argtypes = [vp, vp, vp, sz, sz, C.c_double, C.c_uint, vp, vp, vp, sz, C.POINTER(sz)]
     L.pclb200_comm_unique_id.argtypes = [vp]
@@ -603,6 +611,75 @@ class Index:
             fit = np.float32(fit + d)
         fit = np.float32(fit / np.float32(m.value)) if m.value else np.finfo(np.float32).max
         return c["index_query"].copy(), float(fit)
+
+    def correspondences_sharded(self, src, max_distance=np.sqrt(np.finfo(np.float64).max), indices=None, is_dense=True,
+                                src_index=None, tgt_normals=None, rows=False, normal_rows=False):
+        """Collective correspondences over a map sharded across the communicator's ranks (this index = this rank's tile,
+        built with ids=...; every rank passes the same source, src_index = its own ordinary index of that source for the
+        reciprocal variant).  Returns the list, or (list, xyz1 rows, normal rows) when rows / normal_rows: the matched map
+        point {x, y, z, 1} and its normal {nx, ny, nz, 0} per correspondence (normal_rows needs tgt_normals, one per
+        record of the tile), numpy float32 (m, 4), or None for the rows not asked for."""
+        b, ib, tn = _Buf(src), _Buf(indices, np.int32), _Buf(tgt_normals)
+        n = ib.rows if indices is not None else b.rows
+        out = np.empty(max(n, 1), dtype=CORR_DTYPE)
+        xyz = np.empty((max(n, 1), 4), np.float32) if rows else None
+        nrm = np.empty((max(n, 1), 4), np.float32) if normal_rows else None
+        m = C.c_size_t()
+        _check(lib().pclb200_correspondences_sharded(
+            self.ctx.h, self.h, None if src_index is None else src_index.h, b.ptr, b.rows, b.stride, ib.ptr, ib.rows,
+            int(is_dense), float(max_distance), tn.ptr, tn.stride, C.c_void_p(out.ctypes.data),
+            None if xyz is None else C.c_void_p(xyz.ctypes.data), None if nrm is None else C.c_void_p(nrm.ctypes.data),
+            C.byref(m)))
+        corr = out[:m.value]
+        if not (rows or normal_rows):
+            return corr
+        return corr, None if xyz is None else xyz[:m.value], None if nrm is None else nrm[:m.value]
+
+    def correspondences_normals_sharded(self, kind, src, src_normals, tgt_normals=None, k=10,
+                                        max_distance=np.sqrt(np.finfo(np.float64).max), indices=None, rows=False,
+                                        normal_rows=False):
+        """Collective correspondences_normals over a map sharded across the communicator's ranks (this index = this
+        rank's tile, built with ids=...; tgt_normals: one per record of the tile; every rank passes the same source).
+        Returns the list, or (list, xyz1 rows, normal rows) as correspondences_sharded does."""
+        b, sn, tn, ib = _Buf(src), _Buf(src_normals), _Buf(tgt_normals), _Buf(indices, np.int32)
+        n = ib.rows if indices is not None else b.rows
+        out = np.empty(max(n, 1), dtype=CORR_DTYPE)
+        xyz = np.empty((max(n, 1), 4), np.float32) if rows else None
+        nrm = np.empty((max(n, 1), 4), np.float32) if normal_rows else None
+        m = C.c_size_t()
+        _check(lib().pclb200_correspondences_normals_sharded(
+            self.ctx.h, self.h, int(kind), b.ptr, b.rows, b.stride, sn.ptr, sn.stride, tn.ptr, tn.stride, ib.ptr, ib.rows,
+            int(k), float(max_distance), C.c_void_p(out.ctypes.data), None if xyz is None else C.c_void_p(xyz.ctypes.data),
+            None if nrm is None else C.c_void_p(nrm.ctypes.data), C.byref(m)))
+        corr = out[:m.value]
+        if not (rows or normal_rows):
+            return corr
+        return corr, None if xyz is None else xyz[:m.value], None if nrm is None else nrm[:m.value]
+
+    def validate_transformation_sharded(self, src, T, max_range=np.finfo(np.float64).max, scalar_is_double=False):
+        """Collective validate_transformation over a map sharded across the communicator's ranks (this index = this
+        rank's tile; every rank passes the same source): the same value on every rank."""
+        b = _Buf(src)
+        T = np.ascontiguousarray(T, dtype=np.float64)
+        out = C.c_double()
+        _check(lib().pclb200_validate_transformation_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride,
+                                                             T.ctypes.data_as(C.POINTER(C.c_double)),
+                                                             int(scalar_is_double), float(max_range), C.byref(out)))
+        return float(out.value)
+
+    def inliers_sharded(self, src, T, inlier_threshold, rows=False):
+        """Collective pclb200_inliers over a map sharded across the communicator's ranks: the inlier correspondence list
+        (and, with rows, the matched map points as {x, y, z, 1} rows), the same on every rank."""
+        b = _Buf(src)
+        T = np.ascontiguousarray(T, dtype=np.float64)
+        out = np.empty(max(b.rows, 1), dtype=CORR_DTYPE)
+        xyz = np.empty((max(b.rows, 1), 4), np.float32) if rows else None
+        m = C.c_size_t()
+        _check(lib().pclb200_inliers_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride,
+                                             T.ctypes.data_as(C.POINTER(C.c_double)), float(inlier_threshold),
+                                             C.c_void_p(out.ctypes.data), None if xyz is None else C.c_void_p(xyz.ctypes.data),
+                                             C.byref(m)))
+        return (out[:m.value], xyz[:m.value]) if rows else out[:m.value]
 
     def normals_knn(self, cloud, k, viewpoint=(0, 0, 0), indices=None, is_dense=True, out=None):
         b = _Buf(cloud)

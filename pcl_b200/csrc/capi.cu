@@ -32,8 +32,18 @@ size_t correspondences(Ctx& c, const Index& tgt, const Index* src_index, const v
                        const double* pre_T = nullptr, int pre_mode = kApplyIcp, const float* gate_override = nullptr);
 double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t stride, const int32_t* indices,
                      size_t n_idx, const double* T, int scalar_is_double, double max_range, int mode_override = -1);
-double fitness_score_sharded(Ctx& c, const Index& tile, const void* src, size_t n, size_t stride, const int32_t* indices,
-                             size_t n_idx, const double* T, int scalar_is_double, double max_range);
+double fitness_score_sharded(Ctx& c, const Index* tile, const void* src, size_t n, size_t stride, const int32_t* indices,
+                             size_t n_idx, const double* T, int scalar_is_double, double max_range, int mode_override = -1,
+                             const char* fault = nullptr);
+size_t correspondences_normals_sharded(Ctx& c, const Index* tile, int kind, const void* src, size_t n, size_t stride,
+                                       const void* src_normals, size_t stride_sn, const void* tgt_normals,
+                                       size_t stride_tn, const int32_t* indices, size_t n_idx, int k, double max_dist,
+                                       pclb200_corr* out, float* out_xyz1, float* out_normals, const char* fault);
+size_t correspondences_sharded(Ctx& c, const Index* tile, const Index* src_index, const void* src, size_t n, size_t stride,
+                               const int32_t* indices, size_t n_idx, double max_dist, const void* tgt_normals,
+                               size_t stride_tn, pclb200_corr* out, float* out_xyz1, float* out_normals, const char* fault,
+                               const double* pre_T = nullptr, int pre_mode = kApplyIcp,
+                               const float* gate_override = nullptr);
 void gicp_covariances(Ctx& c, Index& idx, const void* pts, size_t n, size_t stride, int k, double gicp_epsilon,
                       double* out);
 // shard_filter.cu
@@ -750,8 +760,91 @@ int pclb200_fitness_score_sharded(pclb200_ctx* ctx, const pclb200_index* idx_til
 {
   (void)is_dense;
   return on_ctx(ctx, [&](Ctx& c) {
-    PCLB_REQUIRE(idx_tile && idx_tile->idx && T && score, PCLB200_ERR_INVALID, "NULL argument");
-    *score = fitness_score_sharded(c, *idx_tile->idx, src, n, stride, src_indices, n_idx, T, scalar_is_double, max_range);
+    const char* fault = idx_tile && idx_tile->idx && T && score && (src || !n) ? nullptr
+                                                                              : "fitness_score_sharded: NULL argument";
+    const double v = fitness_score_sharded(c, idx_tile ? idx_tile->idx : nullptr, src, n, stride, src_indices, n_idx, T,
+                                           scalar_is_double, max_range, -1, fault);
+    *score = v;
+  });
+}
+
+// The collective calls below refuse on every rank when any rank refuses its arguments: a fault found here travels with the
+// first exchange (require_same_count in icp.cu) instead of returning before it.
+int pclb200_validate_transformation_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* src, size_t n,
+                                            size_t stride, const double T[16], int scalar_is_double, double max_range,
+                                            double* score)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const char* fault = idx_tile && idx_tile->idx && T && score && (src || !n)
+                            ? nullptr
+                            : "validate_transformation_sharded: NULL argument";
+    const double v = fitness_score_sharded(c, idx_tile ? idx_tile->idx : nullptr, src, n, stride, nullptr, 0, T, scalar_is_double, max_range,
+                                           scalar_is_double ? kApplyValidationDouble : kApplyIcp, fault);
+    *score = v;
+  });
+}
+
+int pclb200_correspondences_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const pclb200_index* idx_src,
+                                    const void* src, size_t n, size_t stride, const int32_t* src_indices, size_t n_idx,
+                                    int is_dense, double max_dist, const void* tgt_normals, size_t stride_tn,
+                                    pclb200_corr* out, float* out_xyz1, float* out_normals, size_t* n_out)
+{
+  (void)is_dense;  // non-finite source points never produce a correspondence on either setting
+  return on_ctx(ctx, [&](Ctx& c) {
+    const size_t nq = src_indices ? n_idx : n;
+    const char* fault = nullptr;
+    if (!idx_tile || !idx_tile->idx || !n_out || (nq && (!src || !out)) || (idx_src && !idx_src->idx))
+      fault = "correspondences_sharded: NULL argument";
+    const size_t m = correspondences_sharded(c, idx_tile ? idx_tile->idx : nullptr, idx_src ? idx_src->idx : nullptr, src, n, stride,
+                                             src_indices, n_idx, max_dist, tgt_normals, stride_tn, out, out_xyz1,
+                                             out_normals, fault);
+    *n_out = m;
+  });
+}
+
+int pclb200_correspondences_normals_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, int kind, const void* src,
+                                            size_t n, size_t stride, const void* src_normals, size_t stride_sn,
+                                            const void* tgt_normals, size_t stride_tn, const int32_t* src_indices,
+                                            size_t n_idx, int k, double max_dist, pclb200_corr* out, float* out_xyz1,
+                                            float* out_normals, size_t* n_out)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const size_t nq = src_indices ? n_idx : n;
+    const char* fault = nullptr;
+    if (!idx_tile || !idx_tile->idx || !n_out || (nq && k && (!src || !out)))
+      fault = "correspondences_normals_sharded: NULL argument";
+    else if (kind != PCLB200_CORR_NORMAL_SHOOTING && kind != PCLB200_CORR_BACK_PROJECTION)
+      fault = "correspondences_normals_sharded: kind must be PCLB200_CORR_NORMAL_SHOOTING or PCLB200_CORR_BACK_PROJECTION";
+    else if (k < 0)
+      fault = "correspondences_normals_sharded: k < 0";
+    else if (nq && k && !src_normals)
+      fault = "correspondences_normals_sharded: source normals are required";
+    else if (nq && k && kind == PCLB200_CORR_BACK_PROJECTION && !tgt_normals)
+      fault = "correspondences_normals_sharded: back projection needs target normals";
+    else if (out_normals && !tgt_normals)
+      fault = "correspondences_normals_sharded: out_normals needs tgt_normals";
+    const size_t m = correspondences_normals_sharded(c, idx_tile ? idx_tile->idx : nullptr, kind, src, n, stride,
+                                                     src_normals, stride_sn, tgt_normals, stride_tn, src_indices, n_idx,
+                                                     k, max_dist, out, out_xyz1, out_normals, fault);
+    *n_out = m;
+  });
+}
+
+int pclb200_inliers_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* src, size_t n, size_t stride,
+                            const double T[16], float inlier_threshold, pclb200_corr* out, float* out_xyz1,
+                            size_t* n_out)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const char* fault =
+        idx_tile && idx_tile->idx && T && out && n_out && (src || !n) ? nullptr : "inliers_sharded: NULL argument";
+    // pclb200_inliers: transformPointCloud (float), then d2 < inlier_threshold^2 (strict); no point passes a threshold of 0
+    // on any rank, but every rank still takes part in the exchange
+    const float max_range = inlier_threshold * inlier_threshold;
+    const float gate = max_range > 0.f ? std::nextafter(max_range, -std::numeric_limits<float>::infinity()) : -1.f;
+    const size_t m = correspondences_sharded(c, idx_tile ? idx_tile->idx : nullptr, nullptr, src, n, stride, nullptr, 0,
+                                             0.0, nullptr, 0, out,
+                                             out_xyz1, nullptr, fault, T, kApplyTransformsFloat, &gate);
+    *n_out = m;
   });
 }
 

@@ -18,6 +18,24 @@
 
 namespace pclb200 {
 
+// The score of one candidate, the per-candidate arithmetic of both loops below (and of their form on a sharded map,
+// shard_target_kernels.cuh).  Normal shooting: pt = target - source in float (:106-108), then the squared norm of its
+// cross product with the source normal in double (:110-116).  Back projection: d2 (2 - cos^2) in float (:99-108).
+__device__ __forceinline__ double shooting_score(const float4 q, float px, float py, float pz, double Nx, double Ny,
+                                                 double Nz)
+{
+  const double Vx = (double)__fsub_rn(q.x, px), Vy = (double)__fsub_rn(q.y, py), Vz = (double)__fsub_rn(q.z, pz);
+  const double Cx = __dsub_rn(__dmul_rn(Ny, Vz), __dmul_rn(Nz, Vy));
+  const double Cy = __dsub_rn(__dmul_rn(Nz, Vx), __dmul_rn(Nx, Vz));
+  const double Cz = __dsub_rn(__dmul_rn(Nx, Vy), __dmul_rn(Ny, Vx));
+  return __dadd_rn(__dadd_rn(__dmul_rn(Cx, Cx), __dmul_rn(Cy, Cy)), __dmul_rn(Cz, Cz));
+}
+__device__ __forceinline__ float backprojection_score(float d2, float nx, float ny, float nz, const float4 m)
+{
+  const float cos_angle = __fadd_rn(__fadd_rn(__fmul_rn(nx, m.x), __fmul_rn(ny, m.y)), __fmul_rn(nz, m.z));
+  return __fmul_rn(d2, __fsub_rn(2.0f, __fmul_rn(cos_angle, cos_angle)));
+}
+
 // Returns the column of the chosen candidate, or -1 when the gate rejects the point.
 //   row_idx / row_d2 : this query's k candidates (k >= 1, all valid)
 //   (px,py,pz), (nx,ny,nz) : source point and its normal
@@ -39,12 +57,7 @@ __device__ __forceinline__ int select_by_normals(int kind, int k, const int32_t*
       if (oi < 0)
         break;
       const float4 q = ldg4(tgt_pts + pos_of_orig[oi]);
-      // pt = target - source in float (:106-108), then the cross product and its squared norm in double (:110-116)
-      const double Vx = (double)__fsub_rn(q.x, px), Vy = (double)__fsub_rn(q.y, py), Vz = (double)__fsub_rn(q.z, pz);
-      const double Cx = __dsub_rn(__dmul_rn(Ny, Vz), __dmul_rn(Nz, Vy));
-      const double Cy = __dsub_rn(__dmul_rn(Nz, Vx), __dmul_rn(Nx, Vz));
-      const double Cz = __dsub_rn(__dmul_rn(Nx, Vy), __dmul_rn(Ny, Vx));
-      const double dist = __dadd_rn(__dadd_rn(__dmul_rn(Cx, Cx), __dmul_rn(Cy, Cy)), __dmul_rn(Cz, Cz));
+      const double dist = shooting_score(q, px, py, pz, Nx, Ny, Nz);
       if (dist < min_dist) {
         min_dist = dist;
         min_j = j;
@@ -60,8 +73,7 @@ __device__ __forceinline__ int select_by_normals(int kind, int k, const int32_t*
       if (oi < 0)
         break;
       const float4 m = ldg4(tgt_nrm + (NRM_BY_POS ? pos_of_orig[oi] : oi));
-      const float cos_angle = __fadd_rn(__fadd_rn(__fmul_rn(nx, m.x), __fmul_rn(ny, m.y)), __fmul_rn(nz, m.z));
-      const float dist = __fmul_rn(row_d2[j], __fsub_rn(2.0f, __fmul_rn(cos_angle, cos_angle)));
+      const float dist = backprojection_score(row_d2[j], nx, ny, nz, m);
       if (dist < min_dist) {
         min_dist = dist;
         min_j = j;

@@ -475,25 +475,27 @@ __global__ void k_permute_normals_by_slot(const float4* __restrict__ nrm_rec, co
   out[j] = slot < 0 ? make_float4(qn, qn, qn, 0.f) : nrm_rec[slot];
 }
 
-// the target normals (one per record of the cloud idx was built from) in the Morton order of idx
+// the normals (one per record of the cloud idx was built from) in the Morton order of idx
+static void normals_by_pos(Ctx& c, const Index* idx, const void* normals, size_t stride_n, DevBuf<float4>& out)
+{
+  DevBuf<float4> dense;
+  dense.alloc(idx->n_cloud, c.stream);
+  load_vec3_as_float4(c, normals, idx->n_cloud, stride_n, dense.p, c.stream);
+  out.alloc(idx->pts.n, c.stream);
+  if (idx->labelled)
+    k_permute_normals_by_slot<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->slot_of_pos.p, idx->pts.n,
+                                                                              out.p);
+  else
+    k_permute_normals<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->pts.p, idx->pts.n, out.p);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
 static void stage_target_normals(Icp& s, const Index* idx, const void* tgt_normals, size_t stride_n)
 {
-  Ctx& c = *s.ctx;
   s.tgt_normals.release();
-  if (tgt_normals) {
-    DevBuf<float4> dense;
-    dense.alloc(idx->n_cloud, c.stream);
-    load_vec3_as_float4(c, tgt_normals, idx->n_cloud, stride_n, dense.p, c.stream);
-    s.tgt_normals.alloc(idx->pts.n, c.stream);
-    if (idx->labelled)
-      k_permute_normals_by_slot<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->slot_of_pos.p, idx->pts.n,
-                                                                                s.tgt_normals.p);
-    else
-      k_permute_normals<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->pts.p, idx->pts.n,
-                                                                        s.tgt_normals.p);
-    ++c.launches;
-    PCLB_CUDA(cudaGetLastError());
-  }
+  if (tgt_normals)
+    normals_by_pos(*s.ctx, idx, tgt_normals, stride_n, s.tgt_normals);
 }
 
 void icp_set_target(Icp& s, const Index* idx, const void* tgt_normals, size_t stride_n)
@@ -546,17 +548,21 @@ static void union_frame(Ctx& c, const Index& tile, Index& frame)
     frame.morton_scale = 1.f;
 }
 
-// Collective: one u64 minimum over (n, ~n) gives the smallest and the largest n of all ranks
-static void require_same_count(Ctx& c, unsigned long long n, const char* msg)
+// Collective: one u64 minimum over (n, ~n, verdict) gives the smallest and the largest n of all ranks and whether every
+// rank accepted its own arguments (fault: this rank's reason to refuse, or null), so that a refusal happens on every rank
+// and no rank is left waiting in an exchange the others never enter
+static void require_same_count(Ctx& c, unsigned long long n, const char* msg, const char* fault = nullptr)
 {
   cudaStream_t st = c.stream;
-  unsigned long long h[2] = {n, ~n};
+  unsigned long long h[3] = {n, ~n, fault ? 0ull : 1ull};
   DevBuf<unsigned long long> d;
-  d.alloc(2, st);
+  d.alloc(3, st);
   PCLB_CUDA(cudaMemcpyAsync(d.p, h, sizeof(h), cudaMemcpyHostToDevice, st));
-  comm_allreduce_u64(c, d.p, d.p, 2, kU64Min);
+  comm_allreduce_u64(c, d.p, d.p, 3, kU64Min);
   PCLB_CUDA(cudaMemcpyAsync(h, d.p, sizeof(h), cudaMemcpyDeviceToHost, st));
   check_device_error(c);
+  PCLB_REQUIRE(!fault, PCLB200_ERR_INVALID, fault);
+  PCLB_REQUIRE(h[2], PCLB200_ERR_INVALID, "another rank refused its arguments");
   PCLB_REQUIRE(h[0] == ~h[1], PCLB200_ERR_INVALID, msg);
 }
 
@@ -597,17 +603,26 @@ static void check_sharded_target(Icp& s)
   }
 }
 
-// The tile's matches of this iteration -> the whole map's, on every rank (shard_target_kernels.cuh).  Peer path: publish,
-// barrier, gather from every rank's arrays, barrier (no rank overwrites its arrays while a peer may still read them).
-// NCCL path: publish, min of the keys, non-winners' records zeroed, max of the records' bit patterns, gather.
-static void exchange_shard_matches(Icp& s, bool with_normals)
+// words of the tables of exchange_shard_records: the keys, rounded up so that the records are 16-byte aligned, then the
+// point records and the normal records
+static size_t shard_record_words(size_t n, bool with_normals)
 {
-  Ctx& c = *s.ctx;
+  return ((n + 1) & ~(size_t)1) + 2 * n * (with_normals ? 2 : 1);
+}
+
+// The tile's matches match[0..n) (by query) -> the whole map's, on every rank (shard_target_kernels.cuh): gmatch, and the
+// winners' records in gpts / gnrm.  t has shard_record_words(n, tile_nrm != null) words.  Peer path: publish, barrier,
+// gather from every rank's arrays, barrier (no rank overwrites its arrays while a peer may still read them).  NCCL path:
+// publish, min of the keys, non-winners' records zeroed, max of the records' bit patterns, gather.  ctrl (nullable): a
+// finished loop turns the kernels into no-ops.  The ICP session's loop and correspondences_sharded share it.
+static void exchange_shard_records(Ctx& c, const PeerTables& t, const Match* match, size_t n, const float4* tile_pts,
+                                   const float4* tile_nrm, const LoopCtrl* ctrl, Match* gmatch, float4* gpts,
+                                   float4* gnrm)
+{
   cudaStream_t st = c.stream;
-  const size_t n = s.n_q;
-  const size_t kw = (n + 1) & ~(size_t)1;  // key words, rounded up so that the records are 16-byte aligned
-  const size_t words = kw + 2 * n * (with_normals ? 2 : 1);
-  const PeerTables t = comm_peer_tables(c, s.shard_tab, words);
+  const bool with_normals = tile_nrm != nullptr;
+  const size_t kw = (n + 1) & ~(size_t)1;
+  const size_t words = shard_record_words(n, with_normals);
   auto records = [&](unsigned long long* base) {
     ShardRecords r;
     r.key = base;
@@ -625,8 +640,7 @@ static void exchange_shard_matches(Icp& s, bool with_normals)
     rs.nrm[r] = with_normals ? rs.pts[r] + n : nullptr;
   }
   if (n) {
-    k_shard_publish<<<grid_for(n, 256), 256, 0, st>>>(s.match.p, n, s.tgt->pts.p, with_normals ? s.tgt_normals.p : nullptr,
-                                                      s.ctrl.p, mine);
+    k_shard_publish<<<grid_for(n, 256), 256, 0, st>>>(match, n, tile_pts, tile_nrm, ctrl, mine);
     ++c.launches;
   }
   if (t.peer)
@@ -635,18 +649,27 @@ static void exchange_shard_matches(Icp& s, bool with_normals)
     const ShardRecords all = records(t.recv);
     comm_allreduce_u64(c, mine.key, all.key, n, kU64Min);
     if (n) {
-      k_shard_keep_winners<<<grid_for(n, 256), 256, 0, st>>>(all.key, n, s.ctrl.p, mine);
+      k_shard_keep_winners<<<grid_for(n, 256), 256, 0, st>>>(all.key, n, ctrl, mine);
       ++c.launches;
     }
     comm_allreduce_u32_max(c, reinterpret_cast<const unsigned*>(mine.pts), reinterpret_cast<unsigned*>(all.pts),
                            (words - kw) * 2);
   }
   if (n) {
-    k_shard_gather<<<grid_for(n, 256), 256, 0, st>>>(rs, n, s.ctrl.p, s.gmatch.p, s.gpts.p, with_normals ? s.gnrm.p : nullptr);
+    k_shard_gather<<<grid_for(n, 256), 256, 0, st>>>(rs, n, ctrl, gmatch, gpts, with_normals ? gnrm : nullptr);
     ++c.launches;
   }
   comm_tables_release(c, t);
   PCLB_CUDA(cudaGetLastError());
+}
+
+// The session's matches of this iteration -> the whole map's, through its own table (shard_tab)
+static void exchange_shard_matches(Icp& s, bool with_normals)
+{
+  Ctx& c = *s.ctx;
+  const PeerTables t = comm_peer_tables(c, s.shard_tab, shard_record_words(s.n_q, with_normals));
+  exchange_shard_records(c, t, s.match.p, s.n_q, s.tgt->pts.p, with_normals ? s.tgt_normals.p : nullptr, s.ctrl.p,
+                         s.gmatch.p, s.gpts.p, s.gnrm.p);
 }
 
 __global__ void k_cur_labels(const float4* __restrict__ cur, const int32_t* __restrict__ src_orig, size_t n,
@@ -1303,28 +1326,32 @@ double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t
 // Collective getFitnessScore over a map sharded across ranks (every rank passes its tile and the same source): the
 // tile's nearest key of every query by slot, the minimum over the ranks (the peer-mapped tables after a barrier, or an
 // NCCL min reduction), then fitness_score's count and sum over the winners in slot order — the same value on every rank.
-double fitness_score_sharded(Ctx& c, const Index& tile, const void* src, size_t n, size_t stride, const int32_t* indices,
-                             size_t n_idx, const double* T, int scalar_is_double, double max_range)
+// mode_override as in fitness_score (validateTransformation's order); fault: this rank's refusal (require_same_count).
+double fitness_score_sharded(Ctx& c, const Index* tile, const void* src, size_t n, size_t stride, const int32_t* indices,
+                             size_t n_idx, const double* T, int scalar_is_double, double max_range, int mode_override,
+                             const char* fault)
 {
   cudaStream_t st = c.stream;
   PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
                "fitness_score_sharded needs an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
-  PCLB_REQUIRE(tile.labelled, PCLB200_ERR_INVALID,
-               "fitness_score_sharded: every rank's tile must be built with pclb200_index_build_ids");
+  if (!fault && !tile->labelled)
+    fault = "fitness_score_sharded: every rank's tile must be built with pclb200_index_build_ids";
   const bool use_sub = indices && n_idx != n;
   const size_t nq = use_sub ? n_idx : n;
-  require_same_count(c, nq, "fitness_score_sharded: every rank must pass the same source");
+  require_same_count(c, nq, "fitness_score_sharded: every rank must pass the same source", fault);
   if (!nq)
     return std::numeric_limits<double>::max();
   DevBuf<float4> dense;
   dense.alloc(nq, st);
   load_xyz_as_float4(c, src, n, stride, use_sub ? indices : nullptr, use_sub ? n_idx : 0, dense.p, st);
-  transform_on_device(c, T, scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat, dense.p, nq, nullptr);
+  const int mode = mode_override >= 0 ? mode_override : (scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat);
+  transform_on_device(c, T, mode, dense.p, nq, nullptr);
   QueryBatch qb;
-  make_query_batch(c, tile, dense.p, nq, qb);
+  make_query_batch(c, *tile, dense.p, nq, qb);
   const PeerTables t = comm_scratch_tables(c, nq);
   const unsigned grid = persistent_blocks(c, nq);
-  k_fitness_keys<<<grid, 256, 0, st>>>(tree_view(tile), qb.q.p, nq, t.local, c.d_error);
+  k_tile_keys<false><<<grid, 256, 0, st>>>(tree_view(*tile), qb.q.p, nq, std::numeric_limits<float>::infinity(), nullptr,
+                                           nullptr, 0, nullptr, t.local, nullptr, c.d_error);
   ++c.launches;
   comm_tables_publish(c, t, kU64Min);
   Reducer red;
@@ -1337,6 +1364,267 @@ double fitness_score_sharded(Ctx& c, const Index& tile, const void* src, size_t 
   PCLB_CUDA(cudaMemcpyAsync(acc, red.accum.p, sizeof(acc), cudaMemcpyDeviceToHost, st));
   check_device_error(c);
   return acc[0] > 0 ? acc[1] / acc[0] : std::numeric_limits<double>::max();
+}
+
+// the flagged rows of rows[0..n) in order (m of them) to the caller's host or device array of float4 rows
+static void compact_rows_to(Ctx& c, const float4* rows, const unsigned char* flag, size_t n, size_t m, float* out)
+{
+  cudaStream_t st = c.stream;
+  if (!m)
+    return;
+  DevBuf<float4> tmp;
+  float4* d_out = out_on_device(c, reinterpret_cast<float4*>(out), m, tmp);
+  DevBuf<int> count;
+  count.alloc(1, st);
+  size_t tmp_bytes = 0;
+  PCLB_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, rows, flag, d_out, count.p, (int)n, st));
+  DevBuf<unsigned char> scratch;
+  scratch.alloc(tmp_bytes, st);
+  PCLB_CUDA(cub::DeviceSelect::Flagged(scratch.p, tmp_bytes, rows, flag, d_out, count.p, (int)n, st));
+  c.launches += 2;
+  copy_out(c, reinterpret_cast<float4*>(out), tmp, m);
+}
+
+// a labelled tile's ids by position (padding: kSentinelIndex) and the positions, for the sort of
+// correspondences_normals_sharded
+__global__ void k_tile_ids_pos(const float4* __restrict__ pts, size_t n, unsigned* __restrict__ ids, int* __restrict__ pos)
+{
+  const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (j >= n)
+    return;
+  ids[j] = (unsigned)__float_as_int(pts[j].w);
+  pos[j] = (int)j;
+}
+
+// The record rows of a sharded list: the tile matches match[0..nq) (by slot) -> the winners' points (and normals, when
+// with_normals: tile_nrm by position) through exchange_shard_records, as k_corr_rows's rows and flags by slot.  The scratch
+// table is drawn at table_words (>= shard_record_words), the size of the call's other exchanges, so it stays mapped.
+static void records_of_matches(Ctx& c, const Index* tile, const float4* tile_nrm, bool with_normals, const Match* match,
+                               const pclb200_corr* by_slot, size_t nq, bool with_pts, size_t table_words,
+                               DevBuf<float4>& row_pts, DevBuf<float4>& row_nrm, DevBuf<unsigned char>& flag)
+{
+  cudaStream_t st = c.stream;
+  ProfScope ps(c, "shard_corr_records");
+  DevBuf<float4> gpts, gnrm;
+  DevBuf<Match> gmatch;
+  if (with_normals) {
+    gnrm.alloc(nq, st);
+    row_nrm.alloc(nq, st);
+  }
+  gmatch.alloc(nq, st);
+  gpts.alloc(nq, st);
+  exchange_shard_records(c, comm_scratch_tables(c, table_words), match, nq, tile->pts.p,
+                         with_normals ? tile_nrm : nullptr, nullptr, gmatch.p, gpts.p, gnrm.p);
+  if (with_pts)
+    row_pts.alloc(nq, st);
+  flag.alloc(nq, st);
+  k_corr_rows<<<grid_for(nq, 256), 256, 0, st>>>(by_slot, gpts.p, gnrm.p, nq, row_pts.p, row_nrm.p, flag.p);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
+// Collective correspondences() over a map sharded across ranks// Collective correspondences() over a map sharded across ranks (every rank passes its tile and the same whole source):
+// per slot this tile's key within the gate (and, reciprocal, the key again where the tile point's reverse search onto the
+// source returns the query), the minimum over the ranks through the scratch tables, then correspondences()'s list, the
+// same on every rank.  out_xyz1 / out_normals (nullable): the matched map point {x, y, z, 1} and its normal {nx, ny, nz, 0}
+// per output correspondence, moved by the record exchange of the ICP session (exchange_shard_records); tgt_normals has
+// one record per record of the tile.  pre_T / pre_mode / gate_override as in correspondences() (inliers).  fault: this
+// rank's refusal of its arguments, agreed on by every rank before any exchange (require_same_count).
+size_t correspondences_sharded(Ctx& c, const Index* tile, const Index* src_index, const void* src, size_t n, size_t stride,
+                               const int32_t* indices, size_t n_idx, double max_dist, const void* tgt_normals,
+                               size_t stride_tn, pclb200_corr* out, float* out_xyz1, float* out_normals, const char* fault,
+                               const double* pre_T, int pre_mode, const float* gate_override)
+{
+  cudaStream_t st = c.stream;
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+               "correspondences_sharded needs an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
+  if (!fault && !tile->labelled)
+    fault = "correspondences_sharded: every rank's tile must be built with pclb200_index_build_ids";
+  if (!fault && src_index && src_index->labelled)
+    fault = "correspondences_sharded: the source index of reciprocal correspondences must be built without ids";
+  if (!fault && out_normals && !tgt_normals)
+    fault = "correspondences_sharded: out_normals needs tgt_normals";
+  for (const float* o : {out_xyz1, out_normals})
+    if (!fault && o && is_device_ptr(o) && reinterpret_cast<uintptr_t>(o) % 16)
+      fault = "correspondences_sharded: device rows out_xyz1 / out_normals must be 16-byte aligned";
+  const bool recip = src_index != nullptr, rows = out_xyz1 || out_normals;
+  const size_t nq = indices ? n_idx : n;
+  // the count and the variant (reciprocal, records, normals): every rank must lay its tables out alike
+  require_same_count(c, (unsigned long long)nq << 3 | (recip ? 1 : 0) | (rows ? 2 : 0) | (out_normals ? 4 : 0),
+                     "correspondences_sharded: every rank must pass the same whole source, reciprocal or not, and ask "
+                     "for the same record rows",
+                     fault);
+  if (nq == 0)
+    return 0;
+  DevBuf<float4> dense;
+  dense.alloc(nq, st);
+  load_xyz_as_float4(c, src, n, stride, indices, n_idx, dense.p, st);
+  if (pre_T)
+    transform_on_device(c, pre_T, pre_mode, dense.p, nq, nullptr);
+  DevBuf<int32_t> staged_ind;
+  const int32_t* d_ind = on_device(c, indices, n_idx, staged_ind);
+  QueryBatch qb;
+  make_query_batch(c, *tile, dense.p, nq, qb);
+  const float gate = gate_override ? *gate_override : gate_from_max_dist(max_dist);
+  // one scratch size for the key and the record exchange keeps the table mapped across both (and across calls)
+  const size_t words = std::max(recip ? 2 * nq : nq, rows ? shard_record_words(nq, out_normals != nullptr) : 0);
+  DevBuf<Match> match;
+  if (rows)
+    match.alloc(nq, st);
+  DevBuf<pclb200_corr> by_slot;
+  by_slot.alloc(nq, st);
+  {
+    ProfScope ps(c, "shard_corr_keys");
+    PeerTables t = comm_scratch_tables(c, words);
+    t.words = recip ? 2 * nq : nq;  // the NCCL reduction moves the keys only
+    const unsigned grid = persistent_blocks(c, nq);
+    if (recip)
+      k_tile_keys<true><<<grid, 256, 0, st>>>(tree_view(*tile), qb.q.p, nq, gate, src_index->nodes.p, src_index->pts.p,
+                                              src_index->root, d_ind, t.local, match.p, c.d_error);
+    else
+      k_tile_keys<false><<<grid, 256, 0, st>>>(tree_view(*tile), qb.q.p, nq, gate, nullptr, nullptr, 0, nullptr, t.local,
+                                               match.p, c.d_error);
+    ++c.launches;
+    comm_tables_publish(c, t, kU64Min);
+    k_keys_to_corr<<<grid_for(nq, 256), 256, 0, st>>>(peer_table_set(t), nq, recip ? 1 : 0, d_ind, by_slot.p);
+    ++c.launches;
+    comm_tables_release(c, t);
+    PCLB_CUDA(cudaGetLastError());
+  }
+  DevBuf<float4> row_pts, row_nrm;
+  DevBuf<unsigned char> flag;
+  if (rows) {
+    DevBuf<float4> tile_nrm;
+    if (out_normals)
+      normals_by_pos(c, tile, tgt_normals, stride_tn, tile_nrm);
+    records_of_matches(c, tile, tile_nrm.p, out_normals != nullptr, match.p, by_slot.p, nq, out_xyz1 != nullptr, words,
+                       row_pts, row_nrm, flag);
+  }
+  const size_t m = compact_corr_to(c, by_slot.p, nq, out);
+  if (out_xyz1)
+    compact_rows_to(c, row_pts.p, flag.p, nq, m, out_xyz1);
+  if (out_normals)
+    compact_rows_to(c, row_nrm.p, flag.p, nq, m, out_normals);
+  check_device_error(c);
+  PCLB_CUDA(cudaStreamSynchronize(st));
+  return m;
+}
+
+int comm_nranks(const Ctx& c);  // comm.cu
+
+// Collective correspondences_by_normals over a map sharded across ranks (normal shooting / back projection; the layout
+// of correspondences_sharded).  keff is the whole map's clamp.  Each rank's k-NN rows of its tile, as keys, travel through
+// the segment tables (peer path: read in place; NCCL: all-gathered), every rank merges the R rows of each query into the
+// whole map's row (shard_target_kernels.cuh), scores the merged candidates its tile holds and publishes the scores'
+// bit patterns (~0 elsewhere) for one u64 minimum, and runs select_by_normals's choice on the result.  The tile's ids are
+// sorted once per call to find a candidate's position.  Resident per rank at the peak: its rows (nq keff 8 B), the other
+// ranks' rows under NCCL ((R - 1) nq keff 8 B), the merged row and the scores (2 nq keff 8 B).
+size_t correspondences_normals_sharded(Ctx& c, const Index* tile, int kind, const void* src, size_t n, size_t stride,
+                                       const void* src_normals, size_t stride_sn, const void* tgt_normals,
+                                       size_t stride_tn, const int32_t* indices, size_t n_idx, int k, double max_dist,
+                                       pclb200_corr* out, float* out_xyz1, float* out_normals, const char* fault)
+{
+  cudaStream_t st = c.stream;
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+               "correspondences_normals_sharded needs an active communicator (pclb200_comm_init or pclb200_comm_export / "
+               "_import)");
+  if (!fault && !tile->labelled)
+    fault = "correspondences_normals_sharded: every rank's tile must be built with pclb200_index_build_ids";
+  for (const float* o : {out_xyz1, out_normals})
+    if (!fault && o && is_device_ptr(o) && reinterpret_cast<uintptr_t>(o) % 16)
+      fault = "correspondences_normals_sharded: device rows out_xyz1 / out_normals must be 16-byte aligned";
+  const bool rows = out_xyz1 || out_normals;
+  const size_t nq = indices ? n_idx : n;
+  const int R = comm_nranks(c);
+  // the count, the kind, k and the rows asked for: every rank must lay its tables out alike
+  require_same_count(c, ((((unsigned long long)nq << 2 | (unsigned)kind) << 1 | (rows ? 1 : 0)) << 1 |
+                         (out_normals ? 1 : 0)) << 32 | (unsigned)k,
+                     "correspondences_normals_sharded: every rank must pass the same whole source, kind and k, and ask "
+                     "for the same record rows",
+                     fault);
+  if (nq == 0 || k == 0)
+    return 0;
+  const int keff = sharded_keff(c, *tile, k);
+  if (keff <= 0)
+    return 0;
+  const size_t nk = nq * (size_t)keff;
+  DevBuf<float4> dense, sn, tile_nrm;
+  QueryBatch qb = load_queries(c, *tile, src, n, stride, indices, n_idx, dense);
+  sn.alloc(n, st);
+  load_vec3_as_float4(c, src_normals, n, stride_sn, sn.p, st);
+  if (tgt_normals)
+    normals_by_pos(c, tile, tgt_normals, stride_tn, tile_nrm);
+  DevBuf<int32_t> staged_ind;
+  const int32_t* d_ind = on_device(c, indices, n_idx, staged_ind);
+  // the tile's ids sorted, with their positions (padding sorts last under kSentinelIndex)
+  const size_t np = tile->pts.n;
+  DevBuf<unsigned> ids_in, sid;
+  DevBuf<int> pos_in, spos;
+  ids_in.alloc(np, st);
+  pos_in.alloc(np, st);
+  sid.alloc(np, st);
+  spos.alloc(np, st);
+  k_tile_ids_pos<<<grid_for(np, 256), 256, 0, st>>>(tile->pts.p, np, ids_in.p, pos_in.p);
+  ++c.launches;
+  {
+    size_t tb = 0;
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, ids_in.p, sid.p, pos_in.p, spos.p, (int)np, 0, 32, st));
+    DevBuf<unsigned char> tmp;
+    tmp.alloc(tb, st);
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, ids_in.p, sid.p, pos_in.p, spos.p, (int)np, 0, 32, st));
+    c.launches += 2;
+  }
+  DevBuf<unsigned long long> merged;
+  merged.alloc(nk, st);
+  {
+    ProfScope ps(c, "shard_corr_knn");
+    DevBuf<int32_t> nn_idx;
+    DevBuf<float> nn_d2;
+    nn_idx.alloc(nk, st);
+    nn_d2.alloc(nk, st);
+    launch_knn(c, *tile, qb.q.p, nq, keff, std::numeric_limits<float>::infinity(), nn_idx.p, nn_d2.p);
+    std::vector<unsigned long long> cnt(R, (unsigned long long)nk);
+    const PeerTables t = comm_segment_tables(c, cnt.data(), sizeof(unsigned long long));
+    k_knn_keys<<<persistent_blocks(c, nk), 256, 0, st>>>(nn_idx.p, nn_d2.p, nk, t.local);
+    ++c.launches;
+    comm_tables_publish(c, t, kU64Sum);  // NCCL: the tables lie end to end in one zeroed table, one writer per word
+    k_merge_rows<<<grid_for(nq, 256), 256, 0, st>>>(peer_table_set(t), nq, keff, merged.p);
+    ++c.launches;
+    comm_tables_release(c, t);
+    PCLB_CUDA(cudaGetLastError());
+  }
+  DevBuf<pclb200_corr> by_slot;
+  by_slot.alloc(nq, st);
+  DevBuf<Match> match;
+  if (rows)
+    match.alloc(nq, st);
+  {
+    ProfScope ps(c, "shard_corr_select");
+    PeerTables t = comm_scratch_tables(c, rows ? std::max(nk, shard_record_words(nq, out_normals != nullptr)) : nk);
+    t.words = nk;
+    k_candidate_scores<<<grid_for(nq, 256), 256, 0, st>>>(merged.p, nq, keff, kind, dense.p, d_ind, sn.p, sid.p, spos.p,
+                                                           np, tile->pts.p, tile_nrm.p, t.local);
+    ++c.launches;
+    comm_tables_publish(c, t, kU64Min);
+    k_select_sharded<<<grid_for(nq, 256), 256, 0, st>>>(merged.p, peer_table_set(t), nq, keff, kind, dense.p, d_ind,
+                                                         max_dist, sid.p, spos.p, np, by_slot.p, match.p);
+    ++c.launches;
+    comm_tables_release(c, t);
+    PCLB_CUDA(cudaGetLastError());
+  }
+  DevBuf<float4> row_pts, row_nrm;
+  DevBuf<unsigned char> flag;
+  if (rows)
+    records_of_matches(c, tile, tile_nrm.p, out_normals != nullptr, match.p, by_slot.p, nq, out_xyz1 != nullptr,
+                       std::max(nk, shard_record_words(nq, out_normals != nullptr)), row_pts, row_nrm, flag);
+  const size_t m = compact_corr_to(c, by_slot.p, nq, out);
+  if (out_xyz1)
+    compact_rows_to(c, row_pts.p, flag.p, nq, m, out_xyz1);
+  if (out_normals)
+    compact_rows_to(c, row_nrm.p, flag.p, nq, m, out_normals);
+  check_device_error(c);
+  PCLB_CUDA(cudaStreamSynchronize(st));
+  return m;
 }
 
 }  // namespace pclb200

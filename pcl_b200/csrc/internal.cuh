@@ -369,6 +369,9 @@ void cluster_labels(Ctx& c, const Index& idx, double tolerance, int32_t* d_label
 // the same over a map sharded across the communicator's ranks (collective, shard_cluster.cu): labels and, when d_sizes is
 // not null, component sizes of the tile's records (tile.n_cloud entries each, on the device)
 void cluster_labels_sharded(Ctx& c, const Index& tile, double tolerance, int32_t* d_labels, int64_t* d_sizes);
+// min(k, the number of distinct finite ids of a map sharded across the communicator's ranks), the same on every rank
+// (collective, shard_filter.cu: the clamp of pclb200_knn_sharded)
+int sharded_keff(Ctx& c, const Index& tile, int k);
 // every rank's d_send[0..n) concatenated in rank order, identically on every rank (collective, comm.cu: the count
 // exchange, then comm_segment_tables); returns the total
 size_t allgather_u64(Ctx& c, const unsigned long long* d_send, size_t n, DevBuf<unsigned long long>& out);

@@ -80,7 +80,13 @@ int knn_sharded(Ctx& c, const Index& tile, const void* queries, size_t nq, size_
     }
   }
   fm.local.reset();
-  // k_eff: the whole map's clamp (kdtree_flann.hpp:241-242), the same on every rank
+  return sharded_keff(c, tile, k);
+}
+
+// k_eff: the whole map's clamp (kdtree_flann.hpp:241-242), the same on every rank (collective)
+int sharded_keff(Ctx& c, const Index& tile, int k)
+{
+  cudaStream_t st = c.stream;
   DevBuf<unsigned long long> w;
   w.alloc(1, st);
   const unsigned long long not_n = ~(unsigned long long)tile.n_valid;
