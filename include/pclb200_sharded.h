@@ -26,7 +26,8 @@ extern "C" {
  * pclb200_knn_stats_sharded, pclb200_statistical_outlier_sharded and pclb200_radius_outlier_sharded, its VoxelGrid from
  * pclb200_voxelgrid_sharded, its nearest and reciprocal correspondences, validation and inliers from
  * pclb200_correspondences_sharded, pclb200_correspondences_normals_sharded, pclb200_validate_transformation_sharded
- * and pclb200_inliers_sharded. */
+ * and pclb200_inliers_sharded, its radius neighbourhoods from pclb200_radius_sharded and pclb200_radius_into_sharded,
+ * and its GICP covariances from pclb200_gicp_covariances_sharded. */
 PCLB200_API int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                         const int32_t* ids, pclb200_index** out);
 
@@ -169,6 +170,47 @@ PCLB200_API int pclb200_statistical_outlier_sharded(pclb200_ctx* ctx, const pclb
 PCLB200_API int pclb200_radius_outlier_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts,
                                                size_t n, size_t stride, const int32_t* indices, size_t n_idx,
                                                int is_dense, double radius, int min_pts, int negative, uint8_t* keep);
+
+/* Radius search and GICP covariances of a map sharded across the ranks of the context's communicator.  Collective: every
+ * rank passes its tile (built with pclb200_index_build_ids; the map is the union of the ids, an id held by two ranks names
+ * the same point and counts once).  "One index of the whole map" is pclb200_index_build over the map with subset = the
+ * union of the ids in ascending order.  Arrays may be host or device memory, as for the single-index calls.
+ *
+ * pclb200_radius_sharded / pclb200_radius_into_sharded: every rank passes its OWN queries (any points; a rank may pass
+ * none), and its own radius and max_nn (they serve only its queries; the ranks need not agree).  Each query's row of
+ * out_offsets / out_idx / out_d2 is, byte for byte, what pclb200_radius / pclb200_radius_into return for it on one index
+ * of the whole map: the ids, the d2, the (d2, id) order, strict d2 < float(radius * radius), max_nn keeping the nearest,
+ * empty rows for non-finite queries.  A radius of 0 or NaN gives empty lists, a radius whose square overflows the whole
+ * map.  A rank with nq == 0 takes part in every exchange and gets out_offsets[0] = 0 (and, from pclb200_radius_sharded,
+ * *out_idx = *out_d2 = NULL).  pclb200_radius_sharded takes host out_offsets and allocates the lists (pclb200_free).
+ * pclb200_radius_into_sharded keeps pclb200_radius_into's rule on each rank: when *total > capacity only out_offsets and
+ * *total are written, else the lists too.  Once every rank has counted, one u64 minimum sets *all_fit (nullable; the
+ * exchange runs either way) to the same value on every rank: 1 exactly when every rank's lists fit.  So every rank runs the
+ * same loop, while (!all_fit) { grow to *total; call again }, and a rank whose lists already fit may pass the same
+ * buffers again and gets the same bytes.  Each call rebuilds the halo.  A rank's lists share pclb200_radius's limit of
+ * 2^31 neighbours (max_nn <= 32 materialises only the kept ones).
+ * Each rank fetches, from the other ranks' tiles, every point within the radius of its queries' box, and indexes its tile
+ * plus those points: both are resident at the peak, and on a random partition the halo is nearly the whole map.
+ *
+ * pclb200_gicp_covariances_sharded: pts, n, stride are the records the tile was built from (n = its record count).
+ * Row i of out_cov (9 doubles) is, byte for byte, row ids[i] of pclb200_gicp_covariances on one index of the whole map
+ * called with the whole map's array: zero rows for non-finite records, k clamped to the whole map's distinct finite ids,
+ * the division by k.  Each rank fetches the points within its records' k-th nearest distance in its tile, as
+ * pclb200_knn_sharded does.
+ *
+ * PCLB200_ERR_INVALID on every rank, before any halo moves, when any rank has no active communicator, a NULL or
+ * unlabelled tile, a NULL argument where one is not allowed, device out_offsets given to pclb200_radius_sharded,
+ * capacity > 0 with NULL output buffers, k < 1, or (covariances) n other than its tile's record count.  Each rank's
+ * verdict on its own arguments travels in one u64 minimum. */
+PCLB200_API int pclb200_radius_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* queries, size_t nq,
+                                       size_t stride, double radius, unsigned max_nn, int sorted,
+                                       int64_t* out_offsets, int32_t** out_idx, float** out_d2);
+PCLB200_API int pclb200_radius_into_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* queries,
+                                            size_t nq, size_t stride, double radius, unsigned max_nn,
+                                            int64_t* out_offsets, int32_t* out_idx, float* out_d2, size_t capacity,
+                                            size_t* total, int* all_fit /*nullable*/);
+PCLB200_API int pclb200_gicp_covariances_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts,
+                                                 size_t n, size_t stride, int k, double gicp_epsilon, double* out_cov);
 
 /* Euclidean clustering of a map sharded across the ranks of the context's communicator (collective: every rank passes its
  * tile, built with pclb200_index_build_ids; the whole map is the union of the tiles' ids).  n_labels is the number of

@@ -83,7 +83,8 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_comm_allgather_u64", "pclb200_knn_sharded", "pclb200_knn_stats_sharded",
                    "pclb200_statistical_outlier_sharded", "pclb200_radius_outlier_sharded", "pclb200_voxelgrid_sharded",
                    "pclb200_correspondences_sharded", "pclb200_correspondences_normals_sharded",
-                   "pclb200_validate_transformation_sharded", "pclb200_inliers_sharded"]
+                   "pclb200_validate_transformation_sharded", "pclb200_inliers_sharded", "pclb200_radius_sharded",
+                   "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
 
 _lib = None
 
@@ -170,6 +171,9 @@ def lib():
     L.pclb200_inliers_sharded.argtypes = [vp, vp, vp, sz, sz, dp, C.c_float, vp, vp, C.POINTER(sz)]
     L.pclb200_gicp_covariances.argtypes = [vp, vp, vp, sz, sz, C.c_int, C.c_double, vp]
     L.pclb200_radius_into.argtypes = [vp, vp, vp, sz, sz, C.c_double, C.c_uint, vp, vp, vp, sz, C.POINTER(sz)]
+    L.pclb200_radius_sharded.argtypes = L.pclb200_radius.argtypes
+    L.pclb200_radius_into_sharded.argtypes = L.pclb200_radius_into.argtypes + [C.POINTER(C.c_int)]
+    L.pclb200_gicp_covariances_sharded.argtypes = L.pclb200_gicp_covariances.argtypes
     L.pclb200_comm_unique_id.argtypes = [vp]
     L.pclb200_comm_set_mode.argtypes = [vp, C.c_int]
     L.pclb200_comm_export.argtypes = [vp, vp]
@@ -822,6 +826,52 @@ class Index:
                                                     int(is_dense), float(radius), int(min_pts), int(negative),
                                                     C.c_void_p(keep.ctypes.data)))
         return keep
+
+    def radius_sharded(self, q, r, max_nn=0, sorted_results=True):
+        """Collective radius over a map sharded across the communicator's ranks (this index = this rank's tile, built with
+        ids=...; q = this rank's own queries, r and max_nn its own): (offsets, ids, d2), bit for bit one index of the whole
+        map's answer."""
+        b = _Buf(q)
+        offs = np.zeros(b.rows + 1, dtype=np.int64)
+        pi, pd = C.POINTER(C.c_int32)(), C.POINTER(C.c_float)()
+        try:
+            _check(lib().pclb200_radius_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, float(r), int(max_nn),
+                                                int(sorted_results), offs.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                C.byref(pi), C.byref(pd)))
+            total = int(offs[-1])
+            idx = np.ctypeslib.as_array(pi, shape=(total,)).copy() if total else np.zeros(0, np.int32)
+            d2 = np.ctypeslib.as_array(pd, shape=(total,)).copy() if total else np.zeros(0, np.float32)
+        finally:
+            lib().pclb200_free(pi)
+            lib().pclb200_free(pd)
+        return offs, idx, d2
+
+    def radius_into_sharded(self, q, r, offsets, idx, d2, max_nn=0):
+        """Collective radius_into over a sharded map (see radius_sharded) into caller buffers (numpy or torch, host or
+        cuda): (total, all_fit).  total is this rank's number of neighbours; when it exceeds the capacity of idx / d2 only
+        `offsets` was written.  all_fit, the same on every rank, says whether every rank's lists fit: while it is False,
+        every rank grows its buffers to its total and calls again."""
+        b = _Buf(q)
+        ob, ib, db = _Buf(offsets, np.int64), _Buf(idx, np.int32), _Buf(d2)
+        total, fit = C.c_size_t(), C.c_int()
+        _check(lib().pclb200_radius_into_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, float(r), int(max_nn),
+                                                 ob.ptr, ib.ptr, db.ptr, min(ib.rows, db.rows), C.byref(total),
+                                                 C.byref(fit)))
+        return int(total.value), bool(fit.value)
+
+    def gicp_covariances_sharded(self, cloud, k=20, gicp_epsilon=0.001, out=None):
+        """Collective gicp_covariances over a sharded map (cloud = the records this tile was built from): (n, 3, 3)
+        float64, row i bit for bit row ids[i] of one index of the whole map's answer.  out: (n, 9) float64, numpy or
+        torch, host or cuda (returned as given)."""
+        b = _Buf(cloud)
+        ret = out
+        if out is None:
+            out = np.zeros((b.rows, 9), dtype=np.float64)
+            ret = out.reshape(-1, 3, 3)
+        ob = _Buf(out, np.float64)
+        _check(lib().pclb200_gicp_covariances_sharded(self.ctx.h, self.h, b.ptr, b.rows, b.stride, int(k),
+                                                      float(gicp_epsilon), ob.ptr))
+        return ret
 
 
 def clusters_from_labels(labels, min_size=1, max_size=2 ** 32 - 1):

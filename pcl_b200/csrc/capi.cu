@@ -56,6 +56,12 @@ void statistical_outlier_sharded(Ctx& c, const Index& tile, const void* pts, siz
                                  unsigned char* d_keep, double* d_stats);
 void radius_outlier_sharded(Ctx& c, const Index& tile, const void* pts, size_t n, size_t stride, const int32_t* indices,
                             size_t n_idx, int is_dense, double radius, int min_pts, int negative, unsigned char* d_keep);
+unsigned long long radius_sharded(Ctx& c, const Index* tile, const void* queries, size_t nq, size_t stride, double radius,
+                                  unsigned max_nn, int64_t* out_offsets,
+                                  const std::function<RadiusSinkBuffers(unsigned long long)>& sink, const char* fault);
+void gicp_covariances_sharded(Ctx& c, const Index* tile, const void* pts, size_t n, size_t stride, int k,
+                              double gicp_epsilon, double* out, const char* fault);
+unsigned long long ranks_min(Ctx& c, unsigned long long word);
 // voxel.cu
 size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* indices, size_t n_idx, int is_dense,
                  const float leaf[3], unsigned min_pts, float* out_xyz1, const void* normals, size_t stride_n,
@@ -1013,6 +1019,77 @@ int pclb200_radius_outlier_sharded(pclb200_ctx* ctx, const pclb200_index* idx_ti
     radius_outlier_sharded(c, *idx_tile->idx, pts, n, stride, indices, n_idx, is_dense, radius, min_pts, negative,
                            out_on_device(c, keep, nq, tk));
     copy_out(c, keep, tk, nq);
+    check_device_error(c);
+  });
+}
+
+// ---- radius search and GICP covariances on a sharded map ----------------------------------------------------------------------
+// A fault found here travels with the verdict exchange (shard_filter.cu) instead of returning before it.
+int pclb200_radius_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* queries, size_t nq, size_t stride,
+                           double radius, unsigned max_nn, int sorted, int64_t* out_offsets, int32_t** out_idx,
+                           float** out_d2)
+{
+  (void)sorted;
+  return on_ctx(ctx, [&](Ctx& c) {
+    const char* fault = nullptr;
+    if (!idx_tile || !idx_tile->idx || !out_offsets || !out_idx || !out_d2 || (nq && !queries))
+      fault = "radius_sharded: NULL argument";
+    else if (is_device_ptr(out_offsets))
+      fault = "radius_sharded returns host arrays: out_offsets must be host memory";
+    if (!fault) {
+      *out_idx = nullptr;
+      *out_d2 = nullptr;
+    }
+    radius_sharded(c, idx_tile ? idx_tile->idx : nullptr, queries, nq, stride, radius, max_nn, out_offsets,
+                   [&](unsigned long long total) {
+                     if (!nq)
+                       return RadiusSinkBuffers{nullptr, nullptr};  // as pclb200_radius: no arrays for no query
+                     int32_t* hi = static_cast<int32_t*>(malloc(std::max<size_t>(total, 1) * sizeof(int32_t)));
+                     float* hd = static_cast<float*>(malloc(std::max<size_t>(total, 1) * sizeof(float)));
+                     *out_idx = hi;  // owned by the caller from here on (pclb200_free), also on the error paths
+                     *out_d2 = hd;
+                     PCLB_REQUIRE(hi && hd, PCLB200_ERR_INTERNAL, "host allocation failed");
+                     return RadiusSinkBuffers{hi, hd};
+                   },
+                   fault);
+  });
+}
+
+int pclb200_radius_into_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* queries, size_t nq,
+                                size_t stride, double radius, unsigned max_nn, int64_t* out_offsets, int32_t* out_idx,
+                                float* out_d2, size_t capacity, size_t* total, int* all_fit)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const char* fault = nullptr;
+    if (!idx_tile || !idx_tile->idx || !out_offsets || !total || (nq && !queries))
+      fault = "radius_into_sharded: NULL argument";
+    else if (capacity > 0 && !(out_idx && out_d2))
+      fault = "radius_into_sharded: NULL output buffers with a non-zero capacity";
+    if (!fault)
+      *total = 0;
+    radius_sharded(c, idx_tile ? idx_tile->idx : nullptr, queries, nq, stride, radius, max_nn, out_offsets,
+                   [&](unsigned long long n) {
+                     *total = (size_t)n;
+                     // every rank has its count here: one u64 minimum tells all of them whether every rank's lists fit
+                     const bool fits = (size_t)n <= capacity;
+                     const int every = ranks_min(c, fits ? 1 : 0) ? 1 : 0;
+                     if (all_fit)
+                       *all_fit = every;
+                     if (!fits)
+                       return RadiusSinkBuffers{nullptr, nullptr};  // offsets and *total are valid; call again with room
+                     return RadiusSinkBuffers{out_idx, out_d2};
+                   },
+                   fault);
+  });
+}
+
+int pclb200_gicp_covariances_sharded(pclb200_ctx* ctx, const pclb200_index* idx_tile, const void* pts, size_t n,
+                                     size_t stride, int k, double gicp_epsilon, double* out_cov)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    const char* fault =
+        idx_tile && idx_tile->idx && (!n || (pts && out_cov)) ? nullptr : "gicp_covariances_sharded: NULL argument";
+    gicp_covariances_sharded(c, idx_tile ? idx_tile->idx : nullptr, pts, n, stride, k, gicp_epsilon, out_cov, fault);
     check_device_error(c);
   });
 }

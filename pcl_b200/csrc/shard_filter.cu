@@ -12,6 +12,10 @@
 //             comm_segment_tables, three words; publish; every rank folds every rank's words in rank order and applies
 //             the reference's mean / variance / threshold; release; the mask on the device.
 //   ROR       one u64 minimum of the ranks' is_dense flags picks the rule on every rank; the mask on the device.
+// Radius search (pclb200_radius_sharded, pclb200_radius_into_sharded) and GICP covariances (pclb200_gicp_covariances_sharded)
+// run the unchanged radius_search / gicp_covariances on the local map of the radius, or of k for the tile's own records
+// (DESIGN.md §5, "Radius search and GICP covariances of a sharded map").  Their refusals travel in one u64 minimum of
+// the ranks' verdicts before any halo moves.
 #include <limits>
 #include <memory>
 #include <vector>
@@ -26,6 +30,8 @@ int comm_nranks(const Ctx& c);
 int comm_rank(const Ctx& c);
 template <typename K>
 size_t sort_unique(Ctx& c, const K* keys, size_t n, DevBuf<K>& out);  // shard_cluster.cu
+void gicp_covariances(Ctx& c, Index& idx, const void* pts, size_t n, size_t stride, int k, double gicp_epsilon,
+                      double* out);  // icp.cu
 
 static const ShardedMapStages kFilterStages{"sharded_filter_bound", "sharded_filter_halo", "sharded_filter_build"};
 
@@ -81,6 +87,111 @@ int knn_sharded(Ctx& c, const Index& tile, const void* queries, size_t nq, size_
   }
   fm.local.reset();
   return sharded_keff(c, tile, k);
+}
+
+// Collective: the minimum of one word over the ranks, the same on every rank
+unsigned long long ranks_min(Ctx& c, unsigned long long word)
+{
+  cudaStream_t st = c.stream;
+  DevBuf<unsigned long long> w;
+  w.alloc(1, st);
+  PCLB_CUDA(cudaMemcpyAsync(w.p, &word, sizeof(word), cudaMemcpyHostToDevice, st));
+  comm_allreduce_u64(c, w.p, w.p, 1, kU64Min);
+  PCLB_CUDA(cudaMemcpyAsync(&word, w.p, sizeof(word), cudaMemcpyDeviceToHost, st));
+  check_device_error(c);
+  return word;
+}
+
+// Collective: every rank's verdict on its own arguments (fault: this rank's reason to refuse, or null) in one u64
+// minimum, so that a refusal happens on every rank before anything moves.  The ranks' query counts may differ, so unlike
+// the ICP session's check (icp.cu: require_same_count) no count travels with it.
+static void require_every_rank_accepts(Ctx& c, const char* fault)
+{
+  const unsigned long long all = ranks_min(c, fault ? 0 : 1);
+  PCLB_REQUIRE(!fault, PCLB200_ERR_INVALID, fault);
+  PCLB_REQUIRE(all, PCLB200_ERR_INVALID, "another rank refused its arguments");
+}
+
+// Radius search of this rank's queries on the whole map (DESIGN.md §5, "Radius search and GICP covariances of a sharded
+// map"): the local map of every point of the other tiles within r2 of the queries' box, then the unchanged radius_search
+// on it.  Its lists go to device buffers, whichever the caller's are, so that the local record numbers become ids
+// (k_sf_row_ids) before they leave the device; both paths of radius_search (sorted keys, register k-NN rows) unpack to
+// such lists.  sink(total) is called once on every rank, a rank with no query included (total 0), so that it can hold a
+// collective exchange.  Returns the total delivered (0 when the sink declined the lists).
+unsigned long long radius_sharded(Ctx& c, const Index* tile, const void* queries, size_t nq, size_t stride, double radius,
+                                  unsigned max_nn, int64_t* out_offsets,
+                                  const std::function<RadiusSinkBuffers(unsigned long long)>& sink, const char* fault)
+{
+  cudaStream_t st = c.stream;
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+               "sharded radius search needs an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
+  if (!fault && !tile->labelled)
+    fault = "sharded radius search: every rank's tile must be built with pclb200_index_build_ids";
+  require_every_rank_accepts(c, fault);
+  const float r2 = (float)(radius * radius);  // what radius_search compares against: d2 < r2
+  DevBuf<float4> dense;
+  dense.alloc(nq, st);
+  if (nq)
+    load_xyz_as_float4(c, queries, nq, stride, nullptr, 0, dense.p, st);
+  // r2 of 0 or NaN holds no point: no halo (a query box of its own would still fetch the points that coincide with it)
+  static const ShardedMapStages stages{"sharded_radius_halo", "sharded_radius_halo", "sharded_radius_build"};
+  HaloTrace trace;
+  std::unique_ptr<Index> local(sharded_local_map(c, *tile, dense.p, r2 > 0.f ? nq : 0, 0, r2, stages, &trace));
+  RadiusSinkBuffers to{nullptr, nullptr};
+  DevBuf<int32_t> di;
+  DevBuf<float> dd;
+  unsigned long long n = 0;
+  auto on_device = [&](unsigned long long total) {
+    to = sink(total);
+    if (!to.idx || !to.d2 || !total)
+      return RadiusSinkBuffers{nullptr, nullptr};
+    n = total;
+    return RadiusSinkBuffers{out_on_device(c, to.idx, n, di), out_on_device(c, to.d2, n, dd)};
+  };
+  if (nq) {
+    ProfScope ps(c, "sharded_radius_search");
+    radius_search(c, *local, dense.p, nq, sizeof(float4), radius, max_nn, out_offsets, on_device);
+  }
+  else {
+    const int64_t zero = 0;
+    PCLB_CUDA(cudaMemcpy(out_offsets, &zero, sizeof(zero), cudaMemcpyDefault));
+    on_device(0);
+  }
+  if (n) {
+    int32_t* d_idx = di.p ? di.p : to.idx;
+    k_sf_row_ids<<<persistent_blocks(c, n), 256, 0, st>>>(d_idx, n, trace.local_ids.p);
+    ++c.launches;
+    PCLB_CUDA(cudaGetLastError());
+    copy_out(c, to.idx, di, n);
+    copy_out(c, to.d2, dd, n);
+  }
+  check_device_error(c);
+  return n;
+}
+
+// GICP covariances of this rank's tile records on the whole map: the local map of their k nearest (the argument of the
+// filters), then the unchanged gicp_covariances on it, an ordinary index, with the staged records as its queries.
+void gicp_covariances_sharded(Ctx& c, const Index* tile, const void* pts, size_t n, size_t stride, int k,
+                              double gicp_epsilon, double* out, const char* fault)
+{
+  cudaStream_t st = c.stream;
+  PCLB_REQUIRE(comm_active(c), PCLB200_ERR_INVALID,
+               "sharded GICP covariances need an active communicator (pclb200_comm_init or pclb200_comm_export / _import)");
+  if (!fault && !tile->labelled)
+    fault = "sharded GICP covariances: every rank's tile must be built with pclb200_index_build_ids";
+  else if (!fault && k < 1)
+    fault = "sharded GICP covariances: k must be positive";
+  else if (!fault && n != tile->n_cloud)
+    fault = "sharded GICP covariances: pts must be the records the tile was built from (n = its record count)";
+  require_every_rank_accepts(c, fault);
+  DevBuf<float4> dense;
+  dense.alloc(n, st);
+  if (n)
+    load_xyz_as_float4(c, pts, n, stride, nullptr, 0, dense.p, st);
+  static const ShardedMapStages stages{"sharded_gicp_bound", "sharded_gicp_halo", "sharded_gicp_build"};
+  std::unique_ptr<Index> local(sharded_local_map(c, *tile, dense.p, n, k, 0.f, stages));
+  ProfScope ps(c, "sharded_gicp_covariances");
+  gicp_covariances(c, *local, dense.p, n, sizeof(float4), k, gicp_epsilon, out);
 }
 
 // k_eff: the whole map's clamp (kdtree_flann.hpp:241-242), the same on every rank (collective)
