@@ -452,30 +452,41 @@ static void run_rejectors(Icp& s)
   PCLB_CUDA(cudaGetLastError());
 }
 
+// the normal of position j with the plane_offset of the point there in w (icp_kernels.cuh); padding keeps a NaN normal
+__device__ __forceinline__ float4 normal_record(const float4* __restrict__ nrm, int rec, const float4& q)
+{
+  const float qn = __int_as_float(0x7fc00000);
+  if (rec < 0)
+    return make_float4(qn, qn, qn, 0.f);
+  float4 n = nrm[rec];
+  n.w = plane_offset(n, q);
+  return n;
+}
+
 __global__ void k_permute_normals(const float4* __restrict__ nrm_orig, const float4* __restrict__ pts, size_t n_padded,
                                   float4* __restrict__ out)
 {
   size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (j >= n_padded)
     return;
-  const int oi = __float_as_int(pts[j].w);
-  const float qn = __int_as_float(0x7fc00000);
-  out[j] = oi == kSentinelIndex ? make_float4(qn, qn, qn, 0.f) : nrm_orig[oi];
+  const float4 q = pts[j];
+  const int oi = __float_as_int(q.w);
+  out[j] = normal_record(nrm_orig, oi == kSentinelIndex ? -1 : oi, q);
 }
 
 // a labelled index (build_index_ids): its w lanes are ids, so the record of position j is slot_of_pos[j]
 __global__ void k_permute_normals_by_slot(const float4* __restrict__ nrm_rec, const int32_t* __restrict__ slot_of_pos,
-                                          size_t n_padded, float4* __restrict__ out)
+                                          const float4* __restrict__ pts, size_t n_padded, float4* __restrict__ out)
 {
   size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (j >= n_padded)
     return;
-  const int slot = slot_of_pos[j];
-  const float qn = __int_as_float(0x7fc00000);
-  out[j] = slot < 0 ? make_float4(qn, qn, qn, 0.f) : nrm_rec[slot];
+  out[j] = normal_record(nrm_rec, slot_of_pos[j], pts[j]);
 }
 
-// the normals (one per record of the cloud idx was built from) in the Morton order of idx
+// the normals (one per record of the cloud idx was built from) in the Morton order of idx, as the LLS accumulation reads
+// them: {nx, ny, nz, plane_offset}.  The other readers (normal-based correspondences, the surface-normal rejector, the
+// symmetric objective, the record rows of correspondences_sharded) read xyz only.
 static void normals_by_pos(Ctx& c, const Index* idx, const void* normals, size_t stride_n, DevBuf<float4>& out)
 {
   DevBuf<float4> dense;
@@ -483,8 +494,8 @@ static void normals_by_pos(Ctx& c, const Index* idx, const void* normals, size_t
   load_vec3_as_float4(c, normals, idx->n_cloud, stride_n, dense.p, c.stream);
   out.alloc(idx->pts.n, c.stream);
   if (idx->labelled)
-    k_permute_normals_by_slot<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->slot_of_pos.p, idx->pts.n,
-                                                                              out.p);
+    k_permute_normals_by_slot<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->slot_of_pos.p, idx->pts.p,
+                                                                              idx->pts.n, out.p);
   else
     k_permute_normals<<<grid_for(idx->pts.n, 256), 256, 0, c.stream>>>(dense.p, idx->pts.p, idx->pts.n, out.p);
   ++c.launches;
@@ -931,6 +942,7 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     a.pts = T.pts.p;
     a.root = T.root;
     a.tgt_normals = s.tgt_normals.p;
+    a.plane_offsets = 1;  // normals_by_pos; the sharded target's record exchange (gnrm) moves whole records
     a.cur = s.cur.p;
     a.n = s.n_q;
     a.pending = s.pending.p;

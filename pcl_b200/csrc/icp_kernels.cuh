@@ -120,6 +120,7 @@ struct IterArgs {
   const float4* pts;
   int root;
   const float4* tgt_normals;  // Morton order of the target (LLS only)
+  int plane_offsets;          // 1: w of tgt_normals = plane_offset of the point there (normals_by_pos), 0: w unused
   float4* cur;                // source, Morton order, w = slot
   size_t n;
   const Pending* pending;
@@ -202,9 +203,19 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
 #endif
 constexpr int kAccumBlocksPerSM = PCLB_ACCUM_BLOCKS;
 
+// The target point's own part of the point-to-plane residual nx dx + ny dy + nz dz - nx sx - ny sy - nz sz
+// (point_to_plane_lls.hpp:235): that float expression is evaluated left to right (no fma: -fmad=false), so its first
+// three terms depend on the target point alone and give the same bits whenever they are computed.  The Morton-ordered
+// target normals of an ICP session carry it in their w lane ({nx, ny, nz, plane_offset}, IterArgs::plane_offsets), so
+// that the accumulation gathers one 16-B record per pair instead of the point and its normal.
+__host__ __device__ __forceinline__ float plane_offset(const float4& n, const float4& q)
+{
+  return n.x * q.x + n.y * q.y + n.z * q.z;
+}
+
 // One pair's row of the contraction: ra = the MMA operand (w for SVD, v for LLS), rb = u (SVD) / the eight plain sums'
-// terms (LLS).  The two gathers (matched target point, its normal) are issued here; rows of pairs that are not accepted
-// stay zero.
+// terms (LLS).  The gathers of the pair's target records (SVD: the matched point; LLS: its normal, and the point only
+// when the normals carry no plane_offset) are issued here; rows of pairs that are not accepted stay zero.
 template <int EST>
 __device__ __forceinline__ void pair_rows(const IterArgs& a, const Match& m, const float4& p, float (&ra)[8], float (&rb)[8])
 {
@@ -212,8 +223,8 @@ __device__ __forceinline__ void pair_rows(const IterArgs& a, const Match& m, con
   for (int k = 0; k < 8; ++k)
     ra[k] = rb[k] = 0.f;
   if (match_accepted(m)) {
-    const float4 q = ldg4(a.pts + m.pos);
     if (EST == PCLB200_EST_SVD) {
+      const float4 q = ldg4(a.pts + m.pos);
       ra[0] = q.x; ra[1] = q.y; ra[2] = q.z; ra[3] = 1.f; ra[4] = m.d2;
       rb[0] = p.x; rb[1] = p.y; rb[2] = p.z; rb[3] = 1.f;
     }
@@ -222,14 +233,20 @@ __device__ __forceinline__ void pair_rows(const IterArgs& a, const Match& m, con
       rb[7] = 1.f;
       const float4 nn = ldg4(a.tgt_normals + m.pos);
       if (isfinite(nn.x) && isfinite(nn.y) && isfinite(nn.z)) {  // point_to_plane_lls.hpp:182-190
-        const float sx = p.x, sy = p.y, sz = p.z, dx = q.x, dy = q.y, dz = q.z, nx = nn.x, ny = nn.y, nz = nn.z;
+        const float sx = p.x, sy = p.y, sz = p.z, nx = nn.x, ny = nn.y, nz = nn.z;
         // float expressions, widened to double when they enter the products, exactly as :202-204 and :235
         // (no fma: -fmad=false)
         ra[0] = nz * sy - ny * sz;
         ra[1] = nx * sz - nz * sx;
         ra[2] = ny * sx - nx * sy;
         ra[3] = nx; ra[4] = ny; ra[5] = nz;
-        ra[6] = nx * dx + ny * dy + nz * dz - nx * sx - ny * sy - nz * sz;
+        if (a.plane_offsets) {
+          ra[6] = nn.w - nx * sx - ny * sy - nz * sz;  // nn.w = plane_offset(nn, q): the same bits
+        }
+        else {
+          const float4 q = ldg4(a.pts + m.pos);
+          ra[6] = nx * q.x + ny * q.y + nz * q.z - nx * sx - ny * sy - nz * sz;
+        }
         rb[0] = nx * nx; rb[1] = nx * ny; rb[2] = nx * nz;
         rb[3] = ny * ny; rb[4] = ny * nz; rb[5] = nz * nz;
       }

@@ -447,10 +447,16 @@ void stage_records(Ctx& c, const Index& frame, const unsigned char* recs, size_t
     keys_in.alloc(n, s);
     vals_in.alloc(n, s);
   }
-  const int vec = stride % 16 == 0 && reinterpret_cast<uintptr_t>(recs) % 16 == 0 &&
-                  reinterpret_cast<uintptr_t>(copy) % 16 == 0;
-  k_stage_records<<<grid_for(n, 256), 256, 0, s>>>(recs, n, stride, vec, copy, dense, frame.lo[0], frame.lo[1],
-                                                    frame.lo[2], frame.morton_scale, keys_in.p, vals_in.p);
+  const bool vec = stride % 16 == 0 && reinterpret_cast<uintptr_t>(recs) % 16 == 0 &&
+                   reinterpret_cast<uintptr_t>(copy) % 16 == 0;
+  if (vec)
+    k_stage_records<<<grid_for(n, 256), 256, 0, s>>>(reinterpret_cast<const float4*>(recs), n, (unsigned)(stride / 16),
+                                                      reinterpret_cast<float4*>(copy), dense, frame.lo[0], frame.lo[1],
+                                                      frame.lo[2], frame.morton_scale, keys_in.p, vals_in.p);
+  else
+    k_stage_records<<<grid_for(n, 256), 256, 0, s>>>(reinterpret_cast<const float*>(recs), n, (unsigned)(stride / 4),
+                                                      reinterpret_cast<float*>(copy), dense, frame.lo[0], frame.lo[1],
+                                                      frame.lo[2], frame.morton_scale, keys_in.p, vals_in.p);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
   if (!qb)

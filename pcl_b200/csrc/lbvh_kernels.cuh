@@ -132,33 +132,50 @@ __device__ __forceinline__ unsigned hilbert_key32(float x, float y, float z, flo
   return (unsigned)(hilbert63(x, y, z, lx, ly, lz, scale) >> 31);
 }
 
+// a unit that starts at word `word` (< 4) of a record, into the record's head (its first four words); a float4 unit
+// starts at word 0 and is the whole head
+__device__ __forceinline__ void put_head(float* head, unsigned, const float4& v) { *reinterpret_cast<float4*>(head) = v; }
+__device__ __forceinline__ void put_head(float* head, unsigned word, float v) { head[word] = v; }
+
 // One pass over n strided records (xyz at offset 0): the whole record into `copy`, xyz into `dense` as float4 (w = the
-// record's w when stride == 16, else 1) and, into keys / vals, the point's hilbert_key32 and its slot.  Each output is
-// nullable.  vec: stride is a multiple of 16 and recs / copy are 16-byte aligned (the copy moves float4s).
-__global__ void k_stage_records(const unsigned char* __restrict__ recs, size_t n, size_t stride, int vec,
-                                unsigned char* __restrict__ copy, float4* __restrict__ dense, float lx, float ly, float lz,
-                                float scale, unsigned* __restrict__ keys, int32_t* __restrict__ vals)
+// record's w when a record is 16 bytes, else 1) and, into keys / vals, the point's hilbert_key32 and its slot.  Each
+// output is nullable.  U: the unit the records are moved in (float4 when the stride is a multiple of 16 and recs / copy
+// are 16-byte aligned, else float); units = record stride / sizeof(U).  Each warp moves the contiguous bytes of its 32
+// records as consecutive units across its lanes, so every load and every store of the copy covers whole sectors (one
+// record per lane would touch 32 sectors per instruction, 16 B of each at a 48-B stride), and hands each record's first
+// 16 bytes to the lane of that record through shared memory.  blockDim.x = 256.
+template <typename U>
+__global__ void __launch_bounds__(256)
+k_stage_records(const U* __restrict__ recs, size_t n, unsigned units, U* __restrict__ copy, float4* __restrict__ dense,
+                float lx, float ly, float lz, float scale, unsigned* __restrict__ keys, int32_t* __restrict__ vals)
 {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= n)
-    return;
-  const float* r = reinterpret_cast<const float*>(recs + i * stride);
-  const float x = r[0], y = r[1], z = r[2];
-  if (copy) {
-    if (vec) {
-      const float4* r4 = reinterpret_cast<const float4*>(r);
-      float4* o4 = reinterpret_cast<float4*>(copy + i * stride);
-      for (size_t k = 0; k < stride / 16; ++k)
-        o4[k] = r4[k];
-    }
-    else {
-      float* o = reinterpret_cast<float*>(copy + i * stride);
-      for (size_t k = 0; k < stride / 4; ++k)
-        o[k] = r[k];
-    }
+  constexpr unsigned kWords = sizeof(U) / 4;
+  __shared__ __align__(16) float s_head[8][32][4];  // per warp: the first four words of each of its records
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t first = blockIdx.x * (size_t)blockDim.x + (threadIdx.x & ~31u);
+  if (first >= n)
+    return;  // the whole warp
+  const unsigned nrec = (unsigned)min((size_t)32, n - first);
+  const U* src = recs + first * units;
+  U* dst = copy ? copy + first * units : nullptr;
+  for (unsigned f = lane; f < nrec * units; f += 32) {
+    const unsigned rec = f / units, word = (f - rec * units) * kWords;
+    if (!dst && word >= 4)
+      continue;
+    const U v = src[f];
+    if (dst)
+      dst[f] = v;
+    if (word < 4)
+      put_head(s_head[warp][rec], word, v);
   }
+  __syncwarp();
+  if (lane >= nrec)
+    return;
+  const size_t i = first + lane;
+  const float4 h = *reinterpret_cast<const float4*>(s_head[warp][lane]);
+  const float x = h.x, y = h.y, z = h.z;
   if (dense)
-    dense[i] = make_float4(x, y, z, stride == 16 ? r[3] : 1.f);
+    dense[i] = make_float4(x, y, z, units * sizeof(U) == 16 ? h.w : 1.f);
   if (keys) {
     keys[i] = hilbert_key32(x, y, z, lx, ly, lz, scale);
     vals[i] = (int32_t)i;
