@@ -1,0 +1,51 @@
+/* pclb200_batch.h — C-ABI of libpclb200.so for a batch of ICP problems against one target in one session: a queue of
+ * scans against one prior map, or one scan from many initial guesses.  Every stage of an iteration is one launch for the
+ * whole batch, however many problems it holds, and the loop state of every problem comes back in one read.
+ *
+ * The entry points follow every convention of include/pclb200.h (status codes, host-or-device arrays, strides, squared
+ * fp32 distances, row-major transforms).  They live in their own header because they have no counterpart in the
+ * reference's API and the PCL facade (pcl_b200/pcl_compat/) does not reach them.  The target is the session's
+ * (pclb200_icp_set_target); no entry point here takes an index.
+ *
+ * Problem p is bit for bit what a fresh session with the same parameters, target and target normals would do after
+ * pclb200_icp_set_source(its records, its guess) and the same sequence of max_steps: every pclb200_icp_stats field
+ * (total_skipped_walks included), every iteration's correspondences and the aligned records.
+ *
+ * A batch takes nearest-neighbour correspondences; SVD (Umeyama or not), point-to-plane LLS or the symmetric objective;
+ * float or double Scalar; with_normals_transform; is_dense = 0; every convergence criterion; tracking OFF / ON / AUTO
+ * (AUTO decides per problem); host or device source arrays.  PCLB200_ERR_INVALID, with the session left as it was, for a
+ * rejector chain, use_reciprocal, a correspondence_kind other than NEAREST, an active communicator or a sharded target,
+ * and the symmetric objective without source normals. */
+#ifndef PCLB200_BATCH_H_
+#define PCLB200_BATCH_H_
+
+#include "pclb200.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* B = n_problems problems, problem p being the records [offsets[p], offsets[p+1]) of src (offsets: host, B + 1 entries,
+ * offsets[0] = 0, strictly increasing, offsets[B] = n); src_normals (nullable) as in pclb200_icp_set_source.  guesses
+ * (host, nullable = identity for every problem): B row-major 4x4 matrices.  Replaces whatever source the session held;
+ * pclb200_icp_set_source puts the session back into single-problem mode.  PCLB200_ERR_INVALID for B < 1 or B > 65536,
+ * bad offsets (an empty problem included), n >= 2^31 - 1, and the refusals in the header comment.
+ * pclb200_icp_get_cloud on a batch session writes all n records, each moved by its own problem's final transform. */
+PCLB200_API int pclb200_icp_set_source_batch(pclb200_icp* icp, const void* src, size_t n, size_t stride,
+                                             const void* src_normals, size_t stride_n, const int64_t* offsets,
+                                             int32_t n_problems, const double* guesses);
+
+/* Advances every problem still NOT_CONVERGED by up to max_steps iterations (pclb200_icp_iterate of each problem's own
+ * session).  stats (host, nullable): B entries.  pclb200_icp_iterate and pclb200_icp_get_correspondences refuse a batch
+ * session (PCLB200_ERR_INVALID). */
+PCLB200_API int pclb200_icp_iterate_batch(pclb200_icp* icp, int max_steps, pclb200_icp_stats* stats);
+
+/* The last evaluated iteration's correspondences of every problem, concatenated in problem order (each problem's list
+ * is what its own session's pclb200_icp_get_correspondences returns: index_query relative to the problem's first
+ * record).  out: host or device, capacity n (the batch's records); counts: host, B entries. */
+PCLB200_API int pclb200_icp_get_correspondences_batch(pclb200_icp* icp, pclb200_corr* out, int64_t* counts);
+
+#ifdef __cplusplus
+}
+#endif
+#endif /* PCLB200_BATCH_H_ */

@@ -85,6 +85,8 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_correspondences_sharded", "pclb200_correspondences_normals_sharded",
                    "pclb200_validate_transformation_sharded", "pclb200_inliers_sharded", "pclb200_radius_sharded",
                    "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
+# every symbol include/pclb200_batch.h declares (a batch of ICP problems in one session; tests/test_icp_batch_symbols.py)
+BATCH_SYMBOLS = ["pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch"]
 
 _lib = None
 
@@ -179,7 +181,10 @@ def lib():
     L.pclb200_comm_export.argtypes = [vp, vp]
     L.pclb200_comm_import.argtypes = [vp, C.c_int, C.c_int, vp]
     L.pclb200_comm_init.argtypes = [vp, C.c_int, C.c_int, vp]
-    for s in SYMBOLS + SHARDED_SYMBOLS:
+    L.pclb200_icp_set_source_batch.argtypes = [vp, vp, sz, sz, vp, sz, vp, C.c_int32, dp]
+    L.pclb200_icp_iterate_batch.argtypes = [vp, C.c_int, vp]
+    L.pclb200_icp_get_correspondences_batch.argtypes = [vp, vp, vp]
+    for s in SYMBOLS + SHARDED_SYMBOLS + BATCH_SYMBOLS:
         getattr(L, s)  # AttributeError here == header and library disagree
     _lib = L
     return L
@@ -944,6 +949,33 @@ class Icp:
         m = C.c_size_t()
         _check(lib().pclb200_icp_get_correspondences(self.h, C.c_void_p(out.ctypes.data), C.byref(m)))
         return out[:m.value]
+
+    def set_source_batch(self, src, offsets, normals=None, guesses=None):
+        """B problems against the session's target, problem p = records offsets[p]:offsets[p+1] of src (B + 1 offsets);
+        guesses: (B, 4, 4) or None.  Each problem then runs as its own set_source session would, bit for bit."""
+        b, nb = _Buf(src), _Buf(normals)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        g = None if guesses is None else np.ascontiguousarray(guesses, dtype=np.float64)
+        _check(lib().pclb200_icp_set_source_batch(self.h, b.ptr, b.rows, b.stride, nb.ptr, nb.stride,
+                                                  off.ctypes.data_as(C.c_void_p), len(off) - 1,
+                                                  None if g is None else g.ctypes.data_as(C.POINTER(C.c_double))))
+        self.n_src = self.n_queries = b.rows
+        self.n_problems = len(off) - 1
+
+    def iterate_batch(self, max_steps=2 ** 31 - 1):
+        """one list entry per problem: the dict iterate() returns"""
+        st = (IcpStats * self.n_problems)()
+        _check(lib().pclb200_icp_iterate_batch(self.h, int(max_steps), C.cast(st, C.c_void_p)))
+        return [x.as_dict() for x in st]
+
+    def get_correspondences_batch(self):
+        """one array per problem: what get_correspondences() of its own session returns"""
+        out = np.empty(max(self.n_queries, 1), dtype=CORR_DTYPE)
+        counts = np.zeros(self.n_problems, dtype=np.int64)
+        _check(lib().pclb200_icp_get_correspondences_batch(self.h, C.c_void_p(out.ctypes.data),
+                                                           C.c_void_p(counts.ctypes.data)))
+        ends = np.cumsum(counts)
+        return [out[e - c:e].copy() for c, e in zip(counts, ends)]
 
     def get_cloud(self, out=None, stride_floats=4, normals=None):
         if out is None:

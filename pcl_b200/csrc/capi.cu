@@ -7,6 +7,7 @@
 #include <memory>
 
 #include "internal.cuh"
+#include "../../include/pclb200_batch.h"
 
 namespace pclb200 {
 // icp.cu
@@ -22,6 +23,10 @@ void icp_set_target_sharded(Icp& s, const Index* tile, const void* tgt_normals, 
 void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
                     const int32_t* indices, size_t n_idx, const double* guess);
 void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats);
+void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
+                          const int64_t* offsets, int n_problems, const double* guesses);
+void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats);
+void icp_get_correspondences_batch(Icp& s, pclb200_corr* out, int64_t* counts);
 void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, size_t stride_n);
 size_t icp_get_correspondences(Icp& s, pclb200_corr* out);
 void estimate_pairs(Ctx& c, int est, const void* src, size_t stride_s, const void* tgt, const void* tgt_normals,
@@ -707,6 +712,27 @@ int pclb200_icp_set_source(pclb200_icp* icp, const void* src, size_t n, size_t s
 int pclb200_icp_iterate(pclb200_icp* icp, int max_steps, pclb200_icp_stats* stats)
 {
   return on_ctx(icp, [&](Icp& s) { icp_iterate(s, max_steps, stats); });
+}
+
+int pclb200_icp_set_source_batch(pclb200_icp* icp, const void* src, size_t n, size_t stride, const void* src_normals,
+                                 size_t stride_n, const int64_t* offsets, int32_t n_problems, const double* guesses)
+{
+  return on_ctx(icp, [&](Icp& s) {
+    icp_set_source_batch(s, src, n, stride, src_normals, stride_n, offsets, n_problems, guesses);
+  });
+}
+
+int pclb200_icp_iterate_batch(pclb200_icp* icp, int max_steps, pclb200_icp_stats* stats)
+{
+  return on_ctx(icp, [&](Icp& s) { icp_iterate_batch(s, max_steps, stats); });
+}
+
+int pclb200_icp_get_correspondences_batch(pclb200_icp* icp, pclb200_corr* out, int64_t* counts)
+{
+  return on_ctx(icp, [&](Icp& s) {
+    PCLB_REQUIRE(out && counts, PCLB200_ERR_INVALID, "NULL argument");
+    icp_get_correspondences_batch(s, out, counts);
+  });
 }
 
 int pclb200_icp_get_cloud(pclb200_icp* icp, void* out_pts, size_t stride_out, void* out_normals, size_t stride_n)

@@ -13,6 +13,19 @@ struct GridSum {
   double* accum;
 };
 
+// Where a block sits in the grid whose sum it takes part in: the launch's grid (HwGrid), or the grid of one problem of a
+// batch that lies inside a larger launch (VirtualGrid, icp_kernels.cuh: BatchBlock).  The sums of a virtual grid are
+// those of a launch of vgrid blocks, bit for bit.
+struct HwGrid {
+  __device__ __forceinline__ unsigned block() const { return blockIdx.x; }
+  __device__ __forceinline__ unsigned blocks() const { return gridDim.x; }
+};
+struct VirtualGrid {
+  unsigned vblock, vgrid;
+  __device__ __forceinline__ unsigned block() const { return vblock; }
+  __device__ __forceinline__ unsigned blocks() const { return vgrid; }
+};
+
 // The fixed-order grid sum of WIDTH slots.  rows[w * WIDTH + t]: the sums of slot t over the pairs of warp w of this
 // block, w < nwarps, in shared memory.  Thread t < WIDTH adds them up over the warps into partials[block * STRIDE + t];
 // the LAST block to take a ticket adds those up over the blocks, in block order (bitwise reproducible), into out[t] and
@@ -20,21 +33,21 @@ struct GridSum {
 // thread of every block.  is_last: a __shared__ flag declared by the caller, so that it keeps its place in the caller's
 // shared memory.  The pointers are taken by reference, so that a kernel reads them from its parameters where they are
 // used.
-template <int WIDTH, int STRIDE>
+template <int WIDTH, int STRIDE, class G = HwGrid>
 __device__ __forceinline__ bool grid_fold(const double* rows, int nwarps, double* const& partials,
-                                          unsigned* const& counter, bool& is_last, double* out)
+                                          unsigned* const& counter, bool& is_last, double* out, const G& grid = G())
 {
   if (threadIdx.x < WIDTH) {
     double v = 0.0;
     for (int w = 0; w < nwarps; ++w)
       v += rows[w * WIDTH + threadIdx.x];
-    partials[(size_t)blockIdx.x * STRIDE + threadIdx.x] = v;
+    partials[(size_t)grid.block() * STRIDE + threadIdx.x] = v;
   }
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
     const unsigned tk = atomicAdd(counter, 1u);
-    is_last = (tk == gridDim.x - 1);
+    is_last = (tk == grid.blocks() - 1);
   }
   __syncthreads();
   const bool last = is_last;
@@ -42,7 +55,7 @@ __device__ __forceinline__ bool grid_fold(const double* rows, int nwarps, double
     __threadfence();
     if (threadIdx.x < WIDTH) {
       double v = 0.0;
-      for (unsigned b = 0; b < gridDim.x; ++b)
+      for (unsigned b = 0; b < grid.blocks(); ++b)
         v += __ldcg(&partials[(size_t)b * STRIDE + threadIdx.x]);
       out[threadIdx.x] = v;
     }
@@ -52,8 +65,8 @@ __device__ __forceinline__ bool grid_fold(const double* rows, int nwarps, double
 
 // per-thread accumulators acc[0..NACC) -> block (fixed order) -> grid (grid_fold) -> g.accum[0..kAccum), zero beyond
 // NACC.  Returns true in the last block.
-template <int NACC>
-__device__ __forceinline__ bool block_reduce_and_publish(const double* acc, const GridSum& g)
+template <int NACC, class G = HwGrid>
+__device__ __forceinline__ bool block_reduce_and_publish(const double* acc, const GridSum& g, const G& grid = G())
 {
   __shared__ double sm[8][NACC];
   __shared__ bool is_last;
@@ -68,7 +81,7 @@ __device__ __forceinline__ bool block_reduce_and_publish(const double* acc, cons
       sm[warp][t] = v;
   }
   __syncthreads();
-  if (!grid_fold<NACC, kAccum>(&sm[0][0], blockDim.x >> 5, g.partials, g.counter, is_last, g.accum))
+  if (!grid_fold<NACC, kAccum>(&sm[0][0], blockDim.x >> 5, g.partials, g.counter, is_last, g.accum, grid))
     return false;
   if (threadIdx.x >= NACC && threadIdx.x < kAccum)
     g.accum[threadIdx.x] = 0.0;

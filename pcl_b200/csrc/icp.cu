@@ -38,23 +38,28 @@ bool comm_peer_fused(const Ctx& c);  // the per-iteration exchange happens insid
 int comm_nranks(const Ctx& c);
 
 // ---- misc streaming kernels ------------------------------------------------------------------------------
+__device__ __forceinline__ void transform_one(const Pending& P, float4* __restrict__ pts, size_t i,
+                                              float4* __restrict__ normals /* nullable */)
+{
+  float4 p = pts[i];
+  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z)))
+    return;
+  apply_pending(P, p.x, p.y, p.z);
+  pts[i] = p;
+  if (normals) {
+    float4 m = normals[i];
+    if (P.mode == kApplyIcp && !(isfinite(m.x) && isfinite(m.y) && isfinite(m.z)))
+      return;  // icp.hpp:97-98
+    apply_pending_normal(P, m.x, m.y, m.z);
+    normals[i] = m;
+  }
+}
+
 __device__ __forceinline__ void transform_range(const Pending& P, float4* __restrict__ pts, size_t n,
                                                 float4* __restrict__ normals /* nullable */)
 {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float4 p = pts[i];
-    if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z)))
-      continue;
-    apply_pending(P, p.x, p.y, p.z);
-    pts[i] = p;
-    if (normals) {
-      float4 m = normals[i];
-      if (P.mode == kApplyIcp && !(isfinite(m.x) && isfinite(m.y) && isfinite(m.z)))
-        continue;  // icp.hpp:97-98
-      apply_pending_normal(P, m.x, m.y, m.z);
-      normals[i] = m;
-    }
-  }
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    transform_one(P, pts, i, normals);
 }
 
 // the transform k_solve left for the next iteration
@@ -72,6 +77,17 @@ __global__ void k_transform(float4* __restrict__ pts, size_t n, const Pending P,
   transform_range(P, pts, n, normals);
 }
 
+// a batch (icp_kernels.cuh: BatchBlock): point i moved by the Pending of its problem, where that one applies
+__global__ void k_transform_batch(float4* __restrict__ pts, size_t n, const long long* __restrict__ offsets,
+                                  int n_problems, const Pending* __restrict__ P, float4* __restrict__ normals)
+{
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const Pending& Q = P[problem_of(offsets, n_problems, (long long)i)];
+    if (Q.apply)
+      transform_one(Q, pts, i, normals);
+  }
+}
+
 __global__ void k_set_pending(Pending* p, const Pending P) { *p = P; }
 __global__ void k_clear_apply(Pending* p) { p->apply = 0; }
 
@@ -84,38 +100,19 @@ __global__ void k_assemble_records(const unsigned char* __restrict__ raw, size_t
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n)
     return;
-  const float* r = reinterpret_cast<const float*>(raw + i * stride);
-  float p[3] = {r[0], r[1], r[2]}, m[3] = {0.f, 0.f, 0.f};
-  if (nrm_word >= 0) {
-    m[0] = r[nrm_word]; m[1] = r[nrm_word + 1]; m[2] = r[nrm_word + 2];
-  }
-  if (isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2])) {
-    apply_pending(P, p[0], p[1], p[2]);
-    if (nrm_word >= 0 && !(P.mode == kApplyIcp && !(isfinite(m[0]) && isfinite(m[1]) && isfinite(m[2]))))
-      apply_pending_normal(P, m[0], m[1], m[2]);  // icp.hpp:97-98
-  }
-  // the normal is written after xyz: it wins where a caller's layout lets the two overlap
-  auto word = [&](int q, float v) {
-    const int qn = q - nrm_word;
-    return nrm_word >= 0 && qn >= 0 && qn < 3 ? m[qn] : q < 3 ? p[q] : v;
-  };
-  if (vec) {
-    const float4* r4 = reinterpret_cast<const float4*>(r);
-    float4* o4 = reinterpret_cast<float4*>(out + i * stride);
-    for (int k = 0; k < (int)(stride / 16); ++k) {
-      float4 v = r4[k];
-      v.x = word(4 * k, v.x);
-      v.y = word(4 * k + 1, v.y);
-      v.z = word(4 * k + 2, v.z);
-      v.w = word(4 * k + 3, v.w);
-      o4[k] = v;
-    }
-  }
-  else {
-    float* o = reinterpret_cast<float*>(out + i * stride);
-    for (int q = 0; q < (int)(stride / 4); ++q)
-      o[q] = word(q, r[q]);
-  }
+#include "assemble_body.inc"
+}
+
+// a batch: record i moved by the final transform of its problem (the offsets of icp_set_source_batch)
+__global__ void k_assemble_records_batch(const unsigned char* __restrict__ raw, size_t n, size_t stride, int nrm_word,
+                                         const long long* __restrict__ offsets, int n_problems,
+                                         const Pending* __restrict__ finals, int vec, unsigned char* __restrict__ out)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const Pending P = finals[problem_of(offsets, n_problems, (long long)i)];
+#include "assemble_body.inc"
 }
 
 // strided write-back of a dense float4 array: xyz into out + i*stride (+ optional w = 1 when stride >= 16)
@@ -222,6 +219,61 @@ struct Reducer {  // scratch of the grid sums (grid_fold)
   GridSum sum() const { return GridSum{partials.p, counter.p, accum.p}; }
 };
 
+// pinned host memory of one session (the batch read-back), freed with it
+struct PinnedBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+  PinnedBuf() = default;
+  PinnedBuf(const PinnedBuf&) = delete;
+  PinnedBuf& operator=(const PinnedBuf&) = delete;
+  PinnedBuf(PinnedBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+  PinnedBuf& operator=(PinnedBuf&& o) noexcept
+  {
+    if (this != &o) {
+      release();
+      p = o.p; bytes = o.bytes;
+      o.p = nullptr; o.bytes = 0;
+    }
+    return *this;
+  }
+  ~PinnedBuf() { release(); }
+  void reserve(size_t b)
+  {
+    if (b <= bytes)
+      return;
+    release();
+    PCLB_CUDA(cudaMallocHost(&p, b));
+    bytes = b;
+  }
+  void release()
+  {
+    if (p)
+      cudaFreeHost(p);
+    p = nullptr;
+    bytes = 0;
+  }
+};
+
+// the state of a batch session (icp_set_source_batch): B > 0 problems over consecutive record ranges of the source, the
+// per-problem slots the batch kernels index (icp_kernels.cuh: BatchBlock) and the block tables of the three grids
+struct IcpBatch {
+  int B = 0;                         // 0: a single-problem session
+  std::vector<long long> offsets;    // B + 1
+  DevBuf<long long> d_offsets;
+  DevBuf<int32_t> rel;               // record -> its index within its problem (index_query of the lists)
+  DevBuf<BatchBlock> wtab, atab, gtab;  // the search's grids, k_accum_dmma's, k_accum's
+  unsigned a_blocks = 0, g_blocks = 0;  // partials slots of atab / gtab
+  DevBuf<Pending> pending;
+  DevBuf<LoopCtrl> ctrl;
+  DevBuf<SolveOut> solve_out;
+  DevBuf<unsigned long long> skip_count;
+  DevBuf<unsigned> counter;
+  DevBuf<double> partials, accum;
+  std::vector<LoopCtrl> loop;
+  std::vector<int64_t> total_skipped;
+  PinnedBuf host;                    // B loop states, B skip counts, the device error flag
+};
+
 struct Icp {
   Ctx* ctx = nullptr;
   pclb200_icp_params P;
@@ -266,6 +318,7 @@ struct Icp {
   // the loop state between icp_iterate calls (Scalar-typed values are kept in double; float mode rounds after every
   // operation): counters, DefaultConvergenceCriteria state, final / last transform, tracking decision
   LoopCtrl loop;
+  IcpBatch batch;
 };
 
 static void set_identity(double* T)
@@ -711,14 +764,12 @@ __global__ void k_gather_subset(const float4* __restrict__ all, const int32_t* _
     out[i] = all[sub[i]];
 }
 
-void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
-                    const int32_t* indices, size_t n_idx, const double* guess)
+// The caller's records into the session (src_all, src_raw) and their queries into qb, in the order of the target frame.
+static void stage_source(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
+                         const int32_t* indices, size_t n_idx, QueryBatch& qb)
 {
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
-  PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
-  PCLB_REQUIRE(src != nullptr && n > 0, PCLB200_ERR_INVALID, "icp: empty source");
-  PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
   s.n_all = n;
   s.shard_comm = 0;
   s.shard_checked = false;
@@ -754,7 +805,6 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   }
   s.n_q = indices ? n_idx : n;
   s.src_orig.release();
-  QueryBatch qb;
   {
     ProfScope ps(c, "query_sort");
     stage_records(c, target_frame(s), recs, n, stride, copy, dense, indices ? nullptr : &qb);
@@ -771,6 +821,14 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
       make_query_batch(c, target_frame(s), sub.p, s.n_q, qb);
     }
   }
+}
+
+// The staged queries qb become the session's `cur`, with their normals and the per-query arrays of the loop
+static void finish_source(Icp& s, QueryBatch& qb, const void* src_normals, size_t stride_n)
+{
+  Ctx& c = *s.ctx;
+  cudaStream_t st = c.stream;
+  const size_t n = s.n_all, stride = s.src_stride;
   s.cur = std::move(qb.q);
   // Nothing in the loop reads the source normals except through cur_normals; the output reads normals that live in the
   // records from src_raw.  So a dense copy is staged only for cur_normals or for normals kept outside the records.
@@ -804,36 +862,97 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
     k_cur_labels<<<grid_for(s.n_q, 256), 256, 0, st>>>(s.cur.p, s.src_orig.p, s.n_q, s.cur_label.p);
     ++c.launches;
   }
+}
+
+static bool is_identity(const double* T)
+{
+  for (int i = 0; i < 16; ++i)
+    if (T[i] != ((i % 5 == 0) ? 1.0 : 0.0))
+      return false;
+  return true;
+}
+
+void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
+                    const int32_t* indices, size_t n_idx, const double* guess)
+{
+  Ctx& c = *s.ctx;
+  PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
+  PCLB_REQUIRE(src != nullptr && n > 0, PCLB200_ERR_INVALID, "icp: empty source");
+  PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
+  s.batch = IcpBatch();
+  QueryBatch qb;
+  stage_source(s, src, n, stride, src_normals, stride_n, indices, n_idx, qb);
+  finish_source(s, qb, src_normals, stride_n);
   icp_reset_state(s, guess);
   // icp.hpp:125-134: a non-identity guess is applied once, before the first search
-  bool guess_identity = true;
-  if (guess)
-    for (int i = 0; i < 16; ++i)
-      if (s.loop.final_T[i] != ((i % 5 == 0) ? 1.0 : 0.0))
-        guess_identity = false;
-  if (!guess_identity)
+  if (!is_identity(s.loop.final_T))
     transform_on_device(c, s.loop.final_T, transform_mode(s.P), s.cur.p, s.n_q, s.cur_normals.p);
   set_pending(c, s.pending.p, make_pending(s.loop.last_T, transform_mode(s.P), 0));
   PCLB_CUDA(cudaGetLastError());
 }
 
-static void fill_stats(const Icp& s, pclb200_icp_stats* st)
+static void fill_stats(const LoopCtrl& L, int64_t total_skipped, pclb200_icp_stats* st)
 {
   if (!st)
     return;
-  const LoopCtrl& L = s.loop;
   st->converged = L.converged ? 1 : 0;
   st->state = L.state;
   st->iterations = L.iterations;
   st->reserved = 0;
   st->n_correspondences = (int64_t)L.n_corr;
   st->total_correspondences = L.total_corr;
-  st->total_skipped_walks = s.total_skipped;
+  st->total_skipped_walks = total_skipped;
   st->mse = L.mse;
   for (int i = 0; i < 16; ++i) {
     st->final_transformation[i] = L.final_T[i];
     st->last_transformation[i] = L.last_T[i];
   }
+}
+
+// what DefaultConvergenceCriteria and the tracking decision of k_solve read
+static CritParams crit_params(const Icp& s, int track_mode)
+{
+  CritParams crit;
+  crit.max_iterations = s.P.max_iterations;
+  crit.failure_after_max_iter = s.P.failure_after_max_iter;
+  crit.max_iterations_similar = s.P.max_iterations_similar_transforms;
+  crit.scalar_is_double = s.P.scalar_is_double;
+  crit.track_mode = track_mode;
+  crit.rot_eps = s.P.transformation_rotation_epsilon;
+  crit.trans_eps = s.P.transformation_epsilon;
+  crit.rel_mse = s.P.euclidean_fitness_epsilon;
+  crit.abs_mse = s.P.mse_threshold_absolute;
+  const Index& F = target_frame(s);
+  double rmax = 0.0;
+  for (int r = 0; r < 3; ++r) {
+    const double m = std::max(std::fabs((double)F.lo[r]), std::fabs((double)F.hi[r]));
+    rmax += m * m;
+  }
+  crit.rmax = std::sqrt(rmax);
+  return crit;
+}
+
+// the search and accumulation arguments that do not depend on where the loop state lives
+static IterArgs loop_args(const Icp& s, int track_mode)
+{
+  const Index& T = *s.tgt;
+  IterArgs a;
+  memset(&a, 0, sizeof(a));
+  a.nodes = T.nodes.p;
+  a.pts = T.pts.p;
+  a.root = T.root;
+  a.tgt_normals = s.tgt_normals.p;
+  a.plane_offsets = 1;  // normals_by_pos; the sharded target's record exchange (gnrm) moves whole records
+  a.cur = s.cur.p;
+  a.n = s.n_q;
+  a.gate = gate_from_max_dist(s.P.max_correspondence_distance);
+  a.d_error = s.ctx->d_error;
+  a.src_orig = s.src_orig.p;
+  a.cur_normals = s.cur_normals.p;
+  a.enforce_same_dir = s.P.enforce_same_direction_normals;
+  a.cells = tree_view(T).cells;
+  a.track_sel = track_mode == PCLB200_TRACK_AUTO;  // the search runs only in the flavour of the device's decision
+  return a;
 }
 
 // The do-while of icp.hpp:164-241.  Every iteration enqueues correspondence estimation -> rejector chain -> accumulation
@@ -844,6 +963,7 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
 {
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
+  PCLB_REQUIRE(!s.batch.B, PCLB200_ERR_INVALID, "icp: a batch session advances with iterate_batch");
   PCLB_REQUIRE(s.tgt && s.cur.p, PCLB200_ERR_INVALID, "icp: set_target and set_source must precede iterate");
   PCLB_REQUIRE(s.P.estimator == PCLB200_EST_SVD || s.tgt_normals.p, PCLB200_ERR_INVALID,
                "icp: point-to-plane needs target normals");
@@ -888,25 +1008,8 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     // RMS correspondence distance (k_solve), and the skip test fires from the following iteration on.  Only the plain
     // nearest-neighbour search keeps the bounds.
     const int track_mode = (normal_based || s.P.use_reciprocal) ? (int)PCLB200_TRACK_OFF : s.P.track_mode;
-    CritParams crit;
-    crit.max_iterations = s.P.max_iterations;
-    crit.failure_after_max_iter = s.P.failure_after_max_iter;
-    crit.max_iterations_similar = s.P.max_iterations_similar_transforms;
-    crit.scalar_is_double = s.P.scalar_is_double;
-    crit.track_mode = track_mode;
-    crit.rot_eps = s.P.transformation_rotation_epsilon;
-    crit.trans_eps = s.P.transformation_epsilon;
-    crit.rel_mse = s.P.euclidean_fitness_epsilon;
-    crit.abs_mse = s.P.mse_threshold_absolute;
+    const CritParams crit = crit_params(s, track_mode);
     const Index& F = target_frame(s);
-    {
-      double rmax = 0.0;
-      for (int r = 0; r < 3; ++r) {
-        const double m = std::max(std::fabs((double)F.lo[r]), std::fabs((double)F.hi[r]));
-        rmax += m * m;
-      }
-      crit.rmax = std::sqrt(rmax);
-    }
     if (track_mode != PCLB200_TRACK_AUTO)  // AUTO carries the last decision over from the previous call
       s.loop.track_next = track_mode == PCLB200_TRACK_ON ? 1 : 0;
     LoopCtrl* h_ctrl = static_cast<LoopCtrl*>(c.pinned);
@@ -936,30 +1039,15 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
       s.loop = *h_ctrl;
       s.total_skipped = (int64_t)*h_skipped;
     };
-    IterArgs a;
-    memset(&a, 0, sizeof(a));
-    a.nodes = T.nodes.p;
-    a.pts = T.pts.p;
-    a.root = T.root;
-    a.tgt_normals = s.tgt_normals.p;
-    a.plane_offsets = 1;  // normals_by_pos; the sharded target's record exchange (gnrm) moves whole records
-    a.cur = s.cur.p;
-    a.n = s.n_q;
+    IterArgs a = loop_args(s, track_mode);
     a.pending = s.pending.p;
-    a.gate = gate_from_max_dist(s.P.max_correspondence_distance);
     a.origin = s.ctrl.p->origin;
     a.partials = s.red.partials.p;
     a.partials2 = s.red.partials2.p;
     a.counter = s.red.counter.p;
     a.accum = s.red.accum.p;
-    a.d_error = c.d_error;
-    a.src_orig = s.src_orig.p;
     a.skip_count = s.skip_count.p;
-    a.cur_normals = s.cur_normals.p;
-    a.enforce_same_dir = s.P.enforce_same_direction_normals;
-    a.cells = tree_view(T).cells;
     a.ctrl = s.ctrl.p;
-    a.track_sel = track_mode == PCLB200_TRACK_AUTO;  // the search runs only in the flavour of the device's decision
     const unsigned grid = persistent_blocks(c, s.n_q);
     // the search: 72 blocks per SM over the 5 that are resident, so a block walks only a few warp rounds and the SMs run
     // out of work together (18 left the last blocks walking alone; a block per warp round pays for every launch that a
@@ -1070,7 +1158,7 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats)
     if (!needs_host_between)
       read_back();
   }
-  fill_stats(s, stats);
+  fill_stats(s.loop, s.total_skipped, stats);
 }
 
 // correspondences of the last evaluated iteration (Registration::correspondences_, what PCL hands to the
@@ -1096,6 +1184,7 @@ size_t icp_get_correspondences(Icp& s, pclb200_corr* out)
 {
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
+  PCLB_REQUIRE(!s.batch.B, PCLB200_ERR_INVALID, "icp: a batch session hands its lists out through get_correspondences_batch");
   PCLB_REQUIRE(s.tgt && s.cur.p && s.match.p, PCLB200_ERR_INVALID, "icp: no iteration has run");
   if (!s.n_q || s.loop.iterations == 0)
     return 0;
@@ -1110,6 +1199,316 @@ size_t icp_get_correspondences(Icp& s, pclb200_corr* out)
   return m;
 }
 
+// ---- a batch of problems in one loop (include/pclb200_batch.h) ---------------------------------------------------------
+// key of the second, stable pass of the batch's query sort: the problem of the record whose query sits at j
+__global__ void k_problem_keys(const float4* __restrict__ q, size_t n, const long long* __restrict__ offsets,
+                               int n_problems, unsigned* __restrict__ keys, int32_t* __restrict__ vals)
+{
+  const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (j >= n)
+    return;
+  keys[j] = (unsigned)problem_of(offsets, n_problems, __float_as_int(q[j].w));
+  vals[j] = (int32_t)j;
+}
+
+__global__ void k_gather_by(const float4* __restrict__ q, const int32_t* __restrict__ vals, size_t n,
+                            float4* __restrict__ out)
+{
+  const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (j < n)
+    out[j] = q[vals[j]];
+}
+
+__global__ void k_relative_index(const long long* __restrict__ offsets, int n_problems, size_t n, int32_t* __restrict__ rel)
+{
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i < n)
+    rel[i] = (int32_t)((long long)i - offsets[problem_of(offsets, n_problems, (long long)i)]);
+}
+
+// the lists of problems that have run no iteration are empty (icp_get_correspondences); counts[p] = the list of p's length
+__global__ void k_mask_and_count(pclb200_corr* __restrict__ by_slot, size_t n, const long long* __restrict__ offsets,
+                                 int n_problems, const int* __restrict__ live, unsigned long long* __restrict__ counts)
+{
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n || by_slot[i].index_match < 0)
+    return;
+  const int p = problem_of(offsets, n_problems, (long long)i);
+  if (live[p])
+    atomicAdd(counts + p, 1ull);
+  else
+    by_slot[i].index_match = -1;
+}
+
+// what a batch refuses (include/pclb200_batch.h), checked by set_source_batch and by every iterate_batch
+static void check_batch_session(const Icp& s)
+{
+  Ctx& c = *s.ctx;
+  PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
+  PCLB_REQUIRE(!comm_active(c) && !s.sharded_target, PCLB200_ERR_INVALID,
+               "icp: a batch runs on one GPU: no communicator, no sharded target");
+  PCLB_REQUIRE(s.rejectors.empty(), PCLB200_ERR_INVALID, "icp: a batch takes no rejector chain");
+  PCLB_REQUIRE(!s.P.use_reciprocal, PCLB200_ERR_INVALID, "icp: a batch takes no reciprocal correspondences");
+  PCLB_REQUIRE(s.P.correspondence_kind == PCLB200_CORR_NEAREST, PCLB200_ERR_INVALID,
+               "icp: a batch takes nearest-neighbour correspondences only");
+}
+
+// batch_blocks's table (icp_kernels.cuh) on the device; *slots = its blocks (partials slots)
+template <typename Grid>
+static void batch_table(Ctx& c, const std::vector<long long>& off, Grid grid, DevBuf<BatchBlock>& out, unsigned* slots)
+{
+  const std::vector<BatchBlock> h = batch_blocks(off, grid);
+  if (slots)
+    *slots = (unsigned)h.size();
+  out.alloc(h.size(), c.stream);
+  PCLB_CUDA(cudaMemcpyAsync(out.p, h.data(), h.size() * sizeof(BatchBlock), cudaMemcpyHostToDevice, c.stream));
+}
+
+void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
+                          const int64_t* offsets, int n_problems, const double* guesses)
+{
+  Ctx& c = *s.ctx;
+  cudaStream_t st = c.stream;
+  check_batch_session(s);
+  PCLB_REQUIRE(n_problems >= 1 && n_problems <= 65536, PCLB200_ERR_INVALID, "icp: a batch holds 1 to 65536 problems");
+  PCLB_REQUIRE(src != nullptr && n > 0 && offsets != nullptr, PCLB200_ERR_INVALID, "icp: empty source");
+  PCLB_REQUIRE(n < (size_t)0x7fffffff, PCLB200_ERR_INVALID, "icp: a batch holds fewer than 2^31 - 1 records");
+  PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
+  PCLB_REQUIRE(offsets[0] == 0 && offsets[n_problems] == (int64_t)n, PCLB200_ERR_INVALID,
+               "icp: batch offsets must run from 0 to n");
+  for (int p = 0; p < n_problems; ++p)
+    PCLB_REQUIRE(offsets[p + 1] > offsets[p], PCLB200_ERR_INVALID,
+                 "icp: batch offsets must increase strictly (every problem holds a record)");
+  PCLB_REQUIRE(s.P.estimator != PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS || src_normals, PCLB200_ERR_INVALID,
+               "icp: the symmetric objective needs source normals");
+  const int B = n_problems;
+  PinnedBuf host = std::move(s.batch.host);  // kept across batches: freeing pinned memory synchronises the device
+  s.batch = IcpBatch();
+  IcpBatch& b = s.batch;
+  b.host = std::move(host);
+  b.B = B;
+  b.offsets.assign(offsets, offsets + B + 1);
+  b.d_offsets.alloc(B + 1, st);
+  PCLB_CUDA(cudaMemcpyAsync(b.d_offsets.p, b.offsets.data(), (B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  // the queries of all problems in the order of the target frame (stable), then by problem (stable): within each
+  // problem the order make_query_batch gives that problem alone; w = the record's index in the batch
+  QueryBatch qb;
+  stage_source(s, src, n, stride, src_normals, stride_n, nullptr, 0, qb);
+  {
+    ProfScope ps(c, "query_sort");
+    DevBuf<unsigned> keys_in, keys;
+    DevBuf<int32_t> vals_in, vals;
+    keys_in.alloc(n, st);
+    keys.alloc(n, st);
+    vals_in.alloc(n, st);
+    vals.alloc(n, st);
+    k_problem_keys<<<grid_for(n, 256), 256, 0, st>>>(qb.q.p, n, b.d_offsets.p, B, keys_in.p, vals_in.p);
+    ++c.launches;
+    int bits = 1;
+    while ((1 << bits) < B)
+      ++bits;
+    size_t tmp_bytes = 0;
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, bits, st));
+    DevBuf<unsigned char> tmp;
+    tmp.alloc(tmp_bytes, st);
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, bits, st));
+    c.launches += 2;
+    DevBuf<float4> sorted;
+    sorted.alloc(n, st);
+    k_gather_by<<<grid_for(n, 256), 256, 0, st>>>(qb.q.p, vals.p, n, sorted.p);
+    ++c.launches;
+    qb.q = std::move(sorted);
+  }
+  finish_source(s, qb, src_normals, stride_n);
+  b.rel.alloc(n, st);
+  k_relative_index<<<grid_for(n, 256), 256, 0, st>>>(b.d_offsets.p, B, n, b.rel.p);
+  ++c.launches;
+  // each problem's grids are the ones its own align launches (icp_iterate)
+  batch_table(c, b.offsets, [&](size_t m) { return persistent_blocks(c, m, 256, 72); }, b.wtab, nullptr);
+  batch_table(c, b.offsets, [&](size_t m) { return std::min(persistent_blocks(c, m, 256, kAccumBlocksPerSM), s.red.max_blocks); },
+              b.atab, &b.a_blocks);
+  batch_table(c, b.offsets, [&](size_t m) { return persistent_blocks(c, m); }, b.gtab, &b.g_blocks);
+  b.ctrl.alloc(B, st);
+  b.solve_out.alloc(B, st);
+  b.skip_count.alloc(B, st);
+  b.counter.alloc(B, st);
+  b.accum.alloc((size_t)B * kAccum, st);
+  PCLB_CUDA(cudaMemsetAsync(b.skip_count.p, 0, B * sizeof(unsigned long long), st));
+  PCLB_CUDA(cudaMemsetAsync(b.counter.p, 0, B * sizeof(unsigned), st));
+  PCLB_CUDA(cudaMemsetAsync(b.accum.p, 0, (size_t)B * kAccum * sizeof(double), st));
+  b.host.reserve(B * (sizeof(LoopCtrl) + sizeof(unsigned long long)) + sizeof(int));
+  // every problem's loop state as icp_set_source leaves it; a guess that is not the identity moves its queries once
+  icp_reset_state(s, nullptr);
+  b.loop.assign(B, s.loop);
+  b.total_skipped.assign(B, 0);
+  const int mode = transform_mode(s.P);
+  std::vector<Pending> h(B);
+  bool any_guess = false;
+  for (int p = 0; p < B; ++p) {
+    if (guesses)
+      for (int i = 0; i < 16; ++i)
+        b.loop[p].final_T[i] = s.P.scalar_is_double ? guesses[16 * p + i] : (double)(float)guesses[16 * p + i];
+    const bool moved = !is_identity(b.loop[p].final_T);
+    any_guess = any_guess || moved;
+    h[p] = make_pending(b.loop[p].final_T, mode, moved ? 1 : 0);
+  }
+  b.pending.alloc(B, st);
+  PCLB_CUDA(cudaMemcpyAsync(b.pending.p, h.data(), B * sizeof(Pending), cudaMemcpyHostToDevice, st));
+  if (any_guess) {
+    k_transform_batch<<<persistent_blocks(c, n), 256, 0, st>>>(s.cur.p, n, b.d_offsets.p, B, b.pending.p, s.cur_normals.p);
+    ++c.launches;
+  }
+  for (int p = 0; p < B; ++p)
+    h[p] = make_pending(b.loop[p].last_T, mode, 0);
+  PCLB_CUDA(cudaMemcpyAsync(b.pending.p, h.data(), B * sizeof(Pending), cudaMemcpyHostToDevice, st));
+  PCLB_CUDA(cudaGetLastError());
+}
+
+// icp_iterate of every problem of the batch at once: every stage one launch, the per-problem loop states read back once
+// per call (the symmetric objective: once per iteration, as icp_iterate does)
+void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats)
+{
+  Ctx& c = *s.ctx;
+  cudaStream_t st = c.stream;
+  IcpBatch& b = s.batch;
+  const int B = b.B;
+  PCLB_REQUIRE(B > 0, PCLB200_ERR_INVALID, "icp: iterate_batch needs a batch source (set_source_batch)");
+  check_batch_session(s);
+  PCLB_REQUIRE(s.P.estimator == PCLB200_EST_SVD || s.tgt_normals.p, PCLB200_ERR_INVALID,
+               "icp: point-to-plane needs target normals");
+  PCLB_REQUIRE(s.P.estimator != PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS || s.cur_normals.p, PCLB200_ERR_INVALID,
+               "icp: the symmetric objective needs source normals (choose the estimator before set_source_batch)");
+  int budget = 0;
+  for (int p = 0; p < B; ++p)
+    if (b.loop[p].state == PCLB200_CONV_NOT_CONVERGED && max_steps > 0)
+      budget = std::max(budget, std::max(1, s.P.max_iterations - b.loop[p].iterations));
+  if (budget > 0) {
+    const int track_mode = s.P.track_mode;
+    const CritParams crit = crit_params(s, track_mode);
+    const Index& F = target_frame(s);
+    LoopCtrl* h_ctrl = static_cast<LoopCtrl*>(b.host.p);
+    unsigned long long* h_skipped = reinterpret_cast<unsigned long long*>(h_ctrl + B);
+    int* h_err = reinterpret_cast<int*>(h_skipped + B);
+    for (int p = 0; p < B; ++p) {
+      LoopCtrl& L = b.loop[p];
+      if (L.state == PCLB200_CONV_NOT_CONVERGED) {
+        if (track_mode != PCLB200_TRACK_AUTO)
+          L.track_next = track_mode == PCLB200_TRACK_ON ? 1 : 0;
+        if (L.iterations == 0)
+          for (int r = 0; r < 3; ++r)
+            L.origin[r] = 0.5f * (F.lo[r] + F.hi[r]);
+      }
+      h_ctrl[p] = L;
+      if (L.state != PCLB200_CONV_NOT_CONVERGED)
+        h_ctrl[p].done = 1;  // its blocks return at once
+    }
+    PCLB_CUDA(cudaMemcpyAsync(b.ctrl.p, h_ctrl, B * sizeof(LoopCtrl), cudaMemcpyHostToDevice, st));
+    if (s.P.estimator == PCLB200_EST_SVD) {
+      k_seed_origin_batch<<<grid_for(B, 256), 256, 0, st>>>(s.cur.p, b.d_offsets.p, B, b.ctrl.p);
+      ++c.launches;
+    }
+    const bool sym = s.P.estimator == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS;
+    const size_t part_words = sym ? (size_t)b.g_blocks * kAccum : (size_t)b.a_blocks * 128;
+    if (b.partials.n < part_words)
+      b.partials.alloc(part_words, st);
+    auto read_back = [&]() {
+      PCLB_CUDA(cudaMemcpyAsync(h_ctrl, b.ctrl.p, B * sizeof(LoopCtrl), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaMemcpyAsync(h_skipped, b.skip_count.p, B * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaMemcpyAsync(h_err, c.d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
+      PCLB_CUDA(cudaStreamSynchronize(st));
+      if (*h_err)
+        raise_device_error(c, *h_err);
+      bool all_done = true;
+      for (int p = 0; p < B; ++p) {
+        if (b.loop[p].state == PCLB200_CONV_NOT_CONVERGED) {  // the others' states stay as they were
+          b.loop[p] = h_ctrl[p];
+          b.total_skipped[p] = (int64_t)h_skipped[p];
+        }
+        all_done = all_done && h_ctrl[p].done;
+      }
+      return all_done;
+    };
+    IterArgs a = loop_args(s, track_mode);
+    a.pending = b.pending.p;
+    a.partials = b.partials.p;
+    a.partials2 = b.partials.p;
+    a.counter = b.counter.p;
+    a.accum = b.accum.p;
+    a.skip_count = b.skip_count.p;
+    a.ctrl = b.ctrl.p;
+    const int n_enq = std::min(max_steps, budget);
+    for (int k = 0; k < n_enq; ++k) {
+      {
+        ProfScope ps(c, "icp_search");
+        if (track_mode != PCLB200_TRACK_ON) {
+          k_search_batch<false><<<(unsigned)b.wtab.n, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p);
+          ++c.launches;
+        }
+        if (track_mode != PCLB200_TRACK_OFF) {
+          k_search_batch<true><<<(unsigned)b.wtab.n, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p);
+          ++c.launches;
+        }
+      }
+      {
+        ProfScope ps(c, "icp_accum");
+        if (s.P.estimator == PCLB200_EST_SVD)
+          k_accum_dmma_batch<PCLB200_EST_SVD><<<(unsigned)b.atab.n, 256, 0, st>>>(a, b.atab.p, s.match.p);
+        else if (s.P.estimator == PCLB200_EST_POINT_TO_PLANE_LLS)
+          k_accum_dmma_batch<PCLB200_EST_POINT_TO_PLANE_LLS><<<(unsigned)b.atab.n, 256, 0, st>>>(a, b.atab.p, s.match.p);
+        else
+          k_accum_batch<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS><<<(unsigned)b.gtab.n, 256, 0, st>>>(a, b.gtab.p, s.match.p);
+        ++c.launches;
+      }
+      {
+        ProfScope ps(c, "solve");
+        k_solve_batch<<<grid_for((size_t)B * 32, 256), 256, 0, st>>>(b.accum.p, B, s.P.estimator, s.P.scalar_is_double,
+                                                                     transform_mode(s.P), b.pending.p, b.solve_out.p,
+                                                                     s.P.svd_no_umeyama, b.ctrl.p, crit);
+        ++c.launches;
+      }
+      PCLB_CUDA(cudaGetLastError());
+      if (sym && read_back())
+        break;
+    }
+    if (!sym)
+      read_back();
+  }
+  if (stats)
+    for (int p = 0; p < B; ++p)
+      fill_stats(b.loop[p], b.total_skipped[p], stats + p);
+}
+
+void icp_get_correspondences_batch(Icp& s, pclb200_corr* out, int64_t* counts)
+{
+  Ctx& c = *s.ctx;
+  cudaStream_t st = c.stream;
+  const IcpBatch& b = s.batch;
+  const int B = b.B;
+  PCLB_REQUIRE(B > 0, PCLB200_ERR_INVALID, "icp: get_correspondences_batch needs a batch source (set_source_batch)");
+  const size_t n = s.n_q;
+  DevBuf<pclb200_corr> by_slot;
+  by_slot.alloc(n, st);
+  k_matches_to_corr<<<grid_for(n, 256), 256, 0, st>>>(s.cur.p, s.match.p, n, s.tgt->pts.p, b.rel.p, by_slot.p);
+  std::vector<int> live(B);
+  for (int p = 0; p < B; ++p)
+    live[p] = b.loop[p].iterations > 0;
+  DevBuf<int> d_live;
+  DevBuf<unsigned long long> d_counts;
+  d_live.alloc(B, st);
+  d_counts.alloc(B, st);
+  PCLB_CUDA(cudaMemcpyAsync(d_live.p, live.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
+  PCLB_CUDA(cudaMemsetAsync(d_counts.p, 0, B * sizeof(unsigned long long), st));
+  k_mask_and_count<<<grid_for(n, 256), 256, 0, st>>>(by_slot.p, n, b.d_offsets.p, B, d_live.p, d_counts.p);
+  c.launches += 2;
+  PCLB_CUDA(cudaGetLastError());
+  std::vector<unsigned long long> h(B);
+  compact_corr_to(c, by_slot.p, n, out);  // synchronises: live has reached the device
+  PCLB_CUDA(cudaMemcpyAsync(h.data(), d_counts.p, B * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  PCLB_CUDA(cudaStreamSynchronize(st));
+  for (int p = 0; p < B; ++p)
+    counts[p] = (int64_t)h[p];
+}
+
 // output = *input_ ; transformCloud(*input_, output, final_transformation_) — icp.hpp:265-267
 void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, size_t stride_n)
 {
@@ -1118,6 +1517,16 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
   PCLB_REQUIRE(s.src_all.p, PCLB200_ERR_INVALID, "icp: no source");
   const bool do_n = out_normals && s.have_src_normals;
   const int mode = transform_mode(s.P);
+  // a batch: every record moves by its own problem's final transform
+  const IcpBatch& b = s.batch;
+  DevBuf<Pending> finals;
+  if (b.B) {
+    std::vector<Pending> h(b.B);
+    for (int p = 0; p < b.B; ++p)
+      h[p] = make_pending(b.loop[p].final_T, mode, 1);
+    finals.alloc(b.B, st);
+    PCLB_CUDA(cudaMemcpyAsync(finals.p, h.data(), b.B * sizeof(Pending), cudaMemcpyHostToDevice, st));
+  }
   const bool normals_inside =
       do_n && s.src_normal_off >= 0 &&
       static_cast<unsigned char*>(out_normals) - static_cast<unsigned char*>(out_pts) == s.src_normal_off && stride_n == stride_out;
@@ -1128,9 +1537,13 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
     const int vec = stride_out % 16 == 0 && reinterpret_cast<uintptr_t>(d_rec) % 16 == 0;  // src_raw is 16-aligned
     {
       ProfScope ps(c, "transform_out");
-      k_assemble_records<<<grid_for(s.n_all, 256), 256, 0, st>>>(s.src_raw.p, s.n_all, stride_out,
-                                                                 do_n ? (int)(s.src_normal_off / 4) : -1,
-                                                                 make_pending(s.loop.final_T, mode, 1), vec, d_rec);
+      const int nrm_word = do_n ? (int)(s.src_normal_off / 4) : -1;
+      if (b.B)
+        k_assemble_records_batch<<<grid_for(s.n_all, 256), 256, 0, st>>>(s.src_raw.p, s.n_all, stride_out, nrm_word,
+                                                                         b.d_offsets.p, b.B, finals.p, vec, d_rec);
+      else
+        k_assemble_records<<<grid_for(s.n_all, 256), 256, 0, st>>>(s.src_raw.p, s.n_all, stride_out, nrm_word,
+                                                                   make_pending(s.loop.final_T, mode, 1), vec, d_rec);
       ++c.launches;
     }
     PCLB_CUDA(cudaGetLastError());
@@ -1151,7 +1564,13 @@ void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, 
   }
   {
     ProfScope ps(c, "transform_out");
-    transform_on_device(c, s.loop.final_T, mode, tmp.p, s.n_all, do_n ? tmpn.p : nullptr);
+    if (b.B) {
+      k_transform_batch<<<persistent_blocks(c, s.n_all), 256, 0, st>>>(tmp.p, s.n_all, b.d_offsets.p, b.B, finals.p,
+                                                                       do_n ? tmpn.p : nullptr);
+      ++c.launches;
+    }
+    else
+      transform_on_device(c, s.loop.final_T, mode, tmp.p, s.n_all, do_n ? tmpn.p : nullptr);
   }
   auto write_back = [&](const DevBuf<float4>& d, void* out, size_t stride, int write_w, float w) {
     if (stride == 16 && write_w) {

@@ -328,8 +328,8 @@ __device__ __forceinline__ int dmma_accum_source(int est, int k)
 
 // warp tiles -> block (fixed order) -> grid (fixed order, last block) -> the kAccum layout k_solve reads -> peers.
 // Must be called by every thread of every block; blockDim.x = NWARPS * 32 >= 128.
-template <int EST, int NWARPS>
-__device__ __forceinline__ void fold_tiles_and_publish(const IterArgs& a, double c1a, double c1b, double w)
+template <int EST, int NWARPS, class G>
+__device__ __forceinline__ void fold_tiles_and_publish(const IterArgs& a, double c1a, double c1b, double w, const G& grid)
 {
   __shared__ double s_tiles[NWARPS][128];
   __shared__ double s_fin[128];
@@ -349,7 +349,7 @@ __device__ __forceinline__ void fold_tiles_and_publish(const IterArgs& a, double
       s_tiles[warp][64 + g * 8] = v;
   }
   __syncthreads();
-  if (!grid_fold<128, 128>(&s_tiles[0][0], NWARPS, a.partials2, a.counter, is_last, s_fin))
+  if (!grid_fold<128, 128>(&s_tiles[0][0], NWARPS, a.partials2, a.counter, is_last, s_fin, grid))
     return;
   __syncthreads();
   if (threadIdx.x < kAccum) {
@@ -367,9 +367,11 @@ __device__ __forceinline__ void fold_tiles_and_publish(const IterArgs& a, double
 // lbs (TRACK only): per query, a lower bound on the DISTANCE to every target point other than the match; 0 = unknown.
 // 5 blocks of 256 threads per SM (<= 48 registers).  The walk is a chain of dependent loads that occupancy hides, but at
 // 6 blocks (40 registers) the visitor and walk state spill inside the node loop; on H100 the 5-block build is 6 % faster.
-template <bool RECIP, bool TRACK>
-__global__ void __launch_bounds__(256, 5)
-k_search(const IterArgs a, Match* __restrict__ match, float* __restrict__ lbs)
+// search_queries: the body, over the queries of this block's place in `grid` (grid_sum.cuh: k_search runs on the
+// launch's grid, k_search_batch on one problem's grid inside the batch launch)
+template <bool RECIP, bool TRACK, class G>
+__device__ __forceinline__ void search_queries(const IterArgs& a, Match* __restrict__ match, float* __restrict__ lbs,
+                                               const G& grid)
 {
   if (a.ctrl) {  // enqueued ahead of the host: a finished loop, or the other TRACK flavour, leaves nothing to do
     if (a.ctrl->done || (a.track_sel && (a.ctrl->track_next != 0) != TRACK))
@@ -388,8 +390,8 @@ k_search(const IterArgs a, Match* __restrict__ match, float* __restrict__ lbs)
 #ifdef PCLB_STATS
   unsigned my_nodes = 0;
 #endif
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t base = blockIdx.x * (size_t)blockDim.x + (threadIdx.x & ~31); base < a.n; base += stride) {
+  const size_t stride = (size_t)grid.blocks() * blockDim.x;
+  for (size_t base = grid.block() * (size_t)blockDim.x + (threadIdx.x & ~31); base < a.n; base += stride) {
     const size_t i = base + lane;
     const bool in_range = i < a.n;
     float4 p = in_range ? a.cur[i] : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -491,22 +493,28 @@ k_search(const IterArgs a, Match* __restrict__ match, float* __restrict__ lbs)
     atomicExch(a.d_error, kErrStackOverflow);
 }
 
+template <bool RECIP, bool TRACK>
+__global__ void __launch_bounds__(256, 5)
+k_search(const IterArgs a, Match* __restrict__ match, float* __restrict__ lbs)
+{
+  search_queries<RECIP, TRACK>(a, match, lbs, HwGrid());
+}
+
 // Streaming accumulation on the fp64 tensor cores: one pass over (source point, match) pairs, the normal equations
 // built by pair_rows + mma_rows.  The kernel is bound by the latency of match -> gather: resident warps are what hides
 // it (two pairs in flight per thread at half the occupancy was slower), so the state is kept to ten fp64 registers of
 // accumulators per lane instead of 29 per thread.
-template <int EST>
-__global__ void __launch_bounds__(256, kAccumBlocksPerSM)
-k_accum_dmma(const IterArgs a, const Match* __restrict__ match)
+template <int EST, class G>
+__device__ __forceinline__ void accum_dmma_pairs(const IterArgs& a, const Match* __restrict__ match, const G& grid)
 {
   if (a.ctrl && a.ctrl->done)
     return;
   __shared__ __align__(16) float s_stage[8][2 * 32 * 8];
   const int lane = threadIdx.x & 31;
   double ca = 0.0, cb = 0.0, da = 0.0, db = 0.0, w = 0.0;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  const size_t stride = (size_t)grid.blocks() * blockDim.x;
   float* tiles = s_stage[threadIdx.x >> 5];
-  for (size_t base = blockIdx.x * (size_t)blockDim.x + (threadIdx.x & ~31); base < a.n; base += stride) {
+  for (size_t base = grid.block() * (size_t)blockDim.x + (threadIdx.x & ~31); base < a.n; base += stride) {
     const size_t i = base + lane;
     Match m;
     m.pos = -1;
@@ -520,7 +528,14 @@ k_accum_dmma(const IterArgs a, const Match* __restrict__ match)
     pair_rows<EST>(a, m, p, ra, rb);
     mma_rows<EST>(a, tiles, lane, ra, rb, ca, cb, da, db, w);
   }
-  fold_tiles_and_publish<EST, 8>(a, ca + da, cb + db, w);
+  fold_tiles_and_publish<EST, 8>(a, ca + da, cb + db, w, grid);
+}
+
+template <int EST>
+__global__ void __launch_bounds__(256, kAccumBlocksPerSM)
+k_accum_dmma(const IterArgs a, const Match* __restrict__ match)
+{
+  accum_dmma_pairs<EST>(a, match, HwGrid());
 }
 
 // One pair's terms of the normal equations (slot layout at the top of this file), added to acc[2..): p source point, q
@@ -586,9 +601,8 @@ __device__ __forceinline__ void add_pair_terms(double* acc, const float4& p, con
 
 // The symmetric objective inside the loop (the other estimators run on k_accum_dmma): one streaming pass over (source
 // point, match) pairs, per-thread fp64 sums, fixed reduction order.
-template <int EST>
-__global__ void __launch_bounds__(256)
-k_accum(const IterArgs a, const Match* __restrict__ match)
+template <int EST, class G>
+__device__ __forceinline__ void accum_pairs(const IterArgs& a, const Match* __restrict__ match, const G& grid)
 {
   static_assert(EST == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS, "the other estimators accumulate in k_accum_dmma");
   if (a.ctrl && a.ctrl->done)
@@ -597,7 +611,7 @@ k_accum(const IterArgs a, const Match* __restrict__ match)
 #pragma unroll
   for (int t = 0; t < kAccLls; ++t)
     acc[t] = 0.0;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < a.n; i += (size_t)gridDim.x * blockDim.x) {
+  for (size_t i = grid.block() * (size_t)blockDim.x + threadIdx.x; i < a.n; i += (size_t)grid.blocks() * blockDim.x) {
     const Match m = match[i];
     if (!match_accepted(m))
       continue;
@@ -609,8 +623,15 @@ k_accum(const IterArgs a, const Match* __restrict__ match)
     const float4 n1 = a.cur_normals[i];
     add_pair_terms<EST>(acc, p, q, float3{}, n2, n1, a.enforce_same_dir);
   }
-  if (block_reduce_and_publish<kAccLls>(acc, GridSum{a.partials, a.counter, a.accum}))
+  if (block_reduce_and_publish<kAccLls>(acc, GridSum{a.partials, a.counter, a.accum}, grid))
     peer_exchange(a);
+}
+
+template <int EST>
+__global__ void __launch_bounds__(256)
+k_accum(const IterArgs a, const Match* __restrict__ match)
+{
+  accum_pairs<EST>(a, match, HwGrid());
 }
 
 // ---- accumulation over an explicit correspondence list (stand-alone estimators) ------------------------
@@ -845,170 +866,15 @@ __global__ void k_solve(const double* __restrict__ accum, int est, int scalar_is
 {
   if (threadIdx.x != 0 || blockIdx.x != 0)
     return;
-  if (ctrl && ctrl->done)
-    return;
-  const double n = accum[0];
-  out->n = n;
-  out->sum_d = accum[1];
-  double T[16];
-  for (int i = 0; i < 16; ++i)
-    T[i] = (i % 5 == 0) ? 1.0 : 0.0;
-  bool ok = n >= (double)min_corr;
-  if (ok && est == PCLB200_EST_SVD) {
-    const double inv_n = 1.0 / n;
-    const double mp[3] = {accum[2] * inv_n, accum[3] * inv_n, accum[4] * inv_n};
-    const double mq[3] = {accum[5] * inv_n, accum[6] * inv_n, accum[7] * inv_n};
-    double sig[9];
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c)
-        sig[3 * r + c] = accum[8 + 3 * r + c] * inv_n - mq[r] * mp[c];
-    double U[9], sv[3], V[9];
-    double R[9];
-    if (svd_correlation) {
-      double H[9];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c)
-          H[3 * r + c] = sig[3 * c + r] * n;
-      svd3_dev(H, U, sv, V);
-      if (det3_dev(U) * det3_dev(V) < 0.0)
-        for (int x = 0; x < 3; ++x)
-          V[3 * x + 2] = -V[3 * x + 2];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) {
-          double a = 0.0;
-          for (int k = 0; k < 3; ++k)
-            a += V[3 * r + k] * U[3 * c + k];
-          R[3 * r + c] = a;
-        }
-    }
-    else {
-      svd3_dev(sig, U, sv, V);
-      double S[3] = {1.0, 1.0, 1.0};
-      if (det3_dev(U) * det3_dev(V) < 0.0)
-        S[2] = -1.0;
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) {
-          double a = 0.0;
-          for (int k = 0; k < 3; ++k)
-            a += U[3 * r + k] * S[k] * V[3 * c + k];
-          R[3 * r + c] = a;
-        }
-    }
-    double o[3] = {0.0, 0.0, 0.0};
-    if (origin)
-      for (int r = 0; r < 3; ++r)
-        o[r] = origin[r];
-    for (int r = 0; r < 3; ++r) {
-      for (int c = 0; c < 3; ++c)
-        T[4 * r + c] = R[3 * r + c];
-      T[4 * r + 3] = (mq[r] + o[r]) - (R[3 * r] * (mp[0] + o[0]) + R[3 * r + 1] * (mp[1] + o[1]) +
-                                       R[3 * r + 2] * (mp[2] + o[2]));
-    }
-    if (ctrl)  // the next iteration's pairs lie about where this one's did
-      for (int r = 0; r < 3; ++r)
-        ctrl->origin[r] = (float)(mq[r] + o[r]);
-  }
-  else if (ok) {
-    double A[6][7];
-    int t = 2;
-    for (int r = 0; r < 6; ++r)
-      for (int c = r; c < 6; ++c) {
-        A[r][c] = accum[t];
-        A[c][r] = accum[t];
-        ++t;
-      }
-    for (int r = 0; r < 6; ++r)
-      A[r][6] = accum[23 + r];
-    double x[6];
-    if (!solve6_dev(A, x))
-      for (int i = 0; i < 6; ++i)
-        x[i] = __longlong_as_double(0x7ff8000000000000LL);
-    const double al = x[0], be = x[1], ga = x[2];
-    for (int i = 0; i < 16; ++i)
-      T[i] = 0.0;
-    if (est == PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS) {
-      // T = Rz Ry Rx * translation * Rz Ry Rx = [R R | R t]  (symmetric_point_to_plane_lls.hpp:128-147)
-      const double ca = cos(al), sa = sin(al), cb = cos(be), sb = sin(be), cg = cos(ga), sg = sin(ga);
-      const double Rm[9] = {cg * cb, cg * sb * sa - sg * ca, cg * sb * ca + sg * sa,
-                            sg * cb, sg * sb * sa + cg * ca, sg * sb * ca - cg * sa,
-                            -sb,     cb * sa,                cb * ca};
-      for (int r = 0; r < 3; ++r) {
-        for (int cc = 0; cc < 3; ++cc)
-          T[4 * r + cc] = Rm[3 * r] * Rm[cc] + Rm[3 * r + 1] * Rm[3 + cc] + Rm[3 * r + 2] * Rm[6 + cc];
-        T[4 * r + 3] = Rm[3 * r] * x[3] + Rm[3 * r + 1] * x[4] + Rm[3 * r + 2] * x[5];
-      }
-      T[15] = 1.0;
-    }
-    else {
-    T[0] = cos(ga) * cos(be);
-    T[1] = -sin(ga) * cos(al) + cos(ga) * sin(be) * sin(al);
-    T[2] = sin(ga) * sin(al) + cos(ga) * sin(be) * cos(al);
-    T[4] = sin(ga) * cos(be);
-    T[5] = cos(ga) * cos(al) + sin(ga) * sin(be) * sin(al);
-    T[6] = -cos(ga) * sin(al) + sin(ga) * sin(be) * cos(al);
-    T[8] = -sin(be);
-    T[9] = cos(be) * sin(al);
-    T[10] = cos(be) * cos(al);
-    T[3] = x[3];
-    T[7] = x[4];
-    T[11] = x[5];
-    T[15] = 1.0;
-    }
-  }
-  if (!scalar_is_double)
-    for (int i = 0; i < 16; ++i)
-      T[i] = (double)(float)T[i];
-  for (int i = 0; i < 16; ++i)
-    out->T[i] = T[i];
-  out->ok = ok ? 1 : 0;
-  if (pending) {
-    for (int i = 0; i < 12; ++i) {
-      pending->f[i] = (float)T[i];
-      pending->d[i] = T[i];
-    }
-    pending->apply = ok ? 1 : 0;
-    pending->mode = mode;
-  }
-  if (ctrl) {
-    // the tail of one pass of the do-while at icp.hpp:164-241, in the caller's Scalar
-    LoopCtrl& L = *ctrl;
-    ++L.n_run;
-    L.n_corr = n;
-    L.total_corr += (long long)n;
-    L.mse = n > 0 ? accum[1] / n : 0.0;
-    const int tracked = L.track_next;
-    if (!ok) {  // icp.hpp:204-213
-      L.state = PCLB200_CONV_NO_CORRESPONDENCES;
-      L.converged = 0;
-      L.done = 1;
-    }
-    else {
-      for (int i = 0; i < 16; ++i)
-        L.last_T[i] = T[i];
-      if (scalar_is_double)
-        mat4_mul_dev<double>(L.last_T, L.final_T, L.final_T);
-      else
-        mat4_mul_dev<float>(L.last_T, L.final_T, L.final_T);
-      ++L.iterations;
-      L.converged = (scalar_is_double ? has_converged_dev<double>(L, crit, L.last_T) : has_converged_dev<float>(L, crit, L.last_T)) ? 1 : 0;
-      if (L.state != PCLB200_CONV_NOT_CONVERGED)
-        L.done = 1;
-      // tracking pays once the cloud has almost stopped moving: upper bound of the displacement T_k causes anywhere
-      // near the target, |R - I|_F * r_max + |t|, against half the RMS correspondence distance
-      double rf = 0.0, tn = 0.0;
-      for (int r = 0; r < 3; ++r) {
-        for (int cc = 0; cc < 3; ++cc) {
-          const double d = T[4 * r + cc] - (r == cc ? 1.0 : 0.0);
-          rf += d * d;
-        }
-        tn += T[4 * r + 3] * T[4 * r + 3];
-      }
-      const double disp = sqrt(rf) * crit.rmax + sqrt(tn);
-      L.track_next = crit.track_mode == PCLB200_TRACK_ON ? 1
-                     : crit.track_mode == PCLB200_TRACK_OFF ? 0 : (disp < 0.5 * sqrt(fmax(L.mse, 0.0)) ? 1 : 0);
-    }
-    L.lb_valid = tracked;  // the search of THIS iteration wrote the bounds iff it was a TRACK search
-  }
+#include "solve_body.inc"
+}
+
+// k_solve of one problem of a batch (k_solve_batch): the same body on the problem's own accumulators and loop state
+__device__ __forceinline__ void solve_one(const double* __restrict__ accum, int est, int scalar_is_double, int mode,
+                                          const float* origin, int min_corr, Pending* pending, SolveOut* out,
+                                          int svd_correlation, LoopCtrl* ctrl, const CritParams& crit)
+{
+#include "solve_body.inc"
 }
 
 // An origin of the SVD sums (slot layout at the top of this file): the first finite point of pts, or of
@@ -1021,6 +887,125 @@ __global__ void k_seed_origin(const float4* __restrict__ pts, const pclb200_corr
       out[0] = p.x;
       out[1] = p.y;
       out[2] = p.z;
+      return;
+    }
+  }
+}
+
+// ---- a batch of problems in one loop (icp.cu: icp_iterate_batch) ------------------------------------------------------
+// B problems share the target and the parameters; problem p owns the queries [begin, begin + n) of `cur` (each problem's
+// queries in the order its own session stages them), and slot p of the per-problem arrays that IterArgs points to in a
+// batch: pending, ctrl (its origin is the problem's SVD origin), skip_count, counter, accum (kAccum each).  Every stage is
+// one launch: the grid each problem's single align would launch is laid end to end with the others', and a table tells
+// each block its problem and its place in that problem's grid.  A block works for one problem only, so the per-block
+// tests (done, the tracking flavour) and the shared Pending stay what they are in a single align, and the fixed-order
+// grid sum runs over the problem's own partials in its own block order: the same fp64 sums, bit for bit.
+struct BatchBlock {
+  int problem;
+  unsigned vblock, vgrid;  // this block's place in the problem's grid
+  unsigned part;           // the problem's first partials slot (blocks before it, over all problems)
+  unsigned long long begin, n;  // the problem's queries
+};
+
+// the block table of a grid of grid(n_p) blocks per problem p, laid end to end (off: B + 1 record offsets); each problem's
+// partials slots start at its first block's place in the table
+template <typename Grid>
+inline std::vector<BatchBlock> batch_blocks(const std::vector<long long>& off, Grid grid)
+{
+  std::vector<BatchBlock> h;
+  for (size_t p = 0; p + 1 < off.size(); ++p) {
+    const size_t n = (size_t)(off[p + 1] - off[p]);
+    const unsigned g = grid(n), part = (unsigned)h.size();
+    for (unsigned v = 0; v < g; ++v)
+      h.push_back(BatchBlock{(int)p, v, g, part, (unsigned long long)off[p], (unsigned long long)n});
+  }
+  return h;
+}
+
+// a's per-problem pointers narrowed to the problem of block b
+__device__ __forceinline__ IterArgs problem_args(const IterArgs& a, const BatchBlock& b)
+{
+  IterArgs p = a;
+  p.cur = a.cur + b.begin;
+  p.n = b.n;
+  if (a.cur_normals)
+    p.cur_normals = a.cur_normals + b.begin;
+  p.pending = a.pending + b.problem;
+  p.ctrl = a.ctrl + b.problem;
+  p.origin = p.ctrl->origin;
+  p.skip_count = a.skip_count + b.problem;
+  p.partials = a.partials + (size_t)b.part * kAccum;
+  p.partials2 = a.partials2 + (size_t)b.part * 128;
+  p.counter = a.counter + b.problem;
+  p.accum = a.accum + (size_t)b.problem * kAccum;
+  return p;
+}
+
+template <bool TRACK>
+__global__ void __launch_bounds__(256, 5)
+k_search_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, Match* __restrict__ match, float* __restrict__ lbs)
+{
+  const BatchBlock b = blocks[blockIdx.x];
+  search_queries<false, TRACK>(problem_args(a, b), match + b.begin, lbs + b.begin, VirtualGrid{b.vblock, b.vgrid});
+}
+
+template <int EST>
+__global__ void __launch_bounds__(256, kAccumBlocksPerSM)
+k_accum_dmma_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, const Match* __restrict__ match)
+{
+  const BatchBlock b = blocks[blockIdx.x];
+  accum_dmma_pairs<EST>(problem_args(a, b), match + b.begin, VirtualGrid{b.vblock, b.vgrid});
+}
+
+template <int EST>
+__global__ void __launch_bounds__(256)
+k_accum_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, const Match* __restrict__ match)
+{
+  const BatchBlock b = blocks[blockIdx.x];
+  accum_pairs<EST>(problem_args(a, b), match + b.begin, VirtualGrid{b.vblock, b.vgrid});
+}
+
+// one warp per problem (lane 0 solves): k_solve of each problem on its own accumulators and loop state
+__global__ void k_solve_batch(const double* __restrict__ accum, int n_problems, int est, int scalar_is_double, int mode,
+                              Pending* pending, SolveOut* out, int svd_correlation, LoopCtrl* ctrl, CritParams crit)
+{
+  const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+  const int p = (int)(t >> 5);
+  if ((t & 31) || p >= n_problems)
+    return;
+  solve_one(accum + (size_t)p * kAccum, est, scalar_is_double, mode, ctrl[p].origin, 3, pending + p, out + p,
+            svd_correlation, ctrl + p, crit);
+}
+
+// the problem of record / query i: offsets[p] <= i < offsets[p + 1]
+__host__ __device__ __forceinline__ int problem_of(const long long* offsets, int n_problems, long long i)
+{
+  int lo = 0, hi = n_problems - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (offsets[mid] <= i)
+      lo = mid;
+    else
+      hi = mid - 1;
+  }
+  return lo;
+}
+
+// k_seed_origin of every problem that has not run an iteration yet, one thread per problem, into its loop state
+__global__ void k_seed_origin_batch(const float4* __restrict__ cur, const long long* __restrict__ offsets, int n_problems,
+                                    LoopCtrl* ctrl)
+{
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_problems || ctrl[p].iterations != 0 || ctrl[p].done)
+    return;
+  const float4* q = cur + offsets[p];
+  const size_t n = (size_t)(offsets[p + 1] - offsets[p]);
+  for (size_t i = 0; i < n; ++i) {
+    const float4 v = q[i];
+    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
+      ctrl[p].origin[0] = v.x;
+      ctrl[p].origin[1] = v.y;
+      ctrl[p].origin[2] = v.z;
       return;
     }
   }
