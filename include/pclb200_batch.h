@@ -1,11 +1,13 @@
-/* pclb200_batch.h — C-ABI of libpclb200.so for a batch of ICP problems against one target in one session: a queue of
- * scans against one prior map, or one scan from many initial guesses.  Every stage of an iteration is one launch for the
- * whole batch, however many problems it holds, and the loop state of every problem comes back in one read.
+/* pclb200_batch.h — C-ABI of libpclb200.so for a batch of ICP problems in one session: a queue of scans against one
+ * prior map, one scan from many initial guesses (one target for all problems), or many independent scan pairs such as
+ * the consecutive scans of an odometry sequence or the edges of a pose graph (pclb200_icp_set_target_batch: one target
+ * per problem).  Every stage of an iteration is one launch for the whole batch, however many problems and targets it
+ * holds, and the loop state of every problem comes back in one read.
  *
  * The entry points follow every convention of include/pclb200.h (status codes, host-or-device arrays, strides, squared
  * fp32 distances, row-major transforms).  They live in their own header because they have no counterpart in the
  * reference's API and the PCL facade (pcl_b200/pcl_compat/) does not reach them.  The target is the session's
- * (pclb200_icp_set_target); no entry point here takes an index.
+ * (pclb200_icp_set_target), or one per problem (pclb200_icp_set_target_batch).
  *
  * Problem p is bit for bit what a fresh session with the same parameters, target and target normals would do after
  * pclb200_icp_set_source(its records, its guess) and the same sequence of max_steps: every pclb200_icp_stats field
@@ -24,6 +26,23 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
+
+/* Problem p of the next set_source_batch is registered against targets[p] (and tgt_normals[p]) instead of the session's
+ * single target: problem p is bit for bit a fresh session after pclb200_icp_set_target(targets[p], tgt_normals[p],
+ * stride_n) + pclb200_icp_set_source(its records, its guess) and the same max_steps.  A handle may repeat.
+ *
+ * targets: host, n_targets handles, kept alive by the caller as with pclb200_icp_set_target.  tgt_normals (host, nullable;
+ * entries nullable): one array per problem, one normal per point of the cloud its index was built from, host or device,
+ * all with stride stride_n.  set_target_batch drops whatever source the session held, so iterate_batch refuses until
+ * set_source_batch runs again (the query order depends on the targets' frames); set_source_batch then refuses unless
+ * n_problems == n_targets.  pclb200_icp_set_source refuses while the session holds a target batch;
+ * pclb200_icp_set_target puts the session back to one target (and drops a source staged for the batch).
+ * PCLB200_ERR_INVALID, with the session left as it was, for n_targets outside 1 to 65536, a NULL array or NULL handle,
+ * an index on another device than the session, point-to-plane or the symmetric objective when some problem has no
+ * target normals, and the refusals in the header comment. */
+PCLB200_API int pclb200_icp_set_target_batch(pclb200_icp* icp, const pclb200_index* const* targets,
+                                             const void* const* tgt_normals /* nullable; entries nullable */,
+                                             size_t stride_n, int32_t n_targets);
 
 /* B = n_problems problems, problem p being the records [offsets[p], offsets[p+1]) of src (offsets: host, B + 1 entries,
  * offsets[0] = 0, strictly increasing, offsets[B] = n); src_normals (nullable) as in pclb200_icp_set_source.  guesses

@@ -86,7 +86,7 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_validate_transformation_sharded", "pclb200_inliers_sharded", "pclb200_radius_sharded",
                    "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
 # every symbol include/pclb200_batch.h declares (a batch of ICP problems in one session; tests/test_icp_batch_symbols.py)
-BATCH_SYMBOLS = ["pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch"]
+BATCH_SYMBOLS = ["pclb200_icp_set_target_batch", "pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch"]
 
 _lib = None
 
@@ -181,6 +181,7 @@ def lib():
     L.pclb200_comm_export.argtypes = [vp, vp]
     L.pclb200_comm_import.argtypes = [vp, C.c_int, C.c_int, vp]
     L.pclb200_comm_init.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.pclb200_icp_set_target_batch.argtypes = [vp, vp, vp, sz, C.c_int32]
     L.pclb200_icp_set_source_batch.argtypes = [vp, vp, sz, sz, vp, sz, vp, C.c_int32, dp]
     L.pclb200_icp_iterate_batch.argtypes = [vp, C.c_int, vp]
     L.pclb200_icp_get_correspondences_batch.argtypes = [vp, vp, vp]
@@ -949,6 +950,19 @@ class Icp:
         m = C.c_size_t()
         _check(lib().pclb200_icp_get_correspondences(self.h, C.c_void_p(out.ctypes.data), C.byref(m)))
         return out[:m.value]
+
+    def set_target_batch(self, indices, normals=None):
+        """One target per problem of the next set_source_batch: problem p runs as a session after set_target(indices[p],
+        normals[p]) would, bit for bit.  normals: None or a list of B arrays (or None entries) of one stride."""
+        B = len(indices)
+        handles = (C.c_void_p * max(B, 1))(*[None if i is None else i.h for i in indices])
+        bufs = [None if x is None else _Buf(x) for x in normals] if normals is not None else []
+        strides = {b.stride for b in bufs if b is not None}
+        if len(strides) > 1:
+            raise ValueError("set_target_batch: every normals array must have the same row stride")
+        nptr = (C.c_void_p * max(B, 1))(*[None if b is None else b.ptr for b in bufs]) if normals is not None else None
+        _check(lib().pclb200_icp_set_target_batch(self.h, handles, nptr, strides.pop() if strides else 0, B))
+        self._keep = [list(indices), bufs]
 
     def set_source_batch(self, src, offsets, normals=None, guesses=None):
         """B problems against the session's target, problem p = records offsets[p]:offsets[p+1] of src (B + 1 offsets);

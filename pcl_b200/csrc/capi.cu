@@ -26,6 +26,8 @@ void icp_iterate(Icp& s, int max_steps, pclb200_icp_stats* stats);
 void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
                           const int64_t* offsets, int n_problems, const double* guesses);
 void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats);
+void icp_set_target_batch(Icp& s, const Index* const* targets, const void* const* tgt_normals, size_t stride_n,
+                          int n_targets);
 void icp_get_correspondences_batch(Icp& s, pclb200_corr* out, int64_t* counts);
 void icp_get_cloud(Icp& s, void* out_pts, size_t stride_out, void* out_normals, size_t stride_n);
 size_t icp_get_correspondences(Icp& s, pclb200_corr* out);
@@ -719,6 +721,21 @@ int pclb200_icp_set_source_batch(pclb200_icp* icp, const void* src, size_t n, si
 {
   return on_ctx(icp, [&](Icp& s) {
     icp_set_source_batch(s, src, n, stride, src_normals, stride_n, offsets, n_problems, guesses);
+  });
+}
+
+int pclb200_icp_set_target_batch(pclb200_icp* icp, const pclb200_index* const* targets, const void* const* tgt_normals,
+                                 size_t stride_n, int32_t n_targets)
+{
+  return on_ctx(icp, [&](Icp& s) {
+    PCLB_REQUIRE(targets, PCLB200_ERR_INVALID, "NULL argument");
+    PCLB_REQUIRE(n_targets >= 1 && n_targets <= 65536, PCLB200_ERR_INVALID, "icp: a batch holds 1 to 65536 problems");
+    std::vector<const Index*> idx(n_targets);
+    for (int p = 0; p < n_targets; ++p) {
+      PCLB_REQUIRE(targets[p] && targets[p]->idx, PCLB200_ERR_INVALID, "NULL argument");
+      idx[p] = targets[p]->idx;
+    }
+    icp_set_target_batch(s, idx.data(), tgt_normals, stride_n, n_targets);
   });
 }
 

@@ -274,6 +274,16 @@ struct IcpBatch {
   PinnedBuf host;                    // B loop states, B skip counts, the device error flag
 };
 
+// a batch of scan pairs (icp_set_target_batch): problem p of the next batch source is registered against idx[p]
+struct IcpTargets {
+  int B = 0;                            // 0: the session's one target (Icp::tgt)
+  std::vector<const Index*> idx;        // problem -> its index (kept alive by the caller)
+  bool all_normals = false;             // every problem's target normals were given
+  std::vector<DevBuf<float4>> normals;  // normals_by_pos of each distinct (index, normals) pair
+  DevBuf<BatchTarget> table;            // problem -> its target (icp_kernels.cuh)
+  DevBuf<float4> frames;                // problem -> {lo, morton_scale} of its index: the frame of its query order
+};
+
 struct Icp {
   Ctx* ctx = nullptr;
   pclb200_icp_params P;
@@ -319,6 +329,7 @@ struct Icp {
   // operation): counters, DefaultConvergenceCriteria state, final / last transform, tracking decision
   LoopCtrl loop;
   IcpBatch batch;
+  IcpTargets targets;
 };
 
 static void set_identity(double* T)
@@ -562,8 +573,14 @@ static void stage_target_normals(Icp& s, const Index* idx, const void* tgt_norma
     normals_by_pos(*s.ctx, idx, tgt_normals, stride_n, s.tgt_normals);
 }
 
+static void drop_source(Icp& s);
+
 void icp_set_target(Icp& s, const Index* idx, const void* tgt_normals, size_t stride_n)
 {
+  if (s.targets.B) {  // a source staged for a batch of targets is ordered in their frames, not in this one's
+    drop_source(s);
+    s.targets = IcpTargets();
+  }
   s.tgt = idx;
   s.sharded_target = false;
   stage_target_normals(s, idx, tgt_normals, stride_n);
@@ -766,7 +783,7 @@ __global__ void k_gather_subset(const float4* __restrict__ all, const int32_t* _
 
 // The caller's records into the session (src_all, src_raw) and their queries into qb, in the order of the target frame.
 static void stage_source(Icp& s, const void* src, size_t n, size_t stride, const void* src_normals, size_t stride_n,
-                         const int32_t* indices, size_t n_idx, QueryBatch& qb)
+                         const int32_t* indices, size_t n_idx, QueryBatch* qb)
 {
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
@@ -807,7 +824,7 @@ static void stage_source(Icp& s, const void* src, size_t n, size_t stride, const
   s.src_orig.release();
   {
     ProfScope ps(c, "query_sort");
-    stage_records(c, target_frame(s), recs, n, stride, copy, dense, indices ? nullptr : &qb);
+    stage_records(c, target_frame(s), recs, n, stride, copy, dense, indices ? nullptr : qb);
     if (indices) {
       // index subset: the queries are gathered from the staged points and sorted on their own
       s.src_orig.alloc(n_idx, st);
@@ -818,7 +835,7 @@ static void stage_source(Icp& s, const void* src, size_t n, size_t stride, const
         k_gather_subset<<<grid_for(n_idx, 256), 256, 0, st>>>(s.src_all.p, s.src_orig.p, n_idx, sub.p);
         ++c.launches;
       }
-      make_query_batch(c, target_frame(s), sub.p, s.n_q, qb);
+      make_query_batch(c, target_frame(s), sub.p, s.n_q, *qb);
     }
   }
 }
@@ -879,9 +896,12 @@ void icp_set_source(Icp& s, const void* src, size_t n, size_t stride, const void
   PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
   PCLB_REQUIRE(src != nullptr && n > 0, PCLB200_ERR_INVALID, "icp: empty source");
   PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
+  PCLB_REQUIRE(!s.targets.B, PCLB200_ERR_INVALID,
+               "icp: a session holding a batch of targets takes a batch source (set_source_batch); set_target returns it "
+               "to one target");
   s.batch = IcpBatch();
   QueryBatch qb;
-  stage_source(s, src, n, stride, src_normals, stride_n, indices, n_idx, qb);
+  stage_source(s, src, n, stride, src_normals, stride_n, indices, n_idx, &qb);
   finish_source(s, qb, src_normals, stride_n);
   icp_reset_state(s, guess);
   // icp.hpp:125-134: a non-identity guess is applied once, before the first search
@@ -909,6 +929,17 @@ static void fill_stats(const LoopCtrl& L, int64_t total_skipped, pclb200_icp_sta
   }
 }
 
+// CritParams::rmax of the frame F
+static double frame_rmax(const Index& F)
+{
+  double rmax = 0.0;
+  for (int r = 0; r < 3; ++r) {
+    const double m = std::max(std::fabs((double)F.lo[r]), std::fabs((double)F.hi[r]));
+    rmax += m * m;
+  }
+  return std::sqrt(rmax);
+}
+
 // what DefaultConvergenceCriteria and the tracking decision of k_solve read
 static CritParams crit_params(const Icp& s, int track_mode)
 {
@@ -922,13 +953,7 @@ static CritParams crit_params(const Icp& s, int track_mode)
   crit.trans_eps = s.P.transformation_epsilon;
   crit.rel_mse = s.P.euclidean_fitness_epsilon;
   crit.abs_mse = s.P.mse_threshold_absolute;
-  const Index& F = target_frame(s);
-  double rmax = 0.0;
-  for (int r = 0; r < 3; ++r) {
-    const double m = std::max(std::fabs((double)F.lo[r]), std::fabs((double)F.hi[r]));
-    rmax += m * m;
-  }
-  crit.rmax = std::sqrt(rmax);
+  crit.rmax = frame_rmax(target_frame(s));
   return crit;
 }
 
@@ -1240,17 +1265,106 @@ __global__ void k_mask_and_count(pclb200_corr* __restrict__ by_slot, size_t n, c
     by_slot[i].index_match = -1;
 }
 
-// what a batch refuses (include/pclb200_batch.h), checked by set_source_batch and by every iterate_batch
-static void check_batch_session(const Icp& s)
+// k_matches_to_corr of a batch of scan pairs: each match is a position in its own problem's target
+__global__ void k_matches_to_corr_targets(const float4* __restrict__ cur, const Match* __restrict__ match, size_t n,
+                                          const long long* __restrict__ offsets, int n_problems,
+                                          const BatchTarget* __restrict__ targets, const int32_t* __restrict__ rel,
+                                          pclb200_corr* __restrict__ by_slot)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const int slot = __float_as_int(cur[i].w);
+  const Match m = match[i];
+  pclb200_corr r;
+  r.index_query = rel[slot];
+  const bool acc = match_accepted(m);
+  r.index_match = acc ? __float_as_int(targets[problem_of(offsets, n_problems, slot)].pts[m.pos].w) : -1;
+  r.distance = acc ? m.d2 : 0.f;
+  by_slot[slot] = r;
+}
+
+// what a batch refuses (include/pclb200_batch.h), checked by set_target_batch, set_source_batch and every iterate_batch
+static void check_batch_params(const Icp& s)
 {
   Ctx& c = *s.ctx;
-  PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
-  PCLB_REQUIRE(!comm_active(c) && !s.sharded_target, PCLB200_ERR_INVALID,
-               "icp: a batch runs on one GPU: no communicator, no sharded target");
+  PCLB_REQUIRE(!comm_active(c), PCLB200_ERR_INVALID, "icp: a batch runs on one GPU: no communicator, no sharded target");
   PCLB_REQUIRE(s.rejectors.empty(), PCLB200_ERR_INVALID, "icp: a batch takes no rejector chain");
   PCLB_REQUIRE(!s.P.use_reciprocal, PCLB200_ERR_INVALID, "icp: a batch takes no reciprocal correspondences");
   PCLB_REQUIRE(s.P.correspondence_kind == PCLB200_CORR_NEAREST, PCLB200_ERR_INVALID,
                "icp: a batch takes nearest-neighbour correspondences only");
+}
+
+static void check_batch_session(const Icp& s)
+{
+  PCLB_REQUIRE(s.tgt != nullptr, PCLB200_ERR_INVALID, "icp: no target set (registration.hpp:77-81)");
+  PCLB_REQUIRE(!s.sharded_target, PCLB200_ERR_INVALID, "icp: a batch runs on one GPU: no communicator, no sharded target");
+  check_batch_params(s);
+}
+
+// the session without a source (its batch read-back buffer kept: freeing pinned memory synchronises the device)
+static void drop_source(Icp& s)
+{
+  PinnedBuf host = std::move(s.batch.host);
+  s.batch = IcpBatch();
+  s.batch.host = std::move(host);
+  s.cur.release();
+  s.src_all.release();
+  s.src_raw.release();
+  s.match.release();
+  s.n_all = s.n_q = 0;
+}
+
+void icp_set_target_batch(Icp& s, const Index* const* targets, const void* const* tgt_normals, size_t stride_n,
+                          int n_targets)
+{
+  Ctx& c = *s.ctx;
+  cudaStream_t st = c.stream;
+  PCLB_REQUIRE(n_targets >= 1 && n_targets <= 65536, PCLB200_ERR_INVALID, "icp: a batch holds 1 to 65536 problems");
+  check_batch_params(s);
+  const int B = n_targets;
+  for (int p = 0; p < B; ++p)
+    PCLB_REQUIRE(targets[p]->device == c.device, PCLB200_ERR_INVALID, "icp: a target index lives on another device");
+  bool all_normals = tgt_normals != nullptr;
+  for (int p = 0; all_normals && p < B; ++p)
+    all_normals = tgt_normals[p] != nullptr;
+  PCLB_REQUIRE(s.P.estimator == PCLB200_EST_SVD || all_normals, PCLB200_ERR_INVALID,
+               "icp: point-to-plane and the symmetric objective need every problem's target normals");
+  IcpTargets T;
+  T.B = B;
+  T.idx.assign(targets, targets + B);
+  T.all_normals = all_normals;
+  std::vector<BatchTarget> h(B);
+  std::vector<float4> frames(B);
+  std::vector<std::pair<std::pair<const Index*, const void*>, const float4*>> staged;  // one normals_by_pos per pair
+  for (int p = 0; p < B; ++p) {
+    const Index& I = *targets[p];
+    const void* nrm = tgt_normals ? tgt_normals[p] : nullptr;
+    const float4* by_pos = nullptr;
+    if (nrm) {
+      for (const auto& e : staged)
+        if (e.first.first == &I && e.first.second == nrm)
+          by_pos = e.second;
+      if (!by_pos) {
+        T.normals.emplace_back();
+        normals_by_pos(c, &I, nrm, stride_n, T.normals.back());
+        by_pos = T.normals.back().p;
+        staged.push_back({{&I, nrm}, by_pos});
+      }
+    }
+    const TreeView v = tree_view(I);
+    h[p] = BatchTarget{v.nodes, v.pts, by_pos, v.root, v.cells, frame_rmax(I)};
+    frames[p] = make_float4(I.lo[0], I.lo[1], I.lo[2], I.morton_scale);
+  }
+  T.table.alloc(B, st);
+  T.frames.alloc(B, st);
+  PCLB_CUDA(cudaMemcpyAsync(T.table.p, h.data(), B * sizeof(BatchTarget), cudaMemcpyHostToDevice, st));
+  PCLB_CUDA(cudaMemcpyAsync(T.frames.p, frames.data(), B * sizeof(float4), cudaMemcpyHostToDevice, st));
+  drop_source(s);
+  s.targets = std::move(T);
+  s.tgt = targets[0];
+  s.sharded_target = false;
+  s.tgt_normals.release();
 }
 
 // batch_blocks's table (icp_kernels.cuh) on the device; *slots = its blocks (partials slots)
@@ -1281,6 +1395,9 @@ void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, cons
                  "icp: batch offsets must increase strictly (every problem holds a record)");
   PCLB_REQUIRE(s.P.estimator != PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS || src_normals, PCLB200_ERR_INVALID,
                "icp: the symmetric objective needs source normals");
+  const bool per_target = s.targets.B > 0;
+  PCLB_REQUIRE(!per_target || n_problems == s.targets.B, PCLB200_ERR_INVALID,
+               "icp: a batch source holds one problem per target of set_target_batch");
   const int B = n_problems;
   PinnedBuf host = std::move(s.batch.host);  // kept across batches: freeing pinned memory synchronises the device
   s.batch = IcpBatch();
@@ -1290,12 +1407,15 @@ void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, cons
   b.offsets.assign(offsets, offsets + B + 1);
   b.d_offsets.alloc(B + 1, st);
   PCLB_CUDA(cudaMemcpyAsync(b.d_offsets.p, b.offsets.data(), (B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  // the queries of all problems in the order of the target frame (stable), then by problem (stable): within each
-  // problem the order make_query_batch gives that problem alone; w = the record's index in the batch
+  // the queries of all problems in the order of the target frame (a batch of targets: each in its own target's frame)
+  // (stable), then by problem (stable): within each problem the order make_query_batch gives that problem alone; w = the
+  // record's index in the batch
   QueryBatch qb;
-  stage_source(s, src, n, stride, src_normals, stride_n, nullptr, 0, qb);
+  stage_source(s, src, n, stride, src_normals, stride_n, nullptr, 0, per_target ? nullptr : &qb);
   {
     ProfScope ps(c, "query_sort");
+    if (per_target)  // src_all holds the staged xyz
+      make_query_batch_framed(c, s.targets.frames.p, b.d_offsets.p, B, s.src_all.p, n, qb);
     DevBuf<unsigned> keys_in, keys;
     DevBuf<int32_t> vals_in, vals;
     keys_in.alloc(n, st);
@@ -1374,8 +1494,10 @@ void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats)
   const int B = b.B;
   PCLB_REQUIRE(B > 0, PCLB200_ERR_INVALID, "icp: iterate_batch needs a batch source (set_source_batch)");
   check_batch_session(s);
-  PCLB_REQUIRE(s.P.estimator == PCLB200_EST_SVD || s.tgt_normals.p, PCLB200_ERR_INVALID,
-               "icp: point-to-plane needs target normals");
+  const IcpTargets& TB = s.targets;
+  const BatchTarget* targets = TB.B ? TB.table.p : nullptr;  // null: every problem against the session's target
+  PCLB_REQUIRE(s.P.estimator == PCLB200_EST_SVD || (targets ? TB.all_normals : s.tgt_normals.p != nullptr),
+               PCLB200_ERR_INVALID, "icp: point-to-plane needs target normals");
   PCLB_REQUIRE(s.P.estimator != PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS || s.cur_normals.p, PCLB200_ERR_INVALID,
                "icp: the symmetric objective needs source normals (choose the estimator before set_source_batch)");
   int budget = 0;
@@ -1385,7 +1507,6 @@ void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats)
   if (budget > 0) {
     const int track_mode = s.P.track_mode;
     const CritParams crit = crit_params(s, track_mode);
-    const Index& F = target_frame(s);
     LoopCtrl* h_ctrl = static_cast<LoopCtrl*>(b.host.p);
     unsigned long long* h_skipped = reinterpret_cast<unsigned long long*>(h_ctrl + B);
     int* h_err = reinterpret_cast<int*>(h_skipped + B);
@@ -1394,6 +1515,7 @@ void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats)
       if (L.state == PCLB200_CONV_NOT_CONVERGED) {
         if (track_mode != PCLB200_TRACK_AUTO)
           L.track_next = track_mode == PCLB200_TRACK_ON ? 1 : 0;
+        const Index& F = targets ? *TB.idx[p] : target_frame(s);
         if (L.iterations == 0)
           for (int r = 0; r < 3; ++r)
             L.origin[r] = 0.5f * (F.lo[r] + F.hi[r]);
@@ -1440,30 +1562,46 @@ void icp_iterate_batch(Icp& s, int max_steps, pclb200_icp_stats* stats)
     for (int k = 0; k < n_enq; ++k) {
       {
         ProfScope ps(c, "icp_search");
+        const unsigned g = (unsigned)b.wtab.n;
         if (track_mode != PCLB200_TRACK_ON) {
-          k_search_batch<false><<<(unsigned)b.wtab.n, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p);
+          if (targets)
+            k_search_batch<false, true><<<g, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p, targets);
+          else
+            k_search_batch<false><<<g, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p);
           ++c.launches;
         }
         if (track_mode != PCLB200_TRACK_OFF) {
-          k_search_batch<true><<<(unsigned)b.wtab.n, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p);
+          if (targets)
+            k_search_batch<true, true><<<g, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p, targets);
+          else
+            k_search_batch<true><<<g, 256, 0, st>>>(a, b.wtab.p, s.match.p, s.lb.p);
           ++c.launches;
         }
       }
       {
         ProfScope ps(c, "icp_accum");
-        if (s.P.estimator == PCLB200_EST_SVD)
-          k_accum_dmma_batch<PCLB200_EST_SVD><<<(unsigned)b.atab.n, 256, 0, st>>>(a, b.atab.p, s.match.p);
-        else if (s.P.estimator == PCLB200_EST_POINT_TO_PLANE_LLS)
-          k_accum_dmma_batch<PCLB200_EST_POINT_TO_PLANE_LLS><<<(unsigned)b.atab.n, 256, 0, st>>>(a, b.atab.p, s.match.p);
+        const unsigned ag = (unsigned)b.atab.n, gg = (unsigned)b.gtab.n;
+        constexpr int kSvd = PCLB200_EST_SVD, kPlane = PCLB200_EST_POINT_TO_PLANE_LLS,
+                      kSym = PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS;
+        if (s.P.estimator == kSvd && targets)
+          k_accum_dmma_batch<kSvd, true><<<ag, 256, 0, st>>>(a, b.atab.p, s.match.p, targets);
+        else if (s.P.estimator == kSvd)
+          k_accum_dmma_batch<kSvd><<<ag, 256, 0, st>>>(a, b.atab.p, s.match.p);
+        else if (s.P.estimator == kPlane && targets)
+          k_accum_dmma_batch<kPlane, true><<<ag, 256, 0, st>>>(a, b.atab.p, s.match.p, targets);
+        else if (s.P.estimator == kPlane)
+          k_accum_dmma_batch<kPlane><<<ag, 256, 0, st>>>(a, b.atab.p, s.match.p);
+        else if (targets)
+          k_accum_batch<kSym, true><<<gg, 256, 0, st>>>(a, b.gtab.p, s.match.p, targets);
         else
-          k_accum_batch<PCLB200_EST_SYMMETRIC_POINT_TO_PLANE_LLS><<<(unsigned)b.gtab.n, 256, 0, st>>>(a, b.gtab.p, s.match.p);
+          k_accum_batch<kSym><<<gg, 256, 0, st>>>(a, b.gtab.p, s.match.p);
         ++c.launches;
       }
       {
         ProfScope ps(c, "solve");
         k_solve_batch<<<grid_for((size_t)B * 32, 256), 256, 0, st>>>(b.accum.p, B, s.P.estimator, s.P.scalar_is_double,
                                                                      transform_mode(s.P), b.pending.p, b.solve_out.p,
-                                                                     s.P.svd_no_umeyama, b.ctrl.p, crit);
+                                                                     s.P.svd_no_umeyama, b.ctrl.p, crit, targets);
         ++c.launches;
       }
       PCLB_CUDA(cudaGetLastError());
@@ -1488,7 +1626,11 @@ void icp_get_correspondences_batch(Icp& s, pclb200_corr* out, int64_t* counts)
   const size_t n = s.n_q;
   DevBuf<pclb200_corr> by_slot;
   by_slot.alloc(n, st);
-  k_matches_to_corr<<<grid_for(n, 256), 256, 0, st>>>(s.cur.p, s.match.p, n, s.tgt->pts.p, b.rel.p, by_slot.p);
+  if (s.targets.B)
+    k_matches_to_corr_targets<<<grid_for(n, 256), 256, 0, st>>>(s.cur.p, s.match.p, n, b.d_offsets.p, B,
+                                                                s.targets.table.p, b.rel.p, by_slot.p);
+  else
+    k_matches_to_corr<<<grid_for(n, 256), 256, 0, st>>>(s.cur.p, s.match.p, n, s.tgt->pts.p, b.rel.p, by_slot.p);
   std::vector<int> live(B);
   for (int p = 0; p < B; ++p)
     live[p] = b.loop[p].iterations > 0;

@@ -922,6 +922,17 @@ inline std::vector<BatchBlock> batch_blocks(const std::vector<long long>& off, G
   return h;
 }
 
+// A batch of scan pairs (icp.cu: icp_set_target_batch): problem p's own target, everything its single session derives
+// from its index.  The one-target batch reads the target from IterArgs instead (TARGETS = false below).
+struct BatchTarget {
+  const BvhNode* nodes;
+  const float4* pts;
+  const float4* normals;  // normals_by_pos of the problem's index (nullable: SVD)
+  int root;
+  CellTable cells;
+  double rmax;            // CritParams::rmax of the problem's target frame
+};
+
 // a's per-problem pointers narrowed to the problem of block b
 __device__ __forceinline__ IterArgs problem_args(const IterArgs& a, const BatchBlock& b)
 {
@@ -941,54 +952,64 @@ __device__ __forceinline__ IterArgs problem_args(const IterArgs& a, const BatchB
   return p;
 }
 
-template <bool TRACK>
+// ... and, with TARGETS, its target read from the problem's record of the table
+template <bool TARGETS>
+__device__ __forceinline__ IterArgs problem_args(const IterArgs& a, const BatchBlock& b, const BatchTarget* targets)
+{
+  IterArgs p = problem_args(a, b);
+  if (TARGETS) {
+    const BatchTarget& t = targets[b.problem];
+    p.nodes = t.nodes;
+    p.pts = t.pts;
+    p.tgt_normals = t.normals;
+    p.root = t.root;
+    p.cells = t.cells;
+  }
+  return p;
+}
+
+template <bool TRACK, bool TARGETS = false>
 __global__ void __launch_bounds__(256, 5)
-k_search_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, Match* __restrict__ match, float* __restrict__ lbs)
+k_search_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, Match* __restrict__ match, float* __restrict__ lbs,
+               const BatchTarget* __restrict__ targets = nullptr)
 {
   const BatchBlock b = blocks[blockIdx.x];
-  search_queries<false, TRACK>(problem_args(a, b), match + b.begin, lbs + b.begin, VirtualGrid{b.vblock, b.vgrid});
+  search_queries<false, TRACK>(problem_args<TARGETS>(a, b, targets), match + b.begin, lbs + b.begin,
+                               VirtualGrid{b.vblock, b.vgrid});
 }
 
-template <int EST>
+template <int EST, bool TARGETS = false>
 __global__ void __launch_bounds__(256, kAccumBlocksPerSM)
-k_accum_dmma_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, const Match* __restrict__ match)
+k_accum_dmma_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, const Match* __restrict__ match,
+                   const BatchTarget* __restrict__ targets = nullptr)
 {
   const BatchBlock b = blocks[blockIdx.x];
-  accum_dmma_pairs<EST>(problem_args(a, b), match + b.begin, VirtualGrid{b.vblock, b.vgrid});
+  accum_dmma_pairs<EST>(problem_args<TARGETS>(a, b, targets), match + b.begin, VirtualGrid{b.vblock, b.vgrid});
 }
 
-template <int EST>
+template <int EST, bool TARGETS = false>
 __global__ void __launch_bounds__(256)
-k_accum_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, const Match* __restrict__ match)
+k_accum_batch(const IterArgs a, const BatchBlock* __restrict__ blocks, const Match* __restrict__ match,
+              const BatchTarget* __restrict__ targets = nullptr)
 {
   const BatchBlock b = blocks[blockIdx.x];
-  accum_pairs<EST>(problem_args(a, b), match + b.begin, VirtualGrid{b.vblock, b.vgrid});
+  accum_pairs<EST>(problem_args<TARGETS>(a, b, targets), match + b.begin, VirtualGrid{b.vblock, b.vgrid});
 }
 
-// one warp per problem (lane 0 solves): k_solve of each problem on its own accumulators and loop state
+// one warp per problem (lane 0 solves): k_solve of each problem on its own accumulators and loop state; targets
+// (nullable): each problem's rmax replaces crit's
 __global__ void k_solve_batch(const double* __restrict__ accum, int n_problems, int est, int scalar_is_double, int mode,
-                              Pending* pending, SolveOut* out, int svd_correlation, LoopCtrl* ctrl, CritParams crit)
+                              Pending* pending, SolveOut* out, int svd_correlation, LoopCtrl* ctrl, CritParams crit,
+                              const BatchTarget* __restrict__ targets = nullptr)
 {
   const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
   const int p = (int)(t >> 5);
   if ((t & 31) || p >= n_problems)
     return;
+  if (targets)
+    crit.rmax = targets[p].rmax;
   solve_one(accum + (size_t)p * kAccum, est, scalar_is_double, mode, ctrl[p].origin, 3, pending + p, out + p,
             svd_correlation, ctrl + p, crit);
-}
-
-// the problem of record / query i: offsets[p] <= i < offsets[p + 1]
-__host__ __device__ __forceinline__ int problem_of(const long long* offsets, int n_problems, long long i)
-{
-  int lo = 0, hi = n_problems - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (offsets[mid] <= i)
-      lo = mid;
-    else
-      hi = mid - 1;
-  }
-  return lo;
 }
 
 // k_seed_origin of every problem that has not run an iteration yet, one thread per problem, into its loop state

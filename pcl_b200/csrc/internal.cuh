@@ -300,6 +300,24 @@ void make_query_batch(Ctx& c, const Index& ref_frame, const float4* d_q /*n, w i
 // stride == 16) without another pass over them.
 void stage_records(Ctx& c, const Index& ref_frame, const unsigned char* recs, size_t n, size_t stride, unsigned char* copy,
                    float4* dense, QueryBatch* qb);
+// a batch of problems over consecutive ranges of points: the problem of point i, offsets[p] <= i < offsets[p + 1]
+__host__ __device__ __forceinline__ int problem_of(const long long* offsets, int n_problems, long long i)
+{
+  int lo = 0, hi = n_problems - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (offsets[mid] <= i)
+      lo = mid;
+    else
+      hi = mid - 1;
+  }
+  return lo;
+}
+// make_query_batch of the dense points d_q[0..n), each keyed in its own problem's frame (d_offsets: B + 1 entries, device;
+// d_frames: B x {lo, morton_scale}, device).  The queries of one problem keep the order make_query_batch gives them in
+// that problem's frame; the problems interleave until a stable sort by problem follows.
+void make_query_batch_framed(Ctx& c, const float4* d_frames, const long long* d_offsets, int n_problems,
+                             const float4* d_q, size_t n, QueryBatch& out);
 // load_xyz_as_float4 of a caller's query points into `dense` (kept alive: some kernels read it in input order), then
 // make_query_batch over it
 QueryBatch load_queries(Ctx& c, const Index& ref_frame, const void* pts, size_t n, size_t stride, const int32_t* subset,

@@ -433,6 +433,27 @@ __global__ void k_gather_queries(const float4* __restrict__ q, const int32_t* __
   out[j] = make_float4(v.x, v.y, v.z, __int_as_float(slot));
 }
 
+// the queries pts[vals_in[j]] by keys_in (stable: the points of one key cell keep their input order), w = slot
+static void sort_queries(Ctx& c, DevBuf<unsigned>& keys_in, DevBuf<int32_t>& vals_in, const float4* pts, size_t n,
+                         QueryBatch& qb)
+{
+  cudaStream_t s = c.stream;
+  DevBuf<unsigned> keys;
+  DevBuf<int32_t> vals;
+  keys.alloc(n, s);
+  vals.alloc(n, s);
+  size_t tmp_bytes = 0;
+  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, 32, s));
+  DevBuf<unsigned char> tmp;
+  tmp.alloc(tmp_bytes, s);
+  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, 32, s));
+  c.launches += 5;  // onesweep: histogram + one pass per 8-bit digit
+  qb.q.alloc(n, s);
+  k_gather_queries<<<grid_for(n, 256), 256, 0, s>>>(pts, vals.p, n, qb.q.p);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
 void stage_records(Ctx& c, const Index& frame, const unsigned char* recs, size_t n, size_t stride, unsigned char* copy,
                    float4* dense, QueryBatch* qb)
 {
@@ -441,8 +462,8 @@ void stage_records(Ctx& c, const Index& frame, const unsigned char* recs, size_t
     qb->n = n;
   if (n == 0 || !(copy || dense || qb))
     return;
-  DevBuf<unsigned> keys_in, keys;
-  DevBuf<int32_t> vals_in, vals;
+  DevBuf<unsigned> keys_in;
+  DevBuf<int32_t> vals_in;
   if (qb) {
     keys_in.alloc(n, s);
     vals_in.alloc(n, s);
@@ -461,20 +482,24 @@ void stage_records(Ctx& c, const Index& frame, const unsigned char* recs, size_t
   PCLB_CUDA(cudaGetLastError());
   if (!qb)
     return;
-  // stable: the points of one key cell keep their input order
-  keys.alloc(n, s);
-  vals.alloc(n, s);
-  size_t tmp_bytes = 0;
-  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, 32, s));
-  DevBuf<unsigned char> tmp;
-  tmp.alloc(tmp_bytes, s);
-  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, 32, s));
-  c.launches += 5;  // onesweep: histogram + one pass per 8-bit digit
-  qb->q.alloc(n, s);
-  const float4* pts = dense ? dense : reinterpret_cast<const float4*>(recs);
-  k_gather_queries<<<grid_for(n, 256), 256, 0, s>>>(pts, vals.p, n, qb->q.p);
+  sort_queries(c, keys_in, vals_in, dense ? dense : reinterpret_cast<const float4*>(recs), n, *qb);
+}
+
+void make_query_batch_framed(Ctx& c, const float4* d_frames, const long long* d_offsets, int n_problems,
+                             const float4* d_q, size_t n, QueryBatch& out)
+{
+  cudaStream_t s = c.stream;
+  out.n = n;
+  if (n == 0)
+    return;
+  DevBuf<unsigned> keys_in;
+  DevBuf<int32_t> vals_in;
+  keys_in.alloc(n, s);
+  vals_in.alloc(n, s);
+  k_problem_frame_keys<<<grid_for(n, 256), 256, 0, s>>>(d_q, n, d_offsets, n_problems, d_frames, keys_in.p, vals_in.p);
   ++c.launches;
   PCLB_CUDA(cudaGetLastError());
+  sort_queries(c, keys_in, vals_in, d_q, n, out);
 }
 
 void make_query_batch(Ctx& c, const Index& frame, const float4* d_q, size_t n, QueryBatch& out)

@@ -182,6 +182,22 @@ k_stage_records(const U* __restrict__ recs, size_t n, unsigned units, U* __restr
   }
 }
 
+// The key k_stage_records gives point i, in the frame of its own problem instead of one frame for all: a batch of
+// problems over consecutive ranges of pts (offsets: B + 1 entries), frames[p] = {lo[0..2], morton_scale} of problem p's
+// target.  Sorted by these keys and then stably by problem, each problem's points fall in the order its own frame gives.
+__global__ void k_problem_frame_keys(const float4* __restrict__ pts, size_t n, const long long* __restrict__ offsets,
+                                     int n_problems, const float4* __restrict__ frames, unsigned* __restrict__ keys,
+                                     int32_t* __restrict__ vals)
+{
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const float4 f = frames[problem_of(offsets, n_problems, (long long)i)];
+  const float4 v = pts[i];
+  keys[i] = hilbert_key32(v.x, v.y, v.z, f.x, f.y, f.z, f.w);
+  vals[i] = (int32_t)i;
+}
+
 // sorted gather: out[j] = {xyz of slot vals[j], orig index bits}; pads the tail with +inf sentinels
 __global__ void k_gather_sorted(const float4* __restrict__ p, const int32_t* __restrict__ vals,
                                 const int32_t* __restrict__ orig_of_slot, size_t n_valid, size_t n_padded,
