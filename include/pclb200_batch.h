@@ -17,7 +17,9 @@
  * float or double Scalar; with_normals_transform; is_dense = 0; every convergence criterion; tracking OFF / ON / AUTO
  * (AUTO decides per problem); host or device source arrays.  PCLB200_ERR_INVALID, with the session left as it was, for a
  * rejector chain, use_reciprocal, a correspondence_kind other than NEAREST, an active communicator or a sharded target,
- * and the symmetric objective without source normals. */
+ * and the symmetric objective without source normals.
+ *
+ * The targets of such a batch can themselves be built as one batch (pclb200_index_build_batch). */
 #ifndef PCLB200_BATCH_H_
 #define PCLB200_BATCH_H_
 
@@ -63,6 +65,20 @@ PCLB200_API int pclb200_icp_iterate_batch(pclb200_icp* icp, int max_steps, pclb2
  * is what its own session's pclb200_icp_get_correspondences returns: index_query relative to the problem's first
  * record).  out: host or device, capacity n (the batch's records); counts: host, B entries. */
 PCLB200_API int pclb200_icp_get_correspondences_batch(pclb200_icp* icp, pclb200_corr* out, int64_t* counts);
+
+/* A batch of independent indices in one build: cloud c = records [offsets[c], offsets[c+1]) of pts.  out[c] is bit for
+ * bit the handle pclb200_index_build(ctx, its first record, its record count, stride, NULL, 0, &h) would give.  Its result
+ * indices are relative to the cloud's first record.  Each handle is independent: it can be destroyed alone and in any
+ * order, and it is accepted by every entry point that takes an index, pclb200_icp_set_target_batch included.
+ *
+ * pts: host or device, with the stride rules of pclb200_index_build.  offsets: host, n_clouds + 1 entries.  out: host,
+ * n_clouds entries.  Every stage of the build is one launch for the whole batch, and the call synchronises the context's
+ * stream three times, as one single build does.  All or nothing: on any error no handle exists afterwards and every
+ * out[c] is NULL.  PCLB200_ERR_INVALID for n_clouds outside 1 to 65536, a NULL pts, offsets or out, offsets[0] != 0, a
+ * cloud with no records, offsets[n_clouds] != n, n >= 2^31 - 1 or a bad stride; PCLB200_ERR_EMPTY when some cloud has no
+ * finite point (pclb200_last_error names it). */
+PCLB200_API int pclb200_index_build_batch(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
+                                          const int64_t* offsets, int32_t n_clouds, pclb200_index** out);
 
 #ifdef __cplusplus
 }

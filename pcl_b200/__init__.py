@@ -86,7 +86,8 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_validate_transformation_sharded", "pclb200_inliers_sharded", "pclb200_radius_sharded",
                    "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
 # every symbol include/pclb200_batch.h declares (a batch of ICP problems in one session; tests/test_icp_batch_symbols.py)
-BATCH_SYMBOLS = ["pclb200_icp_set_target_batch", "pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch"]
+BATCH_SYMBOLS = ["pclb200_icp_set_target_batch", "pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch",
+                 "pclb200_index_build_batch"]
 
 _lib = None
 
@@ -185,6 +186,7 @@ def lib():
     L.pclb200_icp_set_source_batch.argtypes = [vp, vp, sz, sz, vp, sz, vp, C.c_int32, dp]
     L.pclb200_icp_iterate_batch.argtypes = [vp, C.c_int, vp]
     L.pclb200_icp_get_correspondences_batch.argtypes = [vp, vp, vp]
+    L.pclb200_index_build_batch.argtypes = [vp, vp, sz, sz, vp, C.c_int32, vp]
     for s in SYMBOLS + SHARDED_SYMBOLS + BATCH_SYMBOLS:
         getattr(L, s)  # AttributeError here == header and library disagree
     _lib = L
@@ -299,6 +301,16 @@ class Context:
         ms, n = C.c_double(), C.c_uint64()
         _check(lib().pclb200_profile_get(self.h, name.encode(), C.byref(ms), C.byref(n)))
         return float(ms.value), int(n.value)
+
+    def index_build_batch(self, cloud, offsets):
+        """One Index per cloud, cloud c being the records [offsets[c], offsets[c+1]) of `cloud` (numpy, or a torch tensor on
+        the host or the device), built in one batch: each is bit for bit Index(ctx, that cloud alone) and owns its handle."""
+        b = _Buf(cloud)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        nc = max(off.size - 1, 0)
+        out = (C.c_void_p * max(nc, 1))()
+        _check(lib().pclb200_index_build_batch(self.h, b.ptr, b.rows, b.stride, C.c_void_p(off.ctypes.data), nc, out))
+        return [Index._adopt(self, out[c], off[c + 1] - off[c]) for c in range(nc)]
 
     def comm_init(self, rank, nranks, unique_id_bytes):
         buf = C.create_string_buffer(bytes(unique_id_bytes), 128)
@@ -473,6 +485,15 @@ class Index:
             return
         sb = _Buf(subset, np.int32)
         _check(lib().pclb200_index_build(ctx.h, b.ptr, b.rows, b.stride, sb.ptr, sb.rows, C.byref(self.h)))
+
+    @classmethod
+    def _adopt(cls, ctx, handle, n_cloud):
+        """An Index that owns `handle`, an index of n_cloud records already built on ctx (nothing is rebuilt)."""
+        self = cls.__new__(cls)
+        self.ctx = ctx
+        self.n_cloud = int(n_cloud)
+        self.h = C.c_void_p(handle)
+        return self
 
     def close(self):
         if getattr(self, "h", None):

@@ -390,6 +390,28 @@ int pclb200_index_build_ids(pclb200_ctx* ctx, const void* pts, size_t n, size_t 
   });
 }
 
+int pclb200_index_build_batch(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride, const int64_t* offsets,
+                              int32_t n_clouds, pclb200_index** out)
+{
+  if (out && n_clouds > 0 && n_clouds <= 65536)
+    std::fill(out, out + n_clouds, nullptr);
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(out, PCLB200_ERR_INVALID, "NULL argument");
+    std::vector<std::unique_ptr<Index>> idx;
+    {
+      ProfScope ps(c, "index_build_batch");
+      idx = build_index_batch(c, pts, n, stride, offsets, n_clouds);
+    }
+    std::vector<std::unique_ptr<pclb200_index>> h(n_clouds);
+    for (int k = 0; k < n_clouds; ++k)
+      h[k].reset(new pclb200_index{nullptr});
+    for (int k = 0; k < n_clouds; ++k) {
+      h[k]->idx = idx[k].release();
+      out[k] = h[k].release();
+    }
+  });
+}
+
 int pclb200_index_destroy(pclb200_index* h)
 {
   return guarded([&] {

@@ -256,6 +256,11 @@ struct Index {
 };
 
 Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* subset, size_t n_subset);
+// cloud k = records [offsets[k], offsets[k + 1]) of pts (offsets: host, n_clouds + 1 entries): what build_index makes of
+// each cloud alone, in one build whose every stage is one launch for the whole batch.  All or nothing: throws, with no
+// handle left, on any error.
+std::vector<std::unique_ptr<Index>> build_index_batch(Ctx& c, const void* pts, size_t n, size_t stride,
+                                                      const int64_t* offsets, int n_clouds);
 // point i labelled ids[i] (non-negative, distinct, < 2^31 - 1) instead of i: one tile of a map sharded across ranks
 Index* build_index_ids(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* ids);
 // the faults of the caller's ids d_ids[0..n) (device): kIdOutOfRange (outside [0, 2^31 - 2]) | kIdRepeated; synchronises

@@ -120,15 +120,7 @@ static void morton_sort(Ctx& c, const float4* d_pts, size_t n, SortedCloud& out)
     out.n_valid = (size_t)h.count;
     if (out.n_valid == 0)
       return;
-    float ext = 0.f;
-    for (int d = 0; d < 3; ++d) {
-      out.lo[d] = ord2f(h.lo[d]);
-      out.hi[d] = ord2f(h.hi[d]);
-      ext = std::max(ext, out.hi[d] - out.lo[d]);
-    }
-    out.scale = ext > 0.f ? 2097152.f / ext : 1.f;
-    if (!std::isfinite(out.scale))
-      out.scale = 1.f;
+    morton_frame(h, out.lo, out.hi, out.scale);
   }
   DevBuf<unsigned long long> keys_in;
   DevBuf<int32_t> vals_in;
@@ -247,40 +239,14 @@ static Index* build_from_dense(Ctx& c, const float4* d_pts, size_t n, const int3
     k_fill_sentinels<<<grid_for(n_padded, 256), 256, 0, s>>>(idx->pts.p, n_padded);
     k_scatter_cells<<<grid_for(nv, 256), 256, 0, s>>>(d_pts, sc.vals.p, d_orig_of_slot, nv, leaf_incl.p, leaf_start.p,
                                                       idx->pts.p);
-    // cell table (traverse.cuh: CellTable): levels 1..bmax, bmax = the finest level (<= kCellMaxBits) whose occupied
-    // cells still hold >= 4 indexed points on average — finer levels would mostly map single points.  The number of
-    // entries is known exactly from the prefix-length histogram; the table gets >= 2 slots per entry.
+    // cell table (traverse.cuh: CellTable), sized by the prefix-length histogram (cell_table_plan)
     CellTableW cellw{nullptr, 0, 0, 0};
     if (want_cells) {
-      uint64_t cum = 1, entries = 0;
-      int l = 0, bmax = 0;
-      for (int b = 1; b <= kCellMaxBits; ++b) {
-        for (; l < 3 * b; ++l)
-          cum += h_hist[l];
-        if (cum > (uint64_t)nv / 4)
-          break;
-        bmax = b;
-        entries += cum;
-        idx->cells.occupied[b] = cum;
-      }
-      if (bmax >= 1) {
-        unsigned lg = 6;
-        while (((uint64_t)1 << lg) < 2 * entries)
-          ++lg;
-        idx->cell_slots.alloc((size_t)1 << lg, s);
+      idx->cells = cell_table_plan(h_hist, nv, idx->lo, idx->hi, idx->morton_scale);
+      if (idx->cells.log2_slots) {
+        idx->cell_slots.alloc((size_t)1 << idx->cells.log2_slots, s);
         PCLB_CUDA(cudaMemsetAsync(idx->cell_slots.p, 0, idx->cell_slots.bytes(), s));
-        idx->cells.log2_slots = lg;
-        idx->cells.bmax = bmax;
-        idx->cells.entries = entries;
-        float m = 0.f;
-        for (int d = 0; d < 3; ++d)
-          m = std::max(m, std::max(std::fabs(idx->lo[d]), std::fabs(idx->hi[d])));
-        m = std::max(m, 2097152.f / idx->morton_scale);
-        idx->cells.margin = 2e-6f * m;
-        cellw.slots = reinterpret_cast<unsigned long long*>(idx->cell_slots.p);
-        cellw.shift = 32 - lg;
-        cellw.mask = (1u << lg) - 1u;
-        cellw.bmax = bmax;
+        cellw = cell_table_view(idx->cell_slots.p, idx->cells);
       }
     }
     k_link_cells<<<grid_for(ni, 256), 256, 0, s>>>(nv, kchildren.p, krange.p, keep.p, new_id.p, leaf_incl.p, sc.keys.p,
@@ -311,6 +277,234 @@ Index* build_index(Ctx& c, const void* pts, size_t n, size_t stride, const int32
 Index* build_index_from_device(Ctx& c, const float4* d_pts, size_t n, const int32_t* d_orig, bool cell_table)
 {
   return build_from_dense(c, d_pts, n, d_orig, n, cell_table);
+}
+
+// ---- a batch of clouds in one build ------------------------------------------------------------------------------
+// Cloud c = records [offsets[c], offsets[c + 1]) of one array; each Index is what build_index makes of the cloud alone.
+// Every stage is one launch for the whole batch (lbvh_kernels.cuh: the *_batch kernels run the single build's bodies on
+// each cloud's base pointers), and the host synchronises three times, as one single build does: for the clouds' boxes,
+// for their cuts, and at the end.
+std::vector<std::unique_ptr<Index>> build_index_batch(Ctx& c, const void* pts, size_t n, size_t stride,
+                                                      const int64_t* offsets, int n_clouds)
+{
+  cudaStream_t s = c.stream;
+  PCLB_REQUIRE(n_clouds >= 1 && n_clouds <= 65536, PCLB200_ERR_INVALID, "index_build_batch: a batch holds 1 to 65536 clouds");
+  PCLB_REQUIRE(pts && offsets, PCLB200_ERR_INVALID, "index_build_batch: NULL argument");
+  PCLB_REQUIRE(offsets[0] == 0 && offsets[n_clouds] == (int64_t)n, PCLB200_ERR_INVALID,
+               "index_build_batch: offsets must run from 0 to n");
+  for (int k = 0; k < n_clouds; ++k)
+    PCLB_REQUIRE(offsets[k + 1] > offsets[k], PCLB200_ERR_INVALID,
+                 "index_build_batch: offsets must increase strictly (every cloud holds a record)");
+  PCLB_REQUIRE(n < (size_t)0x7fffffff, PCLB200_ERR_INVALID, "cloud too large for int32 indices");
+  const int B = n_clouds;
+  DevBuf<float4> dense;
+  dense.alloc(n, s);
+  load_xyz_as_float4(c, pts, n, stride, nullptr, 0, dense.p, s);
+
+  // prefix tables of the launches' work spaces, B + 1 entries each: records, tiles, leaves, final nodes, cell-table slots
+  enum { kRecords, kTiles, kLeaves, kNodes, kSlots, kSpaces };
+  std::vector<long long> pre((size_t)kSpaces * (B + 1), 0);
+  auto P = [&](int space) { return pre.data() + (size_t)space * (B + 1); };
+  std::vector<BuildCloud> cl(B);
+  for (int k = 0; k < B; ++k) {
+    cl[k].first = offsets[k];
+    cl[k].n = offsets[k + 1] - offsets[k];
+    P(kRecords)[k + 1] = offsets[k + 1];
+    P(kTiles)[k + 1] = P(kTiles)[k] + (cl[k].n + kBatchTile - 1) / kBatchTile;
+  }
+  DevBuf<long long> d_pre;
+  DevBuf<BuildCloud> d_cl;
+  d_pre.alloc(pre.size(), s);
+  d_cl.alloc(B, s);
+  const long long* d_off = d_pre.p + (size_t)kRecords * (B + 1);
+  const long long* d_tiles = d_pre.p + (size_t)kTiles * (B + 1);
+  PCLB_CUDA(cudaMemcpyAsync(d_pre.p, pre.data(), pre.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+  PCLB_CUDA(cudaMemcpyAsync(d_cl.p, cl.data(), B * sizeof(BuildCloud), cudaMemcpyHostToDevice, s));
+
+  // 1. per cloud: box and finite count -> frame (synchronisation 1)
+  std::vector<BBoxAcc> acc(B);
+  for (auto& a : acc) {
+    for (int d = 0; d < 3; ++d) {
+      a.lo[d] = 0x7fffffff;
+      a.hi[d] = (int)0x80000000;
+    }
+    a.count = 0;
+  }
+  {
+    DevBuf<BBoxAcc> d_acc;
+    d_acc.alloc(B, s);
+    PCLB_CUDA(cudaMemcpyAsync(d_acc.p, acc.data(), B * sizeof(BBoxAcc), cudaMemcpyHostToDevice, s));
+    k_bbox_batch<<<(unsigned)P(kTiles)[B], 256, 0, s>>>(dense.p, d_cl.p, d_tiles, B, d_acc.p);
+    ++c.launches;
+    PCLB_CUDA(cudaMemcpyAsync(acc.data(), d_acc.p, B * sizeof(BBoxAcc), cudaMemcpyDeviceToHost, s));
+    PCLB_CUDA(cudaStreamSynchronize(s));
+  }
+  for (int k = 0; k < B; ++k) {
+    PCLB_REQUIRE(acc[k].count > 0, PCLB200_ERR_EMPTY,
+                 "index_build_batch: cloud " + std::to_string(k) + " has no finite point (kdtree_flann.hpp:124-129)");
+    cl[k].nv = (int)acc[k].count;
+    float hi[3];  // the handle's, filled in step 4
+    morton_frame(acc[k], cl[k].lo, hi, cl[k].scale);
+  }
+  PCLB_CUDA(cudaMemcpyAsync(d_cl.p, cl.data(), B * sizeof(BuildCloud), cudaMemcpyHostToDevice, s));
+
+  // 2. keys in each cloud's frame; sorted by key, then stably by cloud: each cloud's range in its single build's order
+  DevBuf<unsigned long long> keys;
+  DevBuf<int32_t> vals;
+  keys.alloc(n, s);
+  vals.alloc(n, s);
+  DevBuf<unsigned> cloud_of;  // the cloud of each sorted position (the key of the per-cloud scans)
+  cloud_of.alloc(n, s);
+  {
+    DevBuf<unsigned long long> keys_in, keys1;
+    DevBuf<int32_t> vals_in, vals1, pos, perm;
+    DevBuf<unsigned> cloud_in;
+    keys_in.alloc(n, s);
+    keys1.alloc(n, s);
+    vals_in.alloc(n, s);
+    vals1.alloc(n, s);
+    pos.alloc(n, s);
+    perm.alloc(n, s);
+    cloud_in.alloc(n, s);
+    k_morton_batch<<<grid_for(n, 256), 256, 0, s>>>(dense.p, n, d_off, B, d_cl.p, keys_in.p, vals_in.p);
+    size_t tb1 = 0, tb2 = 0;
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb1, keys_in.p, keys1.p, vals_in.p, vals1.p, (int)n, 0, 64, s));
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb2, cloud_in.p, cloud_of.p, pos.p, perm.p, (int)n, 0, 16, s));
+    DevBuf<unsigned char> tmp;
+    tmp.alloc(std::max(tb1, tb2), s);
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb1, keys_in.p, keys1.p, vals_in.p, vals1.p, (int)n, 0, 64, s));
+    k_cloud_of_sorted<<<grid_for(n, 256), 256, 0, s>>>(vals1.p, n, d_off, B, cloud_in.p, pos.p);
+    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb2, cloud_in.p, cloud_of.p, pos.p, perm.p, (int)n, 0, 16, s));
+    k_permute_sorted<<<grid_for(n, 256), 256, 0, s>>>(keys1.p, vals1.p, perm.p, n, d_off, B, keys.p, vals.p);
+    c.launches += 3 + 9 + 3;  // onesweep: histogram + one pass per 8-bit digit
+    PCLB_CUDA(cudaGetLastError());
+  }
+
+  // 3. radix trees, cuts, scans by cloud, prefix histograms -> leaf and node counts (synchronisation 2)
+  const size_t n_tree = n - (size_t)B;  // node scratch: cloud c's at first - c (a cloud of m records has <= m - 1 nodes)
+  DevBuf<int2> kchildren, krange;
+  DevBuf<int> knode_parent, kpoint_parent, keep, new_id, leaf_flag, leaf_incl;
+  DevBuf<unsigned> node_cloud;
+  kchildren.alloc(n_tree, s);
+  krange.alloc(n_tree, s);
+  knode_parent.alloc(n_tree, s);
+  keep.alloc(n_tree, s);
+  new_id.alloc(n_tree, s);
+  node_cloud.alloc(n_tree, s);
+  kpoint_parent.alloc(n, s);
+  leaf_flag.alloc(n, s);
+  leaf_incl.alloc(n, s);
+  PCLB_CUDA(cudaMemsetAsync(leaf_flag.p, 0, leaf_flag.bytes(), s));
+  if (n_tree)
+    PCLB_CUDA(cudaMemsetAsync(keep.p, 0, keep.bytes(), s));
+  k_karras_points_batch<<<grid_for(n, 256), 256, 0, s>>>(keys.p, n, d_off, B, d_cl.p, kchildren.p, knode_parent.p,
+                                                         kpoint_parent.p, krange.p, node_cloud.p);
+  k_mark_cells_batch<<<grid_for(n, 256), 256, 0, s>>>(n, d_off, B, d_cl.p, krange.p, knode_parent.p, kpoint_parent.p,
+                                                      keep.p, leaf_flag.p);
+  {
+    size_t tb = 0, tb2 = 0;
+    PCLB_CUDA(cub::DeviceScan::InclusiveSumByKey(nullptr, tb, cloud_of.p, leaf_flag.p, leaf_incl.p, (int)n, cub::Equality(), s));
+    PCLB_CUDA(cub::DeviceScan::ExclusiveSumByKey(nullptr, tb2, node_cloud.p, keep.p, new_id.p, (int)n_tree, cub::Equality(), s));
+    DevBuf<unsigned char> tmp;
+    tmp.alloc(std::max(tb, tb2), s);
+    PCLB_CUDA(cub::DeviceScan::InclusiveSumByKey(tmp.p, tb, cloud_of.p, leaf_flag.p, leaf_incl.p, (int)n, cub::Equality(), s));
+    if (n_tree)
+      PCLB_CUDA(cub::DeviceScan::ExclusiveSumByKey(tmp.p, tb2, node_cloud.p, keep.p, new_id.p, (int)n_tree, cub::Equality(), s));
+    c.launches += 2 + (n_tree ? 2 : 0);  // init + scan pass of each scan
+  }
+  std::vector<CloudSummary> sum(B);
+  {
+    DevBuf<CloudSummary> d_sum;
+    d_sum.alloc(B, s);
+    PCLB_CUDA(cudaMemsetAsync(d_sum.p, 0, d_sum.bytes(), s));
+    k_prefix_hist_batch<<<(unsigned)P(kTiles)[B], 256, 0, s>>>(keys.p, d_cl.p, d_tiles, B, d_sum.p);
+    k_cut_summary<<<grid_for(B, 256), 256, 0, s>>>(d_cl.p, B, leaf_incl.p, new_id.p, keep.p, d_sum.p);
+    c.launches += 2;
+    PCLB_CUDA(cudaGetLastError());
+    PCLB_CUDA(cudaMemcpyAsync(sum.data(), d_sum.p, B * sizeof(CloudSummary), cudaMemcpyDeviceToHost, s));
+    PCLB_CUDA(cudaStreamSynchronize(s));
+  }
+
+  // 4. the handles: sized and planned by the single build's rules, allocated from the block cache, written in place
+  std::vector<std::unique_ptr<Index>> out(B);
+  for (int k = 0; k < B; ++k) {
+    BuildCloud& C = cl[k];
+    const CloudSummary& S = sum[k];
+    std::unique_ptr<Index> idx(new Index());
+    idx->ctx = &c;
+    idx->device = c.device;
+    idx->n_cloud = (size_t)C.n;
+    idx->n_valid = (size_t)C.nv;
+    morton_frame(acc[k], idx->lo, idx->hi, idx->morton_scale);
+    if (C.nv <= kLeafSize) {
+      idx->n_leaves = 1;
+      idx->root = ~0;
+    }
+    else {
+      PCLB_REQUIRE(S.n_leaves >= 2 && S.n_int == S.n_leaves - 1, PCLB200_ERR_INTERNAL, "LBVH build: inconsistent cell cut");
+      idx->n_leaves = S.n_leaves;
+      idx->root = 0;
+      idx->nodes.alloc(S.n_int, s);
+      idx->node_leaves.alloc(S.n_int, s);
+      if (C.nv >= 256) {
+        idx->cells = cell_table_plan(S.hist, C.nv, idx->lo, idx->hi, idx->morton_scale);
+        if (idx->cells.log2_slots) {
+          idx->cell_slots.alloc((size_t)1 << idx->cells.log2_slots, s);
+          C.cells = cell_table_view(idx->cell_slots.p, idx->cells);
+        }
+      }
+    }
+    idx->pts.alloc((size_t)idx->n_leaves * kLeafSize, s);
+    C.n_leaves = idx->n_leaves;
+    C.n_int = C.nv <= kLeafSize ? 0 : S.n_int;
+    C.pts = idx->pts.p;
+    C.nodes = idx->nodes.p;
+    C.node_leaves = idx->node_leaves.p;
+    C.leaf_first = P(kLeaves)[k];
+    C.node_first = P(kNodes)[k];
+    P(kLeaves)[k + 1] = P(kLeaves)[k] + C.n_leaves;
+    P(kNodes)[k + 1] = P(kNodes)[k] + C.n_int;
+    P(kSlots)[k + 1] = P(kSlots)[k] + (long long)idx->cell_slots.n;
+    out[k] = std::move(idx);
+  }
+  PCLB_CUDA(cudaMemcpyAsync(d_pre.p, pre.data(), pre.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+  PCLB_CUDA(cudaMemcpyAsync(d_cl.p, cl.data(), B * sizeof(BuildCloud), cudaMemcpyHostToDevice, s));
+  const long long* d_leaves = d_pre.p + (size_t)kLeaves * (B + 1);
+  const long long* d_nodes = d_pre.p + (size_t)kNodes * (B + 1);
+  const long long* d_slots = d_pre.p + (size_t)kSlots * (B + 1);
+  const size_t n_leaves = (size_t)P(kLeaves)[B], n_int = (size_t)P(kNodes)[B];
+  DevBuf<int> leaf_start, node_parent, leaf_parent;
+  DevBuf<int2> children;
+  DevBuf<float4> leaf_lo, leaf_hi, node_lo, node_hi;
+  DevBuf<unsigned> flags;
+  leaf_start.alloc(n_leaves, s);
+  leaf_parent.alloc(n_leaves, s);
+  leaf_lo.alloc(n_leaves, s);
+  leaf_hi.alloc(n_leaves, s);
+  node_parent.alloc(n_int, s);
+  children.alloc(n_int, s);
+  node_lo.alloc(n_int, s);
+  node_hi.alloc(n_int, s);
+  flags.alloc(n_int, s);
+  if (n_int)
+    PCLB_CUDA(cudaMemsetAsync(flags.p, 0, flags.bytes(), s));
+  const size_t n_clear = std::max<size_t>(n_leaves * kLeafSize, (size_t)P(kSlots)[B]);
+  k_clear_outputs_batch<<<grid_for(n_clear, 256), 256, 0, s>>>(d_cl.p, B, d_leaves, d_slots);
+  k_gather_small_batch<<<grid_for((size_t)B * kLeafSize, 256), 256, 0, s>>>(dense.p, vals.p, d_cl.p, B);
+  k_leaf_starts_batch<<<grid_for(n, 256), 256, 0, s>>>(n, d_off, B, d_cl.p, leaf_flag.p, leaf_incl.p, leaf_start.p);
+  k_scatter_cells_batch<<<grid_for(n, 256), 256, 0, s>>>(dense.p, vals.p, n, d_off, B, d_cl.p, leaf_incl.p,
+                                                         leaf_start.p);
+  k_link_cells_batch<<<grid_for(n, 256), 256, 0, s>>>(n, d_off, B, d_cl.p, kchildren.p, krange.p, keep.p, new_id.p,
+                                                      leaf_incl.p, keys.p, children.p, node_parent.p, leaf_parent.p);
+  k_refit_batch<<<grid_for(n_leaves, 256), 256, 0, s>>>(d_cl.p, B, d_leaves, children.p, node_parent.p, leaf_parent.p,
+                                                        leaf_lo.p, leaf_hi.p, node_lo.p, node_hi.p, flags.p);
+  if (n_int)
+    k_pack_nodes_batch<<<grid_for(n_int, 256), 256, 0, s>>>(d_cl.p, B, d_nodes, children.p, leaf_lo.p, leaf_hi.p,
+                                                            node_lo.p, node_hi.p);
+  c.launches += 6 + (n_int ? 1 : 0);
+  PCLB_CUDA(cudaGetLastError());
+  PCLB_CUDA(cudaStreamSynchronize(s));  // temporaries are released stream-ordered; surface build errors here
+  return out;
 }
 
 // ---- labelled index: one tile of a map, its points carrying the caller's ids -------------------------------------

@@ -2,8 +2,11 @@
 // sorted points, the cut into cell-aligned leaves, the cell table, bottom-up refit, node packing.  A header so that lbvh.cu
 // stays the host-side driver (CUB sorts and scans between the kernels) and tests/host/lbvh_host_test.cpp can compile the
 // SAME kernels for the host, run the same sequence with std:: algorithms in CUB's place, check the invariants the walks
-// rely on and search the result against brute force.
+// rely on and search the result against brute force.  The *_batch kernels build a batch of clouds in one pass, each
+// cloud through the single build's own code (tests/host/lbvh_batch_host_test.cpp compares them with single builds).
 #pragma once
+#include <cmath>
+
 #include "internal.cuh"
 #include "traverse.cuh"
 
@@ -34,19 +37,9 @@ struct BBoxAcc {
   unsigned long long count;
 };
 
-__global__ void k_bbox(const float4* __restrict__ p, size_t n, BBoxAcc* acc)
+// one thread's box and finite count, folded over its warp and into *acc (lanes that saw no finite point add nothing)
+__device__ __forceinline__ void bbox_publish(float lo[3], float hi[3], unsigned cnt, BBoxAcc* acc)
 {
-  float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-  unsigned cnt = 0;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float4 v = __ldg(p + i);
-    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
-      lo[0] = fminf(lo[0], v.x); hi[0] = fmaxf(hi[0], v.x);
-      lo[1] = fminf(lo[1], v.y); hi[1] = fmaxf(hi[1], v.y);
-      lo[2] = fminf(lo[2], v.z); hi[2] = fmaxf(hi[2], v.z);
-      ++cnt;
-    }
-  }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
@@ -64,6 +57,22 @@ __global__ void k_bbox(const float4* __restrict__ p, size_t n, BBoxAcc* acc)
     }
     atomicAdd(&acc->count, (unsigned long long)cnt);
   }
+}
+
+__global__ void k_bbox(const float4* __restrict__ p, size_t n, BBoxAcc* acc)
+{
+  float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+  unsigned cnt = 0;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    float4 v = __ldg(p + i);
+    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
+      lo[0] = fminf(lo[0], v.x); hi[0] = fmaxf(hi[0], v.x);
+      lo[1] = fminf(lo[1], v.y); hi[1] = fmaxf(hi[1], v.y);
+      lo[2] = fminf(lo[2], v.z); hi[2] = fmaxf(hi[2], v.z);
+      ++cnt;
+    }
+  }
+  bbox_publish(lo, hi, cnt, acc);
 }
 
 // ---- Morton keys --------------------------------------------------------------------------------
@@ -219,12 +228,12 @@ __global__ void k_gather_sorted(const float4* __restrict__ p, const int32_t* __r
 }
 
 // ---- refit --------------------------------------------------------------------------------------
-__global__ void k_refit(const float4* __restrict__ pts, int n_leaves, const int2* __restrict__ children,
-                        const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
-                        float4* __restrict__ leaf_lo, float4* __restrict__ leaf_hi, float4* __restrict__ node_lo,
-                        float4* __restrict__ node_hi, unsigned* __restrict__ flags)
+__device__ __forceinline__ void refit_item(int leaf, const float4* __restrict__ pts, int n_leaves,
+                                           const int2* __restrict__ children, const int* __restrict__ node_parent,
+                                           const int* __restrict__ leaf_parent, float4* __restrict__ leaf_lo,
+                                           float4* __restrict__ leaf_hi, float4* __restrict__ node_lo,
+                                           float4* __restrict__ node_hi, unsigned* __restrict__ flags)
 {
-  int leaf = blockIdx.x * blockDim.x + threadIdx.x;
   if (leaf >= n_leaves)
     return;
   float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
@@ -258,11 +267,20 @@ __global__ void k_refit(const float4* __restrict__ pts, int n_leaves, const int2
   }
 }
 
-__global__ void k_pack_nodes(int n_internal, const int2* __restrict__ children, const float4* __restrict__ leaf_lo,
-                             const float4* __restrict__ leaf_hi, const float4* __restrict__ node_lo,
-                             const float4* __restrict__ node_hi, BvhNode* __restrict__ nodes)
+__global__ void k_refit(const float4* __restrict__ pts, int n_leaves, const int2* __restrict__ children,
+                        const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
+                        float4* __restrict__ leaf_lo, float4* __restrict__ leaf_hi, float4* __restrict__ node_lo,
+                        float4* __restrict__ node_hi, unsigned* __restrict__ flags)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  refit_item(blockIdx.x * blockDim.x + threadIdx.x, pts, n_leaves, children, node_parent, leaf_parent, leaf_lo, leaf_hi,
+             node_lo, node_hi, flags);
+}
+
+__device__ __forceinline__ void pack_nodes_item(int i, int n_internal, const int2* __restrict__ children,
+                                                const float4* __restrict__ leaf_lo, const float4* __restrict__ leaf_hi,
+                                                const float4* __restrict__ node_lo, const float4* __restrict__ node_hi,
+                                                BvhNode* __restrict__ nodes)
+{
   if (i >= n_internal)
     return;
   int2 ch = children[i];
@@ -276,6 +294,13 @@ __global__ void k_pack_nodes(int n_internal, const int2* __restrict__ children, 
   nd.c = make_float4(blo.z, bhi.x, bhi.y, bhi.z);
   nd.d = make_int4(ch.x, ch.y, 0, 0);
   nodes[i] = nd;
+}
+
+__global__ void k_pack_nodes(int n_internal, const int2* __restrict__ children, const float4* __restrict__ leaf_lo,
+                             const float4* __restrict__ leaf_hi, const float4* __restrict__ node_lo,
+                             const float4* __restrict__ node_hi, BvhNode* __restrict__ nodes)
+{
+  pack_nodes_item(blockIdx.x * blockDim.x + threadIdx.x, n_internal, children, leaf_lo, leaf_hi, node_lo, node_hi, nodes);
 }
 
 // ---- cell-aligned leaves --------------------------------------------------------------------------------------
@@ -300,48 +325,7 @@ __global__ void k_karras_points(const unsigned long long* __restrict__ keys, int
                                 int* __restrict__ node_parent, int* __restrict__ point_parent, int2* __restrict__ range)
 {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n - 1)
-    return;
-  int d = (delta_pt(keys, n, i, i + 1) - delta_pt(keys, n, i, i - 1)) >= 0 ? 1 : -1;
-  int dmin = delta_pt(keys, n, i, i - d);
-  int lmax = 2;
-  while (delta_pt(keys, n, i, i + lmax * d) > dmin)
-    lmax <<= 1;
-  int l = 0;
-  for (int t = lmax >> 1; t >= 1; t >>= 1)
-    if (delta_pt(keys, n, i, i + (l + t) * d) > dmin)
-      l += t;
-  int j = i + l * d;
-  int dnode = delta_pt(keys, n, i, j);
-  int s = 0;
-  int t = l;
-  do {
-    t = (t + 1) >> 1;
-    if (delta_pt(keys, n, i, i + (s + t) * d) > dnode)
-      s += t;
-  } while (t > 1);
-  int gamma = i + s * d + min(d, 0);
-  int left, right;
-  if (min(i, j) == gamma) {
-    left = ~gamma;
-    point_parent[gamma] = i;
-  }
-  else {
-    left = gamma;
-    node_parent[gamma] = i;
-  }
-  if (max(i, j) == gamma + 1) {
-    right = ~(gamma + 1);
-    point_parent[gamma + 1] = i;
-  }
-  else {
-    right = gamma + 1;
-    node_parent[gamma + 1] = i;
-  }
-  children[i] = make_int2(left, right);
-  range[i] = make_int2(min(i, j), max(i, j));
-  if (i == 0)
-    node_parent[0] = -1;
+#include "karras_points_body.inc"
 }
 
 // keep[i] = node i stays an internal node of the final tree (holds more than kLeafSize points);
@@ -350,28 +334,20 @@ __global__ void k_mark_cells(int n, const int2* __restrict__ range, const int* _
                              const int* __restrict__ point_parent, int* __restrict__ keep, int* __restrict__ leaf_flag)
 {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n - 1) {
-    const int2 r = range[i];
-    const int cnt = r.y - r.x + 1;
-    const int par = node_parent[i];
-    const int pcnt = par < 0 ? 0x7fffffff : (range[par].y - range[par].x + 1);
-    keep[i] = cnt > kLeafSize ? 1 : 0;
-    if (cnt <= kLeafSize && pcnt > kLeafSize)
-      leaf_flag[r.x] = 1;
-  }
-  if (i < n) {
-    const int par = point_parent[i];
-    if (range[par].y - range[par].x + 1 > kLeafSize)
-      leaf_flag[i] = 1;  // a single point whose sibling subtree is large
-  }
+#include "mark_cells_body.inc"
+}
+
+__device__ __forceinline__ void leaf_starts_item(int i, int n, const int* __restrict__ leaf_flag,
+                                                 const int* __restrict__ leaf_incl, int* __restrict__ leaf_start)
+{
+  if (i < n && leaf_flag[i])
+    leaf_start[leaf_incl[i] - 1] = i;
 }
 
 __global__ void k_leaf_starts(int n, const int* __restrict__ leaf_flag, const int* __restrict__ leaf_incl,
                               int* __restrict__ leaf_start)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && leaf_flag[i])
-    leaf_start[leaf_incl[i] - 1] = i;
+  leaf_starts_item(blockIdx.x * blockDim.x + threadIdx.x, n, leaf_flag, leaf_incl, leaf_start);
 }
 
 __global__ void k_fill_sentinels(float4* __restrict__ out, size_t n)
@@ -384,11 +360,12 @@ __global__ void k_fill_sentinels(float4* __restrict__ out, size_t n)
 }
 
 // sorted position -> padded leaf slot
-__global__ void k_scatter_cells(const float4* __restrict__ p, const int32_t* __restrict__ vals,
-                                const int32_t* __restrict__ orig_of_slot, int n, const int* __restrict__ leaf_incl,
-                                const int* __restrict__ leaf_start, float4* __restrict__ out)
+__device__ __forceinline__ void scatter_cells_item(int pos, const float4* __restrict__ p,
+                                                   const int32_t* __restrict__ vals,
+                                                   const int32_t* __restrict__ orig_of_slot, int n,
+                                                   const int* __restrict__ leaf_incl, const int* __restrict__ leaf_start,
+                                                   float4* __restrict__ out)
 {
-  int pos = blockIdx.x * blockDim.x + threadIdx.x;
   if (pos >= n)
     return;
   const int leaf = leaf_incl[pos] - 1;
@@ -396,6 +373,13 @@ __global__ void k_scatter_cells(const float4* __restrict__ p, const int32_t* __r
   const float4 v = __ldg(p + slot);
   const int32_t oi = orig_of_slot ? orig_of_slot[slot] : slot;
   out[(size_t)leaf * kLeafSize + (pos - leaf_start[leaf])] = make_float4(v.x, v.y, v.z, __int_as_float(oi));
+}
+
+__global__ void k_scatter_cells(const float4* __restrict__ p, const int32_t* __restrict__ vals,
+                                const int32_t* __restrict__ orig_of_slot, int n, const int* __restrict__ leaf_incl,
+                                const int* __restrict__ leaf_start, float4* __restrict__ out)
+{
+  scatter_cells_item(blockIdx.x * blockDim.x + threadIdx.x, p, vals, orig_of_slot, n, leaf_incl, leaf_start, out);
 }
 
 // ---- cell table -------------------------------------------------------------------------------------------------------
@@ -463,63 +447,358 @@ __global__ void k_link_cells(int n, const int2* __restrict__ children, const int
                              int* __restrict__ out_leaf_parent, int2* __restrict__ out_node_leaves, CellTableW cells)
 {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n - 1 || !keep[i])
-    return;
-  const int nid = new_id[i];
-  const int2 ch = children[i];
-  int ref[2];
-  const int c2[2] = {ch.x, ch.y};
-#pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const int cc = c2[k];
-    if (cc >= 0 && keep[cc]) {
-      ref[k] = new_id[cc];
-      out_node_parent[new_id[cc]] = nid;
-    }
-    else {
-      const int first = cc >= 0 ? range[cc].x : ~cc;
-      const int leaf = leaf_incl[first] - 1;
-      ref[k] = ~leaf;
-      out_leaf_parent[leaf] = nid;
+#include "link_cells_body.inc"
+}
+
+// ---- host decisions every build shares ------------------------------------------------------------------------------
+// the index's frame from its bbox accumulator: box of the finite points, ONE isotropic scale so Morton cells are cubes
+inline void morton_frame(const BBoxAcc& h, float lo[3], float hi[3], float& scale)
+{
+  float ext = 0.f;
+  for (int d = 0; d < 3; ++d) {
+    lo[d] = ord2f(h.lo[d]);
+    hi[d] = ord2f(h.hi[d]);
+    ext = std::max(ext, hi[d] - lo[d]);
+  }
+  scale = ext > 0.f ? 2097152.f / ext : 1.f;
+  if (!std::isfinite(scale))
+    scale = 1.f;
+}
+
+// The cell table of an index of nv >= 256 points (traverse.cuh: CellTable): levels 1..bmax, bmax = the finest level
+// (<= kCellMaxBits) whose occupied cells still hold >= 4 indexed points on average — finer levels would mostly map single
+// points.  The number of entries is known exactly from the prefix-length histogram (k_prefix_hist); the table gets >= 2
+// slots per entry.  log2_slots = 0: no table.
+inline CellTableHost cell_table_plan(const unsigned hist[64], int nv, const float lo[3], const float hi[3], float scale)
+{
+  CellTableHost t;
+  uint64_t cum = 1, entries = 0;
+  int l = 0, bmax = 0;
+  for (int b = 1; b <= kCellMaxBits; ++b) {
+    for (; l < 3 * b; ++l)
+      cum += hist[l];
+    if (cum > (uint64_t)nv / 4)
+      break;
+    bmax = b;
+    entries += cum;
+    t.occupied[b] = cum;
+  }
+  if (bmax >= 1) {
+    unsigned lg = 6;
+    while (((uint64_t)1 << lg) < 2 * entries)
+      ++lg;
+    t.log2_slots = lg;
+    t.bmax = bmax;
+    t.entries = entries;
+    float m = 0.f;
+    for (int d = 0; d < 3; ++d)
+      m = std::max(m, std::max(std::fabs(lo[d]), std::fabs(hi[d])));
+    m = std::max(m, 2097152.f / scale);
+    t.margin = 2e-6f * m;
+  }
+  return t;
+}
+
+// the kernels' view of a planned table whose slots are allocated (and zeroed before the first insert)
+inline CellTableW cell_table_view(uint2* slots, const CellTableHost& t)
+{
+  return CellTableW{reinterpret_cast<unsigned long long*>(slots), 32 - t.log2_slots, (1u << t.log2_slots) - 1u, t.bmax};
+}
+
+// ---- a batch of clouds in one build ---------------------------------------------------------------------------------
+// Cloud c is the records [first, first + n) of one dense array.  Each stage runs the single build's body on the cloud's
+// base pointers: sorted positions of cloud c start at `first`, its radix-tree node scratch at first - c (a cloud of n
+// points has at most n - 1 nodes), its final leaves and nodes at leaf_first / node_first of the batch's scratch.
+constexpr int kBatchTile = 4096;  // points per block of the per-cloud reductions (tiles never straddle two clouds)
+
+struct BuildCloud {
+  long long first = 0;       // first record (= first sorted position) of the cloud
+  long long n = 0;           // records
+  int nv = 0;                // finite points
+  float lo[3] = {0, 0, 0}, scale = 1.f;  // the cloud's Morton frame
+  // known after the cut (the second read-back)
+  int n_leaves = 0, n_int = 0;
+  long long leaf_first = 0, node_first = 0;  // in the batch's leaf / final-node scratch
+  float4* pts = nullptr;     // the cloud's handle: n_leaves * kLeafSize
+  BvhNode* nodes = nullptr;  // n_int
+  int2* node_leaves = nullptr;
+  CellTableW cells{nullptr, 0, 0, 0};
+};
+
+// what the host reads after the cut: the leaf and node counts, and the prefix-length histogram (nv >= 256 only)
+struct CloudSummary {
+  int n_leaves, n_int;
+  unsigned hist[64];
+};
+
+// per cloud, the box and finite count of its records; block b works on tile b - tiles[c] of cloud c = problem_of(tiles, b)
+__global__ void k_bbox_batch(const float4* __restrict__ p, const BuildCloud* __restrict__ clouds,
+                             const long long* __restrict__ tiles, int n_clouds, BBoxAcc* acc)
+{
+  const int c = problem_of(tiles, n_clouds, (long long)blockIdx.x);
+  const BuildCloud& C = clouds[c];
+  const long long t0 = (blockIdx.x - tiles[c]) * (long long)kBatchTile;
+  const long long end = t0 + kBatchTile < C.n ? t0 + kBatchTile : C.n;
+  float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+  unsigned cnt = 0;
+  for (long long i = t0 + threadIdx.x; i < end; i += blockDim.x) {
+    float4 v = __ldg(p + C.first + i);
+    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
+      lo[0] = fminf(lo[0], v.x); hi[0] = fmaxf(hi[0], v.x);
+      lo[1] = fminf(lo[1], v.y); hi[1] = fmaxf(hi[1], v.y);
+      lo[2] = fminf(lo[2], v.z); hi[2] = fmaxf(hi[2], v.z);
+      ++cnt;
     }
   }
-  out_children[nid] = make_int2(ref[0], ref[1]);
-  {
-    // a subtree's leaves are consecutive in Morton order: the warp-cooperative k-NN gathers whole cells as one range
-    const int fl = leaf_incl[range[i].x] - 1, ll = leaf_incl[range[i].y] - 1;
-    out_node_leaves[nid] = make_int2(fl, ll - fl + 1);
-  }
-  if (i == 0)
-    out_node_parent[nid] = -1;
-  if (cells.slots == nullptr)
+  bbox_publish(lo, hi, cnt, acc + c);
+}
+
+// k_morton<false> of every point in its own cloud's frame; vals = the record (global)
+__global__ void k_morton_batch(const float4* __restrict__ p, size_t n, const long long* __restrict__ offsets,
+                               int n_clouds, const BuildCloud* __restrict__ clouds, unsigned long long* __restrict__ keys,
+                               int32_t* __restrict__ vals)
+{
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
     return;
-  // cell table: child C is the deepest node that holds every indexed point of a 3b-bit prefix cell exactly when
-  //   prefix_len(this node) < 3b <= prefix_len(C).
-  // (Nodes cut INSIDE a run of equal codes have prefix length 63 like their parent and never qualify: only purely
-  // spatial cells enter the table.)
-  const int l_self = prefix_len63(keys[range[i].x], keys[range[i].y]);
-  if (i == 0)  // the root holds every point of the cells its own prefix spans (degenerate frames only)
-    for (int b = 1; b <= cells.bmax && 3 * b <= l_self; ++b)
-      cell_insert(cells, b, keys[0], nid);
-#pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const int cc = c2[k];
-    const int first = cc >= 0 ? range[cc].x : ~cc;
-    const int last = cc >= 0 ? range[cc].y : ~cc;
-    const int l_child = cc >= 0 ? prefix_len63(keys[first], keys[last]) : 63;
-    const bool is_leaf = !(cc >= 0 && keep[cc]);
-    for (int b = l_self / 3 + 1; b <= cells.bmax; ++b) {  // 3b > l_self
-      if (3 * b <= l_child)
-        cell_insert(cells, b, keys[first], ref[k]);
-      else if (is_leaf)
-        // a leaf that spans several level-b cells still holds every indexed point of each of them
-        for (int j = first; j <= last; ++j)
-          cell_insert(cells, b, keys[j], ref[k]);
-      else
-        break;  // a kept child with a shorter prefix: its own thread inserts the finer levels
-    }
+  const BuildCloud& C = clouds[problem_of(offsets, n_clouds, (long long)i)];
+  const float4 v = __ldg(p + i);
+  const bool ok = isfinite(v.x) && isfinite(v.y) && isfinite(v.z);
+  keys[i] = !ok ? ~0ULL : morton63(v.x, v.y, v.z, C.lo[0], C.lo[1], C.lo[2], C.scale);
+  vals[i] = (int32_t)i;
+}
+
+// after the sort by key: the cloud of each sorted record (the key of the stable sort by cloud) and its position
+__global__ void k_cloud_of_sorted(const int32_t* __restrict__ vals, size_t n, const long long* __restrict__ offsets,
+                                  int n_clouds, unsigned* __restrict__ cloud, int32_t* __restrict__ pos)
+{
+  const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (j >= n)
+    return;
+  cloud[j] = (unsigned)problem_of(offsets, n_clouds, (long long)vals[j]);
+  pos[j] = (int32_t)j;
+}
+
+// the permutation of the sort by cloud applied: each cloud's range is its single build's sorted keys and local slots
+__global__ void k_permute_sorted(const unsigned long long* __restrict__ keys_in, const int32_t* __restrict__ vals_in,
+                                 const int32_t* __restrict__ perm, size_t n, const long long* __restrict__ offsets,
+                                 int n_clouds, unsigned long long* __restrict__ keys, int32_t* __restrict__ vals)
+{
+  const size_t k = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (k >= n)
+    return;
+  const int32_t j = perm[k];
+  keys[k] = keys_in[j];
+  vals[k] = vals_in[j] - (int32_t)offsets[problem_of(offsets, n_clouds, (long long)k)];
+}
+
+// work item g of a launch over all records: cloud c and the cloud's local item g - first
+#define PCLB_BATCH_ITEM(offsets, n_clouds, n)                                      \
+  const long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x;            \
+  if (g >= (long long)(n))                                                         \
+    return;                                                                        \
+  const int c = problem_of(offsets, n_clouds, g);                                  \
+  const BuildCloud& C = clouds[c];                                                 \
+  const int i = (int)(g - C.first);
+
+// karras_points_item of every cloud of more than kLeafSize points; node_cloud[node] = the cloud of every node position
+__global__ void k_karras_points_batch(const unsigned long long* __restrict__ keys_all, size_t n_all,
+                                      const long long* __restrict__ offsets, int n_clouds,
+                                      const BuildCloud* __restrict__ clouds, int2* __restrict__ children_all,
+                                      int* __restrict__ node_parent_all, int* __restrict__ point_parent_all,
+                                      int2* __restrict__ range_all, unsigned* __restrict__ node_cloud)
+{
+  PCLB_BATCH_ITEM(offsets, n_clouds, n_all)
+  const long long nb = C.first - c;
+  if (i < C.n - 1)
+    node_cloud[nb + i] = (unsigned)c;
+  if (C.nv <= kLeafSize)
+    return;
+  const unsigned long long* __restrict__ keys = keys_all + C.first;
+  const int n = C.nv;
+  int2* __restrict__ children = children_all + nb;
+  int* __restrict__ node_parent = node_parent_all + nb;
+  int* __restrict__ point_parent = point_parent_all + C.first;
+  int2* __restrict__ range = range_all + nb;
+#include "karras_points_body.inc"
+}
+
+__global__ void k_mark_cells_batch(size_t n_all, const long long* __restrict__ offsets, int n_clouds,
+                                   const BuildCloud* __restrict__ clouds, const int2* __restrict__ range_all,
+                                   const int* __restrict__ node_parent_all, const int* __restrict__ point_parent_all,
+                                   int* __restrict__ keep_all, int* __restrict__ leaf_flag_all)
+{
+  PCLB_BATCH_ITEM(offsets, n_clouds, n_all)
+  if (C.nv <= kLeafSize)
+    return;
+  const long long nb = C.first - c;
+  const int n = C.nv;
+  const int2* __restrict__ range = range_all + nb;
+  const int* __restrict__ node_parent = node_parent_all + nb;
+  const int* __restrict__ point_parent = point_parent_all + C.first;
+  int* __restrict__ keep = keep_all + nb;
+  int* __restrict__ leaf_flag = leaf_flag_all + C.first;
+#include "mark_cells_body.inc"
+}
+
+// k_prefix_hist of every cloud of >= 256 points into its summary (zeroed), over tiles as k_bbox_batch
+__global__ void k_prefix_hist_batch(const unsigned long long* __restrict__ keys, const BuildCloud* __restrict__ clouds,
+                                    const long long* __restrict__ tiles, int n_clouds, CloudSummary* __restrict__ out)
+{
+  __shared__ unsigned sh[64];
+  const int c = problem_of(tiles, n_clouds, (long long)blockIdx.x);
+  const BuildCloud& C = clouds[c];
+  if (C.nv < 256)
+    return;  // the whole block
+  if (threadIdx.x < 64)
+    sh[threadIdx.x] = 0;
+  __syncthreads();
+  const long long t0 = (blockIdx.x - tiles[c]) * (long long)kBatchTile;
+  const long long end = t0 + kBatchTile < C.nv ? t0 + kBatchTile : C.nv;
+  const unsigned long long* k = keys + C.first;
+  for (long long i = (t0 > 0 ? t0 : 1) + threadIdx.x; i < end; i += blockDim.x)
+    atomicAdd(&sh[prefix_len63(k[i - 1], k[i])], 1u);
+  __syncthreads();
+  if (threadIdx.x < 64 && sh[threadIdx.x])
+    atomicAdd(&out[c].hist[threadIdx.x], sh[threadIdx.x]);
+}
+
+// the leaf and node counts of each cloud's cut (one thread per cloud; a cloud of <= kLeafSize points is one leaf)
+__global__ void k_cut_summary(const BuildCloud* __restrict__ clouds, int n_clouds, const int* __restrict__ leaf_incl,
+                              const int* __restrict__ new_id, const int* __restrict__ keep, CloudSummary* __restrict__ out)
+{
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_clouds)
+    return;
+  const BuildCloud& C = clouds[c];
+  if (C.nv <= kLeafSize) {
+    out[c].n_leaves = 1;
+    out[c].n_int = 0;
+    return;
+  }
+  const long long nb = C.first - c, last = nb + C.nv - 2;
+  out[c].n_leaves = leaf_incl[C.first + C.nv - 1];
+  out[c].n_int = new_id[last] + keep[last];
+}
+
+// the handles' sentinel padding (leaf space: n_leaves * kLeafSize per cloud) and zeroed cell-table slots (slot space)
+__global__ void k_clear_outputs_batch(const BuildCloud* __restrict__ clouds, int n_clouds,
+                                      const long long* __restrict__ leaf_offsets, const long long* __restrict__ slot_offsets)
+{
+  const long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (g < leaf_offsets[n_clouds] * kLeafSize) {
+    const int c = problem_of(leaf_offsets, n_clouds, g / kLeafSize);
+    const float inf = __int_as_float(0x7f800000);
+    clouds[c].pts[g - leaf_offsets[c] * kLeafSize] = make_float4(inf, inf, inf, __int_as_float(kSentinelIndex));
+  }
+  if (g < slot_offsets[n_clouds]) {
+    const int c = problem_of(slot_offsets, n_clouds, g);
+    clouds[c].cells.slots[g - slot_offsets[c]] = 0ULL;
   }
 }
+
+// k_gather_sorted of every cloud of <= kLeafSize points: its one leaf (kLeafSize items per cloud)
+__global__ void k_gather_small_batch(const float4* __restrict__ p, const int32_t* __restrict__ vals,
+                                     const BuildCloud* __restrict__ clouds, int n_clouds)
+{
+  const long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (g >= (long long)n_clouds * kLeafSize)
+    return;
+  const BuildCloud& C = clouds[g / kLeafSize];
+  if (C.nv > kLeafSize)
+    return;
+  const size_t j = (size_t)(g % kLeafSize);
+  if (j < (size_t)C.nv) {
+    const int32_t slot = vals[C.first + j];
+    const float4 v = __ldg(p + C.first + slot);
+    C.pts[j] = make_float4(v.x, v.y, v.z, __int_as_float(slot));
+  }
+  else {
+    const float inf = __int_as_float(0x7f800000);
+    C.pts[j] = make_float4(inf, inf, inf, __int_as_float(kSentinelIndex));
+  }
+}
+
+__global__ void k_leaf_starts_batch(size_t n, const long long* __restrict__ offsets, int n_clouds,
+                                    const BuildCloud* __restrict__ clouds, const int* __restrict__ leaf_flag,
+                                    const int* __restrict__ leaf_incl, int* __restrict__ leaf_start)
+{
+  PCLB_BATCH_ITEM(offsets, n_clouds, n)
+  if (C.nv <= kLeafSize)
+    return;
+  leaf_starts_item(i, C.nv, leaf_flag + C.first, leaf_incl + C.first, leaf_start + C.leaf_first);
+}
+
+__global__ void k_scatter_cells_batch(const float4* __restrict__ p, const int32_t* __restrict__ vals, size_t n,
+                                      const long long* __restrict__ offsets, int n_clouds,
+                                      const BuildCloud* __restrict__ clouds, const int* __restrict__ leaf_incl,
+                                      const int* __restrict__ leaf_start)
+{
+  PCLB_BATCH_ITEM(offsets, n_clouds, n)
+  if (C.nv <= kLeafSize)
+    return;
+  scatter_cells_item(i, p + C.first, vals + C.first, nullptr, C.nv, leaf_incl + C.first, leaf_start + C.leaf_first,
+                     C.pts);
+}
+
+__global__ void k_link_cells_batch(size_t n_all, const long long* __restrict__ offsets, int n_clouds,
+                                   const BuildCloud* __restrict__ clouds, const int2* __restrict__ children_all,
+                                   const int2* __restrict__ range_all, const int* __restrict__ keep_all,
+                                   const int* __restrict__ new_id_all, const int* __restrict__ leaf_incl_all,
+                                   const unsigned long long* __restrict__ keys_all, int2* __restrict__ out_children_all,
+                                   int* __restrict__ out_node_parent_all, int* __restrict__ out_leaf_parent_all)
+{
+  PCLB_BATCH_ITEM(offsets, n_clouds, n_all)
+  if (C.nv <= kLeafSize)
+    return;
+  const long long nb = C.first - c;
+  const int n = C.nv;
+  const int2* __restrict__ children = children_all + nb;
+  const int2* __restrict__ range = range_all + nb;
+  const int* __restrict__ keep = keep_all + nb;
+  const int* __restrict__ new_id = new_id_all + nb;
+  const int* __restrict__ leaf_incl = leaf_incl_all + C.first;
+  const unsigned long long* __restrict__ keys = keys_all + C.first;
+  int2* __restrict__ out_children = out_children_all + C.node_first;
+  int* __restrict__ out_node_parent = out_node_parent_all + C.node_first;
+  int* __restrict__ out_leaf_parent = out_leaf_parent_all + C.leaf_first;
+  int2* __restrict__ out_node_leaves = C.node_leaves;
+  const CellTableW cells = C.cells;
+#include "link_cells_body.inc"
+}
+
+// leaf space: every cloud's n_leaves leaves end to end (leaf_offsets)
+__global__ void k_refit_batch(const BuildCloud* __restrict__ clouds, int n_clouds,
+                              const long long* __restrict__ leaf_offsets, const int2* __restrict__ children,
+                              const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
+                              float4* __restrict__ leaf_lo, float4* __restrict__ leaf_hi, float4* __restrict__ node_lo,
+                              float4* __restrict__ node_hi, unsigned* __restrict__ flags)
+{
+  const long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (g >= leaf_offsets[n_clouds])
+    return;
+  const BuildCloud& C = clouds[problem_of(leaf_offsets, n_clouds, g)];
+  if (C.nv <= kLeafSize)
+    return;
+  const long long lb = C.leaf_first, nb = C.node_first;
+  refit_item((int)(g - lb), C.pts, C.n_leaves, children + nb, node_parent + nb, leaf_parent + lb, leaf_lo + lb,
+             leaf_hi + lb, node_lo + nb, node_hi + nb, flags + nb);
+}
+
+// node space: every cloud's n_int final nodes end to end (node_offsets)
+__global__ void k_pack_nodes_batch(const BuildCloud* __restrict__ clouds, int n_clouds,
+                                   const long long* __restrict__ node_offsets, const int2* __restrict__ children,
+                                   const float4* __restrict__ leaf_lo, const float4* __restrict__ leaf_hi,
+                                   const float4* __restrict__ node_lo, const float4* __restrict__ node_hi)
+{
+  const long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (g >= node_offsets[n_clouds])
+    return;
+  const BuildCloud& C = clouds[problem_of(node_offsets, n_clouds, g)];
+  const long long lb = C.leaf_first, nb = C.node_first;
+  pack_nodes_item((int)(g - nb), C.n_int, children + nb, leaf_lo + lb, leaf_hi + lb, node_lo + nb, node_hi + nb, C.nodes);
+}
+#undef PCLB_BATCH_ITEM
 
 // ---- host orchestration -------------------------------------------------------------------------
 
