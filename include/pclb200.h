@@ -177,8 +177,13 @@ PCLB200_API int pclb200_correspondences_normals(pclb200_ctx* ctx, const pclb200_
  * ONE_TO_ONE CorrespondenceRejectorOneToOne        .../correspondence_rejection_one_to_one.cpp:44-71
  *            the closest query of every index_match; output ordered by index_match
  * TRIMMED    CorrespondenceRejectorTrimmed         .../correspondence_rejection_trimmed.cpp:44-63
- *            p = overlap ratio; keeps max(floor(p * n), min_correspondences) smallest distances (sorted output)
- * Exact-distance ties (std::sort in the reference is unstable) resolve to the entry that comes first in the input. */
+ *            p = overlap ratio, clamped like setOverlapRatio: min(1, max(0, float(p))), NaN gives 0;
+ *            min_correspondences is read as the unsigned int of setMinCorrespondences (-1 is 2^32 - 1);
+ *            keep = max(floor(p * float(n)) in float, min): when keep < n the keep smallest distances (sorted output),
+ *            otherwise the input unchanged
+ * Exact-distance ties (std::sort in the reference is unstable) resolve to the entry that comes first in the input.
+ * Distances may be any float but NaN (NaN is outside the contract): -0.0 compares equal to +0.0 and is reported as
+ * +0.0 when it is the median, negatives come before zero, +inf after FLT_MAX. */
 #define PCLB200_REJ_DISTANCE 0
 #define PCLB200_REJ_MEDIAN 1
 #define PCLB200_REJ_ONE_TO_ONE 2
@@ -307,9 +312,11 @@ PCLB200_API int pclb200_icp_create(pclb200_ctx* ctx, const pclb200_icp_params* p
 PCLB200_API int pclb200_icp_destroy(pclb200_icp* icp);
 PCLB200_API int pclb200_icp_set_params(pclb200_icp* icp, const pclb200_icp_params* params);
 /* Registration::addCorrespondenceRejector / clearCorrespondenceRejectors (registration.h:373-416): the chain is
- * applied on the device, in order, to every iteration's correspondences (n == 0 clears it).  With a multi-GPU
- * communicator every rank accepts what one process accepts running the chain over the shards concatenated in rank
- * order (see the communicator section below). */
+ * applied on the device, in order, to every iteration's correspondences (n == 0 clears it).  Every rejector sees the
+ * survivors of the one before in source-position order (the order of the source index list), so exact-distance ties
+ * break by position at every stage, also after a ONE_TO_ONE (whose stand-alone output is in index_match order); the
+ * list get_correspondences returns is in that order too.  With a multi-GPU communicator every rank accepts what one
+ * process accepts running the chain over the shards concatenated in rank order (see the communicator section below). */
 PCLB200_API int pclb200_icp_set_rejectors(pclb200_icp* icp, const pclb200_rejector* list, int n);
 PCLB200_API int pclb200_icp_set_target(pclb200_icp* icp, const pclb200_index* idx_tgt,
                                        const void* tgt_normals, size_t stride_n);
@@ -321,7 +328,8 @@ PCLB200_API int pclb200_icp_iterate(pclb200_icp* icp, int max_steps, pclb200_icp
 PCLB200_API int pclb200_icp_get_cloud(pclb200_icp* icp, void* out_pts, size_t stride_out,
                                       void* out_normals, size_t stride_n);
 /* correspondences of the last evaluated iteration (Registration::correspondences_, what icp.hpp:228-236 hands to
- * the visualisation callback): capacity = number of indexed source points, ordered like the source index list. */
+ * the visualisation callback): capacity = number of indexed source points, ordered like the source index list.  A
+ * loop that stopped with NO_CORRESPONDENCES returns the list (fewer than 3 pairs) that stopped it. */
 PCLB200_API int pclb200_icp_get_correspondences(pclb200_icp* icp, pclb200_corr* out, size_t* n_out);
 
 /* one-call form: Registration::align(output, guess) (registration.hpp:172-221) */

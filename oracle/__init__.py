@@ -83,7 +83,10 @@ def lib():
         L.orc_icp_align_tree.argtypes = [C.POINTER(IcpParams), vp, fp, sz, sz, i32p, sz, fp, sz, sz, dp, C.POINTER(IcpResult), fp]
         L.orc_reject.restype = sz
         L.orc_reject.argtypes = [C.POINTER(Rejector), C.POINTER(Corr), sz, C.POINTER(Corr), dp]
-        L.orc_icp_align_rej.argtypes = [C.POINTER(IcpParams), C.POINTER(Rejector), C.c_int, fp, sz, sz, fp, sz, sz, C.POINTER(IcpResult)]
+        L.orc_reject_chain.restype = sz
+        L.orc_reject_chain.argtypes = [C.POINTER(Rejector), C.c_int, C.POINTER(Corr), sz, C.POINTER(Corr), dp]
+        L.orc_icp_align_full.argtypes = [C.POINTER(IcpParams), vp, C.POINTER(Rejector), C.c_int, vp, fp, sz, sz, i32p, sz,
+                                         fp, sz, sz, dp, C.POINTER(IcpResult), fp, C.POINTER(Corr), C.POINTER(sz)]
         L.orc_fitness_score.restype = C.c_double
         L.orc_fitness_score.argtypes = [vp, fp, sz, sz, i32p, sz, C.c_int, dp, C.c_int, C.c_double, C.c_int]
         L.orc_voxelgrid.restype = C.c_longlong
@@ -403,21 +406,41 @@ def reject(corr, kind, p=0.0, min_correspondences=0):
     return out[:m].copy(), float(med.value)
 
 
+def reject_chain(corr, rejectors):
+    """The ICP loop's chain [(kind, p, min_correspondences), ...] on a list in position order: every rejector sees the
+    survivors in that order (so breaks distance ties by position); returns (remaining in position order, median of the
+    last MEDIAN stage)."""
+    corr = np.ascontiguousarray(corr, dtype=CORR_DTYPE)
+    out = np.empty(max(corr.size, 1), dtype=CORR_DTYPE)
+    arr = (Rejector * max(len(rejectors), 1))(*[Rejector(k, m, float(p)) for (k, p, m) in rejectors])
+    med = C.c_double(0.0)
+    m = lib().orc_reject_chain(arr, len(rejectors), corr.ctypes.data_as(C.POINTER(Corr)), corr.size,
+                               out.ctypes.data_as(C.POINTER(Corr)), C.byref(med))
+    return out[:m].copy(), float(med.value)
+
+
 def icp_align_rejectors(src, tgt, rejectors, **kw):
-    """ICP with a chain of rejectors [(kind, p, min_correspondences), ...] (icp.hpp:187-201)."""
+    """ICP with a chain of rejectors [(kind, p, min_correspondences), ...] (icp.hpp:187-201).  The result's
+    "correspondences" are those of the last evaluated iteration, after the chain (Registration::correspondences_)."""
     src, tgt = as_cloud(src), as_cloud(tgt)
     has_n = int(kw.get("source_has_normals", False))
-    P = IcpParams(kw.get("max_iterations", 10), 0, int(kw.get("estimator", 0)), int(kw.get("scalar_is_double", False)),
-                  has_n, has_n, 1,
+    P = IcpParams(kw.get("max_iterations", 10), int(kw.get("use_reciprocal", False)), int(kw.get("estimator", 0)),
+                  int(kw.get("scalar_is_double", False)), has_n, has_n, int(kw.get("is_dense", True)),
                   kw.get("nthreads", 1), float(kw.get("max_correspondence_distance", np.sqrt(np.finfo(np.float64).max))),
                   float(kw.get("transformation_epsilon", 0.0)), 0.0, float(kw.get("euclidean_fitness_epsilon", -np.finfo(np.float64).max)),
                   int(kw.get("correspondence_kind", 0)), int(kw.get("correspondence_k", 10)))
     arr = (Rejector * len(rejectors))(*[Rejector(k, m, float(p)) for (k, p, m) in rejectors])
     R = IcpResult()
-    lib().orc_icp_align_rej(C.byref(P), arr, len(rejectors), _f(src), src.shape[0], src.shape[1], _f(tgt), tgt.shape[0],
-                            tgt.shape[1], C.byref(R))
+    indices = kw.get("indices")
+    indices = None if indices is None else np.ascontiguousarray(indices, dtype=np.int32)
+    corr = np.empty(max(src.shape[0] if indices is None else indices.size, 1), dtype=CORR_DTYPE)
+    nc = C.c_size_t(0)
+    lib().orc_icp_align_full(C.byref(P), None, arr, len(rejectors), None, _f(src), src.shape[0], src.shape[1], _i(indices),
+                             0 if indices is None else indices.size, _f(tgt), tgt.shape[0], tgt.shape[1], None,
+                             C.byref(R), None, corr.ctypes.data_as(C.POINTER(Corr)), C.byref(nc))
     return dict(final=np.array(R.final_transformation).reshape(4, 4), converged=bool(R.converged), state=int(R.state),
-                iterations=int(R.iterations), n_correspondences=int(R.n_correspondences), mse=float(R.mse))
+                iterations=int(R.iterations), n_correspondences=int(R.n_correspondences), mse=float(R.mse),
+                correspondences=corr[:nc.value].copy())
 
 
 def voxelgrid(cloud, leaf, min_points_per_voxel=0, indices=None, is_dense=True):

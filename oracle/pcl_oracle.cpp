@@ -1395,7 +1395,8 @@ ORC_API void orc_transform(float* pts, size_t n, size_t stride, int normal_off, 
 // registration/src/correspondence_rejection_median_distance.cpp:44-70     keep distance <= median * factor (double), order kept
 // registration/src/correspondence_rejection_one_to_one.cpp:44-71          sort by (index_match, distance), first per match
 // registration/src/correspondence_rejection_trimmed.cpp:44-63             floor(overlap * n) (>= min) smallest distances
-// std::sort in the last two is unstable; canonical tie rule here and on the device: smaller index_query first.
+// std::sort in the last two is unstable; canonical tie rule here and on the device: earlier in the input first.
+// Distances may be any non-NaN float; -0.0 compares equal to +0.0, and a median that is -0.0 is reported as +0.0.
 enum { REJ_DISTANCE = 0, REJ_MEDIAN = 1, REJ_ONE_TO_ONE = 2, REJ_TRIMMED = 3, REJ_SURFACE_NORMAL = 4 };
 
 struct orc_rejector {
@@ -1422,7 +1423,7 @@ static void apply_rejector(const orc_rejector& r, std::vector<orc_corr>& c, doub
       d[i] = c[i].distance;
     std::vector<double> nth(d);
     std::nth_element(nth.begin(), nth.begin() + (nth.size() / 2), nth.end());
-    const double med = nth[nth.size() / 2];
+    const double med = nth[nth.size() / 2] + 0.0;  // -0.0 -> +0.0
     if (median_out)
       *median_out = med;
     for (size_t i = 0; i < c.size(); ++i)
@@ -1444,8 +1445,9 @@ static void apply_rejector(const orc_rejector& r, std::vector<orc_corr>& c, doub
       }
     }
   }
-  else {  // trimmed
-    unsigned keep = static_cast<unsigned>(std::floor(static_cast<float>(r.p) * static_cast<float>(c.size())));
+  else {  // trimmed; setOverlapRatio clamps in float (correspondence_rejection_trimmed.h:84), setMinCorrespondences is unsigned
+    const float overlap = std::min(1.0f, std::max(0.0f, static_cast<float>(r.p)));
+    unsigned keep = static_cast<unsigned>(std::floor(overlap * static_cast<float>(c.size())));
     keep = std::max(keep, static_cast<unsigned>(r.min_correspondences));
     if (keep < c.size()) {
       out = c;
@@ -1462,6 +1464,47 @@ ORC_API size_t orc_reject(const orc_rejector* r, const orc_corr* in, size_t n, o
 {
   std::vector<orc_corr> c(in, in + n);
   apply_rejector(*r, c, median_out);
+  std::copy(c.begin(), c.end(), out);
+  return c.size();
+}
+
+static inline bool surface_normal_keeps(const float* a, const float* b, double threshold);
+
+// The chain of the ICP loop (icp.hpp:187-201), with one tie rule for every stage: each rejector sees the survivors of
+// the one before in source-position order (the order of `c` on entry) and so breaks exact-distance ties by position,
+// even after a one-to-one, whose own output is in index_match order; the result is in position order too.  PCL's
+// std::sort is unstable, so it defines no other order.  SURFACE_NORMAL reads the normals at sn / tn (stride in floats).
+static void apply_chain(const orc_rejector* rej, int n_rej, std::vector<orc_corr>& c, const float* sn, size_t snstride,
+                        const float* tn, size_t tnstride, double* median_out)
+{
+  std::vector<int32_t> query(c.size());
+  for (size_t i = 0; i < c.size(); ++i) {  // index_query carries the position while the chain runs
+    query[i] = c[i].index_query;
+    c[i].index_query = static_cast<int32_t>(i);
+  }
+  for (int ri = 0; ri < n_rej; ++ri) {
+    if (rej[ri].kind == REJ_SURFACE_NORMAL) {
+      std::vector<orc_corr> kept;
+      for (const auto& x : c)
+        if (surface_normal_keeps(sn + snstride * (size_t)query[x.index_query], tn + tnstride * (size_t)x.index_match,
+                                 rej[ri].p))
+          kept.push_back(x);
+      c.swap(kept);
+      continue;
+    }
+    apply_rejector(rej[ri], c, median_out);
+    std::sort(c.begin(), c.end(), [](const orc_corr& a, const orc_corr& b) { return a.index_query < b.index_query; });
+  }
+  for (auto& x : c)
+    x.index_query = query[x.index_query];
+}
+
+// apply_chain on a list given in position order (kinds DISTANCE to TRIMMED); *median_out: the last MEDIAN stage's median
+ORC_API size_t orc_reject_chain(const orc_rejector* rej, int n_rej, const orc_corr* in, size_t n, orc_corr* out,
+                                double* median_out)
+{
+  std::vector<orc_corr> c(in, in + n);
+  apply_chain(rej, n_rej, c, nullptr, 0, nullptr, 0, median_out);
   std::copy(c.begin(), c.end(), out);
   return c.size();
 }
@@ -1674,18 +1717,10 @@ static void icp_run(const orc_icp_params& P, const float* src, size_t n_s, size_
     else
       nc = orc_correspondences(tree, cur.data(), n_s, ss, indices, n_idx, P.is_dense,
                                P.max_correspondence_distance, corr.data(), P.nthreads);
-    if (n_rejectors > 0) {  // icp.hpp:187-201: each rejector filters the previous one's output
+    if (n_rejectors > 0) {  // icp.hpp:187-201: each rejector filters the previous one's survivors (in position order)
       std::vector<orc_corr> cc(corr.begin(), corr.begin() + nc);
-      for (int ri = 0; ri < n_rejectors; ++ri) {
-        if (rejectors[ri].kind == REJ_SURFACE_NORMAL) {  // normals of the transformed source vs the target's
-          std::vector<orc_corr> kept(cc.size());
-          kept.resize(orc_reject_surface_normal(cc.data(), cc.size(), cur.data() + 4, ss, tgt + 4, ts,
-                                                rejectors[ri].p, kept.data()));
-          cc.swap(kept);
-          continue;
-        }
-        apply_rejector(rejectors[ri], cc, nullptr);
-      }
+      // surface normal: the normals of the transformed source vs the target's
+      apply_chain(rejectors, n_rejectors, cc, cur.data() + 4, ss, tgt + 4, ts, nullptr);
       nc = cc.size();
       std::copy(cc.begin(), cc.end(), corr.begin());
     }
@@ -1758,16 +1793,6 @@ ORC_API void orc_icp_align_tree(const orc_icp_params* P, void* h_tgt, const floa
     icp_run<double>(*P, src, n_s, sstride, indices, n_idx, tgt, n_t, tstride, guess, *R, out_cloud, h_tgt);
   else
     icp_run<float>(*P, src, n_s, sstride, indices, n_idx, tgt, n_t, tstride, guess, *R, out_cloud, h_tgt);
-}
-
-ORC_API void orc_icp_align_rej(const orc_icp_params* P, const orc_rejector* rej, int n_rej, const float* src,
-                               size_t n_s, size_t sstride, const float* tgt, size_t n_t, size_t tstride,
-                               orc_icp_result* R)
-{
-  if (P->scalar_is_double)
-    icp_run<double>(*P, src, n_s, sstride, nullptr, 0, tgt, n_t, tstride, nullptr, *R, nullptr, nullptr, rej, n_rej);
-  else
-    icp_run<float>(*P, src, n_s, sstride, nullptr, 0, tgt, n_t, tstride, nullptr, *R, nullptr, nullptr, rej, n_rej);
 }
 
 // Everything at once: rejector chain + kept target tree + source indices + guess + the criteria / estimator knobs, and

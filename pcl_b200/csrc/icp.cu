@@ -1205,13 +1205,20 @@ __global__ void k_matches_to_corr(const float4* __restrict__ cur, const Match* _
   by_slot[slot] = r;
 }
 
+// whether a loop has evaluated correspondences since its last reset: a loop that stopped with NO_CORRESPONDENCES in its
+// first evaluation (iterations == 0) keeps the list that stopped it, as correspondences_ does (icp.hpp:204-213)
+static bool has_evaluated(const LoopCtrl& L)
+{
+  return L.iterations > 0 || L.state != PCLB200_CONV_NOT_CONVERGED;
+}
+
 size_t icp_get_correspondences(Icp& s, pclb200_corr* out)
 {
   Ctx& c = *s.ctx;
   cudaStream_t st = c.stream;
   PCLB_REQUIRE(!s.batch.B, PCLB200_ERR_INVALID, "icp: a batch session hands its lists out through get_correspondences_batch");
   PCLB_REQUIRE(s.tgt && s.cur.p && s.match.p, PCLB200_ERR_INVALID, "icp: no iteration has run");
-  if (!s.n_q || s.loop.iterations == 0)
+  if (!s.n_q || !has_evaluated(s.loop))
     return 0;
   DevBuf<pclb200_corr> by_slot;
   by_slot.alloc(s.n_q, st);
@@ -1633,7 +1640,7 @@ void icp_get_correspondences_batch(Icp& s, pclb200_corr* out, int64_t* counts)
     k_matches_to_corr<<<grid_for(n, 256), 256, 0, st>>>(s.cur.p, s.match.p, n, s.tgt->pts.p, b.rel.p, by_slot.p);
   std::vector<int> live(B);
   for (int p = 0; p < B; ++p)
-    live[p] = b.loop[p].iterations > 0;
+    live[p] = has_evaluated(b.loop[p]);
   DevBuf<int> d_live;
   DevBuf<unsigned long long> d_counts;
   d_live.alloc(B, st);

@@ -10,7 +10,8 @@
 //   CorrespondenceRejectorTrimmed         registration/src/correspondence_rejection_trimmed.cpp:44-63
 //       keep = max(floor(overlap * float(n)), min); if keep < n: sort by distance, keep the first `keep`
 // The reference sorts with the unstable std::sort; the canonical tie rule here (and in the oracle) is "earlier in the
-// input first", obtained with stable radix sorts.
+// input first", obtained with stable radix sorts.  Inside the ICP loop the input of every rejector is the survivors in
+// source-position order (the tie key is the source position), whatever the rejector before it emitted.
 //
 // All four work on flat per-correspondence arrays {d2, match, tie-break, accepted} so the same code serves the
 // stand-alone C entry point (pclb200_reject) and the in-loop form (rejectors applied to the ICP's Match array with no
@@ -25,6 +26,19 @@
 #include "reject_sharded_kernels.cuh"
 
 namespace pclb200 {
+
+// TRIMMED's parameters as CorrespondenceRejectorTrimmed stores them (correspondence_rejection_trimmed.h:84, 103-106): the
+// overlap ratio as min(1, max(0, float(p))) (NaN gives 0), the minimum count as the unsigned int setMinCorrespondences
+// takes (the int32 field's bits, so -1 is 2^32 - 1)
+static float trimmed_overlap(const pclb200_rejector& r)
+{
+  return std::min(1.0f, std::max(0.0f, (float)r.p));
+}
+
+static unsigned trimmed_min(const pclb200_rejector& r)
+{
+  return (unsigned)r.min_correspondences;
+}
 
 // Applies one rejector to the arrays.  perm / keep_sorted (nullable, n entries): for ONE_TO_ONE and TRIMMED the sorted
 // order of the input positions and which of them survive, so a caller can emit the output in the reference's order.
@@ -84,8 +98,8 @@ void apply_rejector(Ctx& c, const pclb200_rejector& r, const RejectArrays& a, in
   PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, k64_in.p, k64_out.p, v_in.p, v_out.p, (int)n, 0, 64, st));
   c.launches += 10;
   if (r.kind == PCLB200_REJ_TRIMMED) {
-    k_rej_trim<<<g, 256, 0, st>>>(v_out.p, n, count.p, (float)r.p, (unsigned)std::max(r.min_correspondences, 0), a.acc,
-                                  keep_sorted, trimmed_flag);
+    k_rej_trim<<<g, 256, 0, st>>>(v_out.p, n, count.p, trimmed_overlap(r), trimmed_min(r), a.acc, keep_sorted,
+                                  trimmed_flag);
     ++c.launches;
     if (perm)
       PCLB_CUDA(cudaMemcpyAsync(perm, v_out.p, n * sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -141,8 +155,8 @@ void apply_rejector_sharded(Ctx& c, const pclb200_rejector& r, const RejectArray
       else
         k_sel_hist<false><<<hg, 256, 0, st>>>(a.d2, a.tie, a.acc, n, s.offset, shift, p == 0, sel.p, hist.p);
       comm_allreduce_u64(c, hist.p, hist.p, kSelBins, kU64Sum);
-      k_sel_decide<<<1, 1, 0, st>>>(hist.p, shift, p == 0, p == passes - 1, r.kind, (float)r.p,
-                                    (unsigned)std::max(r.min_correspondences, 0), r.p, sel.p, info.p);
+      k_sel_decide<<<1, 1, 0, st>>>(hist.p, shift, p == 0, p == passes - 1, r.kind, trimmed_overlap(r), trimmed_min(r),
+                                    r.p, sel.p, info.p);
       c.launches += 2;
     }
     if (wide)

@@ -23,12 +23,25 @@ __global__ void k_rej_distance(const float* __restrict__ d2, int* __restrict__ a
     acc[i] = 0;
 }
 
+// A caller's list may hold any non-NaN distance: -0.0 becomes +0.0 (the reference compares them equal), then the sign
+// flip makes the unsigned order of the bits the order of the values, negatives and +inf included.
+__device__ __forceinline__ unsigned rej_key(float d)
+{
+  const unsigned u = __float_as_uint(d) == 0x80000000u ? 0u : __float_as_uint(d);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+__device__ __forceinline__ float rej_key_value(unsigned k)
+{
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
 __global__ void k_rej_keys32(const float* __restrict__ d2, const int* __restrict__ acc, size_t n,
                              unsigned* __restrict__ keys)
 {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i < n)
-    keys[i] = acc[i] ? __float_as_uint(d2[i]) : 0xffffffffu;  // d2 >= 0: the bit pattern orders like the value
+    keys[i] = acc[i] ? rej_key(d2[i]) : 0xffffffffu;
 }
 
 // median = sorted[count / 2]; threshold = median * factor in double (correspondence_rejection_median_distance.cpp:57-65)
@@ -41,7 +54,7 @@ __global__ void k_rej_median(const unsigned* __restrict__ sorted, const unsigned
     out[1] = -1.0;
     return;
   }
-  const double med = (double)__uint_as_float(sorted[c / 2]);
+  const double med = (double)rej_key_value(sorted[c / 2]);
   out[0] = med;
   out[1] = med * factor;
 }
@@ -61,7 +74,7 @@ __global__ void k_rej_keys64(const float* __restrict__ d2, const unsigned* __res
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n)
     return;
-  keys[i] = acc[i] ? (((unsigned long long)__float_as_uint(d2[i]) << 32) | tie[i]) : ~0ULL;
+  keys[i] = acc[i] ? (((unsigned long long)rej_key(d2[i]) << 32) | tie[i]) : ~0ULL;
   vals[i] = (int)i;
 }
 

@@ -7,7 +7,8 @@
 //   one-to-one: per target record the smallest (distance, global position) key over all ranks, through one u64 table per
 //     rank (k_o2o_min / k_o2o_keep / k_o2o_reset).
 // Keys: median d2 bits (32-bit); trimmed and one-to-one (d2 bits << 32) | (offset + slot), unique, ordered like the
-// single process's (distance, input position) sort.  A header of its own so that tests/host/reject_sharded_host_test.cpp
+// single process's (distance, input position) sort: the loop's squared distances are never negative or -0.0, so their
+// raw bits order like reject_kernels.cuh's rej_key.  A header of its own so that tests/host/reject_sharded_host_test.cpp
 // can compile the kernels for the host and simulate several ranks in one process.
 #pragma once
 #include "internal.cuh"

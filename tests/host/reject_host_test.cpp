@@ -8,7 +8,7 @@
 #include "host_index.h"
 #include "check.h"
 
-
+#include <cfloat>
 
 struct orc_rejector { int32_t kind, min_correspondences; double p; };
 extern "C" size_t orc_reject(const orc_rejector* r, const pclb200_corr* in, size_t n, pclb200_corr* out, double* median_out);
@@ -87,6 +87,12 @@ int main(int argc, char** argv)
   {
     Scene s{"every distance equal", {}};
     for (int i = 0; i < 1200; ++i) s.c.push_back(pclb200_corr{i, i % 300, 0.0025f});
+    scenes.push_back(std::move(s));
+  }
+  {  // any non-NaN distance a caller may pass: -0.0 equal to +0.0, negatives before zero, +inf after FLT_MAX
+    Scene s{"signed distances, -0.0, inf", {}};
+    const float v[] = {0.f, -0.f, -1e-3f, 2e-3f, -2e-3f, 1e-40f, -1e-40f, FLT_MAX, INFINITY, -INFINITY, 5e-4f, -0.f};
+    for (int i = 0; i < 600; ++i) s.c.push_back(pclb200_corr{i, (int)(U(rng) * 150), v[i % 12]});
     scenes.push_back(std::move(s));
   }
   for (const Scene& s : scenes) {

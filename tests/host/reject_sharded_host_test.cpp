@@ -18,7 +18,8 @@ static inline unsigned long long atomicMin(unsigned long long* p, unsigned long 
 template <typename T> static inline T __ldcv(const T* p) { return *p; }
 
 struct orc_rejector { int32_t kind, min_correspondences; double p; };
-extern "C" size_t orc_reject(const orc_rejector* r, const pclb200_corr* in, size_t n, pclb200_corr* out, double* median_out);
+extern "C" size_t orc_reject_chain(const orc_rejector* r, int n_r, const pclb200_corr* in, size_t n, pclb200_corr* out,
+                                   double* median_out);
 
 #include "reject_twin.h"
 #include "../../pcl_b200/csrc/reject_sharded_kernels.cuh"
@@ -68,7 +69,7 @@ static void apply_sharded(World& w, const pclb200_rejector& r, int o2o_mode, dou
       for (int q = 0; q < R; ++q) for (int b = 0; b < kSelBins; ++b) sum[b] += hist[q][b];
       for (int q = 0; q < R; ++q) {
         hist[q] = sum;
-        k_sel_decide(hist[q].data(), shift, p == 0, p == passes - 1, r.kind, (float)r.p, (unsigned)std::max(r.min_correspondences, 0), r.p, &sel[q], info[q].data());
+        k_sel_decide(hist[q].data(), shift, p == 0, p == passes - 1, r.kind, std::min(1.0f, std::max(0.0f, (float)r.p)), (unsigned)r.min_correspondences, r.p, &sel[q], info[q].data());
         for (int b = 0; b < kSelBins; ++b) CHECK(hist[q][b] == 0, "histogram not cleared");
       }
     }
@@ -122,14 +123,16 @@ static std::vector<pclb200_corr> survivors(const World& w)
   return out;
 }
 
-static std::vector<pclb200_corr> oracle(const pclb200_rejector& r, const std::vector<pclb200_corr>& in, double* median)
+// the oracle's chain of the ICP loop: every stage sees the survivors in position order, and so does the result
+static std::vector<pclb200_corr> oracle(const std::vector<pclb200_rejector>& chain, const std::vector<pclb200_corr>& in,
+                                        double* median)
 {
   std::vector<pclb200_corr> out(in.size() ? in.size() : 1);
-  const orc_rejector o{r.kind, r.min_correspondences, r.p};
+  std::vector<orc_rejector> o;
+  for (const pclb200_rejector& r : chain) o.push_back(orc_rejector{r.kind, r.min_correspondences, r.p});
   double m = 0.0;
-  out.resize(in.empty() ? 0 : orc_reject(&o, in.data(), in.size(), out.data(), &m));
+  out.resize(in.empty() ? 0 : orc_reject_chain(o.data(), (int)o.size(), in.data(), in.size(), out.data(), &m));
   if (median) *median = m;
-  std::sort(out.begin(), out.end(), [](const pclb200_corr& a, const pclb200_corr& b) { return a.index_query < b.index_query; });
   return out;
 }
 
@@ -145,15 +148,13 @@ static void check_chain(const char* scene, const World& w0, const std::vector<pc
 {
   for (int mode : {kPeer, kNccl}) {
     World w = w0;
-    std::vector<pclb200_corr> o = survivors(w);
-    for (const pclb200_rejector& r : chain) {
-      double med = -7, omed = -8;
-      const size_t c = o.size();
+    double med = -7, omed = -8;
+    const std::vector<pclb200_corr> in = survivors(w);
+    for (const pclb200_rejector& r : chain)
       apply_sharded(w, r, mode, &med);
-      o = oracle(r, o, &omed);
-      if (chain.size() == 1 && r.kind == PCLB200_REJ_MEDIAN && c > 0)
-        CHECK(std::memcmp(&med, &omed, 8) == 0, "%s, R=%zu: median %.9g, the oracle's %.9g", scene, w.ranks.size(), med, omed);
-    }
+    const std::vector<pclb200_corr> o = oracle(chain, in, &omed);
+    if (chain.size() == 1 && chain[0].kind == PCLB200_REJ_MEDIAN && !in.empty())
+      CHECK(std::memcmp(&med, &omed, 8) == 0, "%s, R=%zu: median %.9g, the oracle's %.9g", scene, w.ranks.size(), med, omed);
     const std::vector<pclb200_corr> g = survivors(w);
     CHECK(same(g, o), "%s, R=%zu, %s, chain of %zu starting with %s p=%g min=%d: %zu survivors, the oracle keeps %zu", scene,
           w.ranks.size(), mode == kPeer ? "peer tables" : "NCCL min", chain.size(), kind_name(chain[0].kind), chain[0].p,

@@ -57,7 +57,8 @@ static void apply_rejector(const pclb200_rejector& r, Arrays& a, std::vector<int
     for (size_t j = 0; j < n; ++j) v_out[j] = v_in[order[j]];
   }
   if (r.kind == PCLB200_REJ_TRIMMED) {
-    launch(g, 256, [&] { k_rej_trim(v_out.data(), n, &count, (float)r.p, (unsigned)std::max(r.min_correspondences, 0), a.acc.data(), keep_sorted.data(), &trimmed_flag); });
+    const float overlap = std::min(1.0f, std::max(0.0f, (float)r.p));  // reject.cu: trimmed_overlap / trimmed_min
+    launch(g, 256, [&] { k_rej_trim(v_out.data(), n, &count, overlap, (unsigned)r.min_correspondences, a.acc.data(), keep_sorted.data(), &trimmed_flag); });
     perm = v_out;
     return;
   }
