@@ -19,7 +19,8 @@
  * rejector chain, use_reciprocal, a correspondence_kind other than NEAREST, an active communicator or a sharded target,
  * and the symmetric objective without source normals.
  *
- * The targets of such a batch can themselves be built as one batch (pclb200_index_build_batch). */
+ * The targets of such a batch can themselves be built as one batch (pclb200_index_build_batch), and their normals for
+ * point-to-plane or the symmetric objective estimated as one batch (pclb200_normals_knn_batch). */
 #ifndef PCLB200_BATCH_H_
 #define PCLB200_BATCH_H_
 
@@ -79,6 +80,25 @@ PCLB200_API int pclb200_icp_get_correspondences_batch(pclb200_icp* icp, pclb200_
  * finite point (pclb200_last_error names it). */
 PCLB200_API int pclb200_index_build_batch(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
                                           const int64_t* offsets, int32_t n_clouds, pclb200_index** out);
+
+/* The k-NN normals of a batch of query sets, each against its own index, in one call: query set c = records
+ * [offsets[c], offsets[c+1]) of pts, searched in indices[c].  Row i of out (n rows of {nx, ny, nz, curvature}) belongs to
+ * record i and is bit for bit what pclb200_normals_knn(ctx, indices[c], pts + offsets[c] * stride, its record count,
+ * stride, NULL, 0, 1, k, viewpoint c, out + 4 offsets[c], &d_c) writes, and is_dense_out[c] (host, nullable, n_clouds
+ * entries) is that call's d_c.  A query set need not be the cloud its index was built from, and a handle may repeat; every
+ * handle pclb200_normals_knn accepts is accepted, from single builds or from pclb200_index_build_batch.
+ *
+ * pts and out: host or device, with the stride rules of pclb200_normals_knn.  offsets: host, n_clouds + 1 entries.
+ * viewpoints: host, nullable, n_clouds rows of xyz; NULL = (0, 0, 0) for every set, PCL's default.  Every k the single call
+ * takes is taken.  Each stage is one launch for the whole batch, whatever n_clouds is, and the call reads the flags back
+ * and synchronises the context's stream once.  PCLB200_ERR_INVALID, with out and is_dense_out untouched, for n_clouds
+ * outside 1 to 65536, a NULL indices, handle, pts, offsets or out, offsets[0] != 0, a query set with no records,
+ * offsets[n_clouds] != n, n >= 2^31 - 1, a bad stride, k <= 0, a handle on another device than the context, and what
+ * pclb200_normals_knn refuses of a handle (k > 32 on an index built with caller ids). */
+PCLB200_API int pclb200_normals_knn_batch(pclb200_ctx* ctx, const pclb200_index* const* indices, int32_t n_clouds,
+                                          const void* pts, size_t n, size_t stride, const int64_t* offsets, int k,
+                                          const float* viewpoints /* nullable: n_clouds x 3 */, float* out,
+                                          int32_t* is_dense_out /* nullable: n_clouds */);
 
 #ifdef __cplusplus
 }

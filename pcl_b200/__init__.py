@@ -87,7 +87,7 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
 # every symbol include/pclb200_batch.h declares (a batch of ICP problems in one session; tests/test_icp_batch_symbols.py)
 BATCH_SYMBOLS = ["pclb200_icp_set_target_batch", "pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch",
-                 "pclb200_index_build_batch"]
+                 "pclb200_index_build_batch", "pclb200_normals_knn_batch"]
 
 _lib = None
 
@@ -187,6 +187,7 @@ def lib():
     L.pclb200_icp_iterate_batch.argtypes = [vp, C.c_int, vp]
     L.pclb200_icp_get_correspondences_batch.argtypes = [vp, vp, vp]
     L.pclb200_index_build_batch.argtypes = [vp, vp, sz, sz, vp, C.c_int32, vp]
+    L.pclb200_normals_knn_batch.argtypes = [vp, vp, C.c_int32, vp, sz, sz, vp, C.c_int, fp, vp, vp]
     for s in SYMBOLS + SHARDED_SYMBOLS + BATCH_SYMBOLS:
         getattr(L, s)  # AttributeError here == header and library disagree
     _lib = L
@@ -311,6 +312,31 @@ class Context:
         out = (C.c_void_p * max(nc, 1))()
         _check(lib().pclb200_index_build_batch(self.h, b.ptr, b.rows, b.stride, C.c_void_p(off.ctypes.data), nc, out))
         return [Index._adopt(self, out[c], off[c + 1] - off[c]) for c in range(nc)]
+
+    def normals_knn_batch(self, indices, cloud, offsets, k, viewpoints=None, out=None):
+        """The k-NN normals of B query sets in one call: set c = the records [offsets[c], offsets[c+1]) of `cloud` (numpy,
+        or a torch tensor on the host or the device), searched in indices[c]; each set's rows and is_dense are bit for
+        bit indices[c].normals_knn(its records, k, its viewpoint).  viewpoints: None (the origin), one xyz for every set
+        or (B, 3).  Returns (out (n, 4), is_dense (B,) bool); out[offsets[c]:offsets[c+1]] are set c's normals, as
+        Icp.set_target_batch takes them."""
+        b = _Buf(cloud)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        B = max(off.size - 1, 0)
+        handles = (C.c_void_p * max(B, 1))(*[None if i is None else i.h for i in indices])
+        vp = None
+        if viewpoints is not None:
+            v = np.asarray(viewpoints, dtype=np.float32)
+            vp = np.ascontiguousarray(np.broadcast_to(v, (B, 3)) if v.ndim == 1 else v, dtype=np.float32)
+            if vp.shape != (B, 3):
+                raise ValueError("normals_knn_batch: viewpoints must be one xyz or one row of xyz per set")
+        if out is None:
+            out = np.empty((b.rows, 4), dtype=np.float32)
+        ob = _Buf(out)
+        dense = np.zeros(max(B, 1), dtype=np.int32)
+        _check(lib().pclb200_normals_knn_batch(self.h, handles, B, b.ptr, b.rows, b.stride, C.c_void_p(off.ctypes.data),
+                                               int(k), None if vp is None else vp.ctypes.data_as(C.POINTER(C.c_float)),
+                                               ob.ptr, C.c_void_p(dense.ctypes.data)))
+        return out, dense[:B].astype(bool)
 
     def comm_init(self, rank, nranks, unique_id_bytes):
         buf = C.create_string_buffer(bytes(unique_id_bytes), 128)

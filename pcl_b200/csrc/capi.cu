@@ -971,6 +971,71 @@ int pclb200_normals_knn(pclb200_ctx* ctx, const pclb200_index* h, const void* pt
   });
 }
 
+int pclb200_normals_knn_batch(pclb200_ctx* ctx, const pclb200_index* const* indices, int32_t n_clouds, const void* pts,
+                              size_t n, size_t stride, const int64_t* offsets, int k, const float* viewpoints, float* out,
+                              int32_t* is_dense_out)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    PCLB_REQUIRE(n_clouds >= 1 && n_clouds <= 65536, PCLB200_ERR_INVALID, "normals_knn_batch: a batch holds 1 to 65536 query sets");
+    PCLB_REQUIRE(indices && pts && offsets && out, PCLB200_ERR_INVALID, "NULL argument");
+    const int B = n_clouds;
+    std::vector<Index*> idx(B);
+    for (int b = 0; b < B; ++b) {
+      PCLB_REQUIRE(indices[b] && indices[b]->idx, PCLB200_ERR_INVALID, "normals_knn_batch: a NULL handle");
+      PCLB_REQUIRE(indices[b]->idx->device == c.device, PCLB200_ERR_INVALID,
+                   "normals_knn_batch: an index lives on another device than the context");
+      idx[b] = indices[b]->idx;
+    }
+    PCLB_REQUIRE(offsets[0] == 0 && offsets[B] == (int64_t)n, PCLB200_ERR_INVALID,
+                 "normals_knn_batch: offsets must run from 0 to n");
+    for (int b = 0; b < B; ++b)
+      PCLB_REQUIRE(offsets[b + 1] > offsets[b], PCLB200_ERR_INVALID,
+                   "normals_knn_batch: offsets must increase strictly (every query set holds a record)");
+    PCLB_REQUIRE(n < (size_t)0x7fffffff, PCLB200_ERR_INVALID, "normals_knn_batch: a batch holds fewer than 2^31 - 1 records");
+    PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
+    PCLB_REQUIRE(k > 0, PCLB200_ERR_INVALID, "k must be positive (feature.hpp:135-176)");
+    cudaStream_t st = c.stream;
+    std::vector<float> vps(3 * (size_t)B, 0.f);
+    if (viewpoints)
+      std::copy(viewpoints, viewpoints + 3 * (size_t)B, vps.begin());
+    // every record once, keyed in its own index's frame, then stably by set: each set's queries in its single call's order
+    std::vector<float4> frames(B);
+    for (int b = 0; b < B; ++b)
+      frames[b] = make_float4(idx[b]->lo[0], idx[b]->lo[1], idx[b]->lo[2], idx[b]->morton_scale);
+    DevBuf<float4> d_frames, dense;
+    DevBuf<long long> d_offsets;
+    d_frames.alloc(B, st);
+    d_offsets.alloc(B + 1, st);
+    PCLB_CUDA(cudaMemcpyAsync(d_frames.p, frames.data(), B * sizeof(float4), cudaMemcpyHostToDevice, st));
+    PCLB_CUDA(cudaMemcpyAsync(d_offsets.p, offsets, (B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+    dense.alloc(n, st);
+    load_xyz_as_float4(c, pts, n, stride, nullptr, 0, dense.p, st);
+    QueryBatch qb;
+    {
+      ProfScope ps(c, "query_sort");
+      make_query_batch_framed(c, d_frames.p, d_offsets.p, B, dense.p, n, qb);
+      sort_by_problem(c, d_offsets.p, B, qb);
+    }
+    DevBuf<float4> tmp;
+    DevBuf<int> d_flags;
+    d_flags.alloc(B, st);
+    PCLB_CUDA(cudaMemsetAsync(d_flags.p, 0, B * sizeof(int), st));
+    float4* const caller_out = reinterpret_cast<float4*>(out);
+    {
+      ProfScope ps(c, "normals_batch");
+      launch_normals_batch(c, idx.data(), B, d_offsets.p, qb.q.p, n, k, vps.data(), out_on_device(c, caller_out, n, tmp),
+                           d_flags.p);
+    }
+    std::vector<int> flags(B);
+    PCLB_CUDA(cudaMemcpyAsync(flags.data(), d_flags.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    copy_out(c, caller_out, tmp, n);
+    check_device_error(c);
+    if (is_dense_out)
+      for (int b = 0; b < B; ++b)
+        is_dense_out[b] = flags[b] ? 0 : 1;
+  });
+}
+
 int pclb200_normals_radius(pclb200_ctx* ctx, const pclb200_index* h, const void* pts, size_t n, size_t stride,
                            const int32_t* indices, size_t n_idx, int is_dense, double radius, const float viewpoint[3],
                            float* out, int* is_dense_out)

@@ -1251,6 +1251,34 @@ __global__ void k_gather_by(const float4* __restrict__ q, const int32_t* __restr
     out[j] = q[vals[j]];
 }
 
+void sort_by_problem(Ctx& c, const long long* d_offsets, int n_problems, QueryBatch& qb)
+{
+  cudaStream_t st = c.stream;
+  const size_t n = qb.n;
+  DevBuf<unsigned> keys_in, keys;
+  DevBuf<int32_t> vals_in, vals;
+  keys_in.alloc(n, st);
+  keys.alloc(n, st);
+  vals_in.alloc(n, st);
+  vals.alloc(n, st);
+  k_problem_keys<<<grid_for(n, 256), 256, 0, st>>>(qb.q.p, n, d_offsets, n_problems, keys_in.p, vals_in.p);
+  ++c.launches;
+  int bits = 1;
+  while ((1 << bits) < n_problems)
+    ++bits;
+  size_t tmp_bytes = 0;
+  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, bits, st));
+  DevBuf<unsigned char> tmp;
+  tmp.alloc(tmp_bytes, st);
+  PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, bits, st));
+  c.launches += 2;
+  DevBuf<float4> sorted;
+  sorted.alloc(n, st);
+  k_gather_by<<<grid_for(n, 256), 256, 0, st>>>(qb.q.p, vals.p, n, sorted.p);
+  ++c.launches;
+  qb.q = std::move(sorted);
+}
+
 __global__ void k_relative_index(const long long* __restrict__ offsets, int n_problems, size_t n, int32_t* __restrict__ rel)
 {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
@@ -1423,28 +1451,7 @@ void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, cons
     ProfScope ps(c, "query_sort");
     if (per_target)  // src_all holds the staged xyz
       make_query_batch_framed(c, s.targets.frames.p, b.d_offsets.p, B, s.src_all.p, n, qb);
-    DevBuf<unsigned> keys_in, keys;
-    DevBuf<int32_t> vals_in, vals;
-    keys_in.alloc(n, st);
-    keys.alloc(n, st);
-    vals_in.alloc(n, st);
-    vals.alloc(n, st);
-    k_problem_keys<<<grid_for(n, 256), 256, 0, st>>>(qb.q.p, n, b.d_offsets.p, B, keys_in.p, vals_in.p);
-    ++c.launches;
-    int bits = 1;
-    while ((1 << bits) < B)
-      ++bits;
-    size_t tmp_bytes = 0;
-    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, bits, st));
-    DevBuf<unsigned char> tmp;
-    tmp.alloc(tmp_bytes, st);
-    PCLB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys_in.p, keys.p, vals_in.p, vals.p, (int)n, 0, bits, st));
-    c.launches += 2;
-    DevBuf<float4> sorted;
-    sorted.alloc(n, st);
-    k_gather_by<<<grid_for(n, 256), 256, 0, st>>>(qb.q.p, vals.p, n, sorted.p);
-    ++c.launches;
-    qb.q = std::move(sorted);
+    sort_by_problem(c, b.d_offsets.p, B, qb);
   }
   finish_source(s, qb, src_normals, stride_n);
   b.rel.alloc(n, st);

@@ -323,6 +323,9 @@ __host__ __device__ __forceinline__ int problem_of(const long long* offsets, int
 // that problem's frame; the problems interleave until a stable sort by problem follows.
 void make_query_batch_framed(Ctx& c, const float4* d_frames, const long long* d_offsets, int n_problems,
                              const float4* d_q, size_t n, QueryBatch& out);
+// stably sorts the query batch qb by the problem of each query's record (w; d_offsets: B + 1 entries, device), so that the
+// queries of problem p fill [offsets[p], offsets[p+1]) in the order they had
+void sort_by_problem(Ctx& c, const long long* d_offsets, int n_problems, QueryBatch& qb);
 // load_xyz_as_float4 of a caller's query points into `dense` (kept alive: some kernels read it in input order), then
 // make_query_batch over it
 QueryBatch load_queries(Ctx& c, const Index& ref_frame, const void* pts, size_t n, size_t stride, const int32_t* subset,
@@ -362,6 +365,11 @@ void launch_normals(Ctx& c, Index& idx, const float4* d_q, size_t nq, int k, con
                     int* d_not_dense);
 void launch_normals_radius(Ctx& c, Index& idx, const float4* d_q, size_t nq, float r2, const float vp[3], float4* d_out,
                            int* d_not_dense);
+// the k-NN normals of B query sets in one launch sequence: d_q = the queries of every set, sorted by set (set b fills
+// [offsets[b], offsets[b+1]) of d_q, d_offsets on the device) and each in the order of idx[b]'s frame, w = the query's
+// row in d_out; set b is searched in idx[b], flipped towards vps[3b..3b+2] (host) and flags d_flags[b] (zeroed)
+void launch_normals_batch(Ctx& c, Index* const* idx, int B, const long long* d_offsets, const float4* d_q, size_t nq, int k,
+                          const float* vps, float4* d_out, int* d_flags);
 void launch_knn_stats(Ctx& c, const Index& idx, const float4* d_q, size_t nq, int k, float* d_mean, float* d_kth);
 // launch_knn_stats's d_kth through materialised k-NN lists (nq * k entries of scratch), whatever k: the warp-cooperative
 // search answers k = 12..32 on an index with a cell table, much faster than the per-thread statistics kernel

@@ -227,247 +227,50 @@ k_knn_warp(const TreeView T, const int2* __restrict__ node_leaves, int b_start, 
            int k, int32_t* __restrict__ out_idx, float* __restrict__ out_d2, float vpx, float vpy, float vpz,
            float4* __restrict__ out_n, int* __restrict__ not_dense, unsigned char* __restrict__ redo)
 {
-  __shared__ int s_pos[NORMALS ? 8 : 1][NORMALS ? 32 : 1][NORMALS ? 33 : 1];  // per warp: 32 queries x k neighbour positions (+1: no bank conflicts)
-  __shared__ float s_cd[8][64];  // per warp: buffered candidates (d2, original index, Morton position)
-  __shared__ int s_ci[8][64];
-  __shared__ int s_cp[8][64];
-  const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned lt = (1u << lane) - 1u;
-  const CellTable& C = T.cells;
-  const float inf = __int_as_float(0x7f800000);
-  const float qnan = __int_as_float(0x7fc00000);
-  const size_t n_warps = (size_t)gridDim.x * (blockDim.x >> 5);
-  const size_t n_batches = (nq + 31) / 32;
-  for (size_t batch = (size_t)blockIdx.x * (blockDim.x >> 5) + warp; batch < n_batches; batch += n_warps) {
-    int my_state = 0;  // epilogue (NORMALS): state of query batch*32 + lane: 0 = none, 1 = list ready, 2 = NaN row, 3 = redo
-    for (int t = 0; t < 32; ++t) {
-      const size_t qi = batch * 32 + t;
-      if (qi >= nq)
-        break;
-      const float4 qq = __ldg(q + qi);
-      const size_t slot = (size_t)(unsigned)__float_as_int(qq.w);
-      if (!(isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z))) {
-        if (NORMALS) {
-          if (lane == t)
-            my_state = 2;
-        }
-        else if (lane < k) {
-          out_idx[slot * k + lane] = -1;
-          out_d2[slot * k + lane] = inf;
-        }
-        continue;
-      }
-      const unsigned cqx = morton_cell(qq.x, C.lo[0], C.scale), cqy = morton_cell(qq.y, C.lo[1], C.scale),
-                     cqz = morton_cell(qq.z, C.lo[2], C.scale);
-      float ld = inf;
-      int li = kSentinelIndex, lp = -1;
-      bool done = false;
-      // attempts: [a ball sized for ~1.4 k points of this cloud's density, when that is well inside half a cell of the
-      // start level,] then half a cell of the start level, then of every coarser level
-      for (int attempt = 0; !done; ++attempt) {
-        const bool sized = r_first > 0.f && attempt == 0;
-        const int b = b_start - (r_first > 0.f ? max(attempt - 1, 0) : attempt);
-        if (b < 1)
-          break;
-        const int s = 21 - b;
-        const float R = sized ? r_first : __fmul_rd(__fmul_rd(0.5f * (float)(1u << s), C.inv_scale), 0.999f);
-        const unsigned ax = morton_cell(__fsub_rd(qq.x, R), C.lo[0], C.scale), bx = morton_cell(__fadd_ru(qq.x, R), C.lo[0], C.scale);
-        const unsigned ay = morton_cell(__fsub_rd(qq.y, R), C.lo[1], C.scale), by = morton_cell(__fadd_ru(qq.y, R), C.lo[1], C.scale);
-        const unsigned az = morton_cell(__fsub_rd(qq.z, R), C.lo[2], C.scale), bz = morton_cell(__fadd_ru(qq.z, R), C.lo[2], C.scale);
-        if ((bx >> s) - (ax >> s) > 1u || (by >> s) - (ay >> s) > 1u || (bz >> s) - (az >> s) > 1u)
-          continue;  // (rounding at a cell edge) the box needs the next coarser level
-        const unsigned hx = cqx >> s, hy = cqy >> s, hz = cqz >> s;
-        const unsigned ox = (ax >> s) + (bx >> s) - hx, oy = (ay >> s) + (by >> s) - hy, oz = (az >> s) + (bz >> s) - hz;
-        const unsigned E = (ox != hx ? 1u : 0u) | (oy != hy ? 2u : 0u) | (oz != hz ? 4u : 0u);
-        // lanes 0..7 look one cell up each; a leaf that spans several cells comes back several times: keep one
-        int ref = kDone;
-        if (lane < 8 && ((unsigned)lane & ~E) == 0u)
-          ref = cell_lookup(C, cell_key(b, (lane & 1) ? ox : hx, (lane & 2) ? oy : hy, (lane & 4) ? oz : hz));
-        const unsigned grp = __match_any_sync(full, ref != kDone ? ref : (int)(0x40000000 | lane));
-        // a leaf shared by several cells is kept once, by the lowest lane, whose cell need not be the nearest of them
-        // (cells 3 and 5 share a leaf, cell 1 is empty): such an entry is never pruned by a cell bound
-        const bool shared = ref != kDone && (grp & (grp - 1u)) != 0u;
-        if (ref != kDone && (grp & lt) != 0u)
-          ref = kDone;
-        int first = 0, cnt = 0;
-        if (ref != kDone) {
-          if (ref < 0) {
-            first = ~ref;
-            cnt = 1;
-          }
-          else {
-            const int2 r = __ldg(node_leaves + ref);
-            first = r.x;
-            cnt = r.y;
-          }
-        }
-        int tot = cnt;
-#pragma unroll
-        for (int o = 4; o > 0; o >>= 1)
-          tot += __shfl_xor_sync(full, tot, o);
-        tot = __shfl_sync(full, tot, 0);
-        if (tot > kWarpKnnMaxLeaves)
-          break;  // a dense knot (duplicates): the exact walk prunes it, a brute-force gather would not
-        ld = inf;
-        li = kSentinelIndex;
-        lp = -1;
-        // Candidates that beat the current k-th are only APPENDED to a per-warp buffer; the list is updated (sort + merge,
-        // or a few ranked insertions) when 32 have collected and at the end of the home cell, so the expensive network
-        // runs once per ~32 survivors instead of once per round.  A stale threshold only admits extra candidates.
-        // the running threshold starts at the certification radius: a candidate beyond it cannot be part of a certified
-        // answer, so only the points inside the ball (~k..2k of the few hundred gathered) ever reach the sorting network
-        const float R2cert = __fmul_rd(__fmul_rd(R, R), 0.999998f);
-        float Tk = R2cert;
-        int Ti = kSentinelIndex;
-        int nbuf = 0;
-        bool have_list = false;
-        auto flush = [&](int take) {  // fold the first `take` (<= 32) buffered candidates into the list
-          float cd = inf;
-          int ci = kSentinelIndex, cp = -1;
-          if (lane < take) {
-            cd = s_cd[warp][lane];
-            ci = s_ci[warp][lane];
-            cp = s_cp[warp][lane];
-          }
-          if (!have_list || take > 12) {
-            warp_sort32(cd, ci, cp, lane);
-            if (have_list)
-              warp_merge32(ld, li, lp, cd, ci, cp, lane);
-            else {  // nothing to merge with yet: the sorted candidates are the list
-              ld = cd; li = ci; lp = cp;
-              have_list = true;
-            }
-          }
-          else {
-            for (int src = 0; src < take; ++src) {
-              const float xd = __shfl_sync(full, cd, src);
-              const int xi = __shfl_sync(full, ci, src), xp = __shfl_sync(full, cp, src);
-              const int rank = __popc(__ballot_sync(full, lex_less(ld, li, xd, xi)));  // entries that stay in front
-              const float ud = __shfl_up_sync(full, ld, 1);
-              const int ui = __shfl_up_sync(full, li, 1), up = __shfl_up_sync(full, lp, 1);
-              if (lane > rank) {
-                ld = ud; li = ui; lp = up;
-              }
-              else if (lane == rank) {
-                ld = xd; li = xi; lp = xp;
-              }
-            }
-          }
-          __syncwarp();
-          // keep what is left of the buffer (at most 31 entries) at its front
-          const int rest = nbuf - take;
-          float md = 0.f;
-          int mi = 0, mp = 0;
-          if (lane < rest) {
-            md = s_cd[warp][take + lane];
-            mi = s_ci[warp][take + lane];
-            mp = s_cp[warp][take + lane];
-          }
-          __syncwarp();
-          if (lane < rest) {
-            s_cd[warp][lane] = md;
-            s_ci[warp][lane] = mi;
-            s_cp[warp][lane] = mp;
-          }
-          nbuf = rest;
-          {
-            const float nk = __shfl_sync(full, ld, k - 1);
-            const int ni = __shfl_sync(full, li, k - 1);
-            if (lex_less(nk, ni, Tk, Ti)) {  // never looser than the certification radius
-              Tk = nk;
-              Ti = ni;
-            }
-          }
-          __syncwarp();
-        };
-        const float gx2 = (E & 1u) ? cell_gap2(C, 0, qq.x, hx, ox, s) : 0.f;
-        const float gy2 = (E & 2u) ? cell_gap2(C, 1, qq.y, hy, oy, s) : 0.f;
-        const float gz2 = (E & 4u) ? cell_gap2(C, 2, qq.z, hz, oz, s) : 0.f;
-        for (int c = 0; c < 8; ++c) {
-          const int f = __shfl_sync(full, first, c), n = __shfl_sync(full, cnt, c);
-          if (n == 0)
-            continue;
-          // every point of cell c is at least this far (traverse.cuh: cell_gap2): a cell the k-th already beats is skipped
-          const float bound = __shfl_sync(full, shared ? 1 : 0, c)
-                                  ? 0.f
-                                  : __fadd_rd(__fadd_rd((c & 1) ? gx2 : 0.f, (c & 2) ? gy2 : 0.f), (c & 4) ? gz2 : 0.f);
-          if (!(bound <= Tk))
-            continue;
-          const int end = (f + n) * kLeafSize;
-          const float4 pad = make_float4(inf, inf, inf, __int_as_float(kSentinelIndex));
-          float4 pnext = f * kLeafSize + lane < end ? ldg4(T.pts + f * kLeafSize + lane) : pad;
-          for (int base = f * kLeafSize; base < end; base += 32) {
-            const int sidx = base + lane;
-            const float4 p = pnext;
-            if (base + 32 < end)  // the next round's line is in flight while this one is folded
-              pnext = sidx + 32 < end ? ldg4(T.pts + sidx + 32) : pad;
-            const float d = dist2_rn(qq.x, qq.y, qq.z, p.x, p.y, p.z);  // +inf for padding slots
-            const int oi = __float_as_int(p.w);
-            const bool pass = d < inf && lex_less(d, oi, Tk, Ti);
-            const unsigned pm = __ballot_sync(full, pass);
-            if (!pm)
-              continue;
-            if (pass) {
-              const int at = nbuf + __popc(pm & lt);
-              s_cd[warp][at] = d;
-              s_ci[warp][at] = oi;
-              s_cp[warp][at] = sidx;
-            }
-            nbuf += __popc(pm);
-            __syncwarp();
-            if (nbuf >= 32)
-              flush(32);
-          }
-        }
-        if (nbuf > 0)
-          flush(nbuf);
-        // exact iff the k-th neighbour lies strictly inside the gathered box (margin >> fp32 rounding of d2)
-        const float dk = __shfl_sync(full, ld, k - 1);
-        done = dk < R2cert;
-      }
-      if (!done) {
-        redo[qi] = 1;  // (all lanes store the same byte)
-        if (NORMALS && lane == t)
-          my_state = 3;
-        continue;
-      }
-      if (NORMALS) {
-        if (lane < k)
-          s_pos[warp][t][lane] = lp;
-        if (lane == t)
-          my_state = 1;
-      }
-      else if (lane < k) {
-        out_idx[slot * k + lane] = li;
-        out_d2[slot * k + lane] = ld;
-      }
-    }
-    if (NORMALS) {
-      // epilogue: lane t folds query t's neighbours sequentially, in list order — the arithmetic of k_normals
-      __syncwarp();
-      const size_t qi = batch * 32 + lane;
-      if (qi < nq && my_state != 0 && my_state != 3) {
-        const float4 qq = __ldg(q + qi);
-        const size_t slot = (size_t)(unsigned)__float_as_int(qq.w);
-        if (my_state == 2) {
-          out_n[slot] = make_float4(qnan, qnan, qnan, qnan);
-          *not_dense = 1;
-        }
-        else {
-          float accu[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-          float Kx = 0.f, Ky = 0.f, Kz = 0.f;
-          for (int j = 0; j < k; ++j) {
-            const float4 p = ldg4(T.pts + s_pos[warp][lane][j]);
-            if (j == 0) { Kx = p.x; Ky = p.y; Kz = p.z; }
-            moments_add(accu, Kx, Ky, Kz, p);
-          }
-          out_n[slot] = normal_from_moments(accu, k, qq, vpx, vpy, vpz, not_dense);
-        }
-      }
-      __syncwarp();
-    }
-  }
+#define PCLB_KNN_WARP_QUERY(qi)
+#define PCLB_KNN_WARP_LANE(qi)
+#include "knn_warp_body.inc"
+#undef PCLB_KNN_WARP_QUERY
+#undef PCLB_KNN_WARP_LANE
+}
+
+// ---- the k-NN normals of a batch of query sets, each against its own index (search.cu: launch_normals_batch) ----------
+// One entry per query set: what the single normals kernels take as parameters.
+struct NormalsCloud {
+  TreeView tree;
+  const int2* node_leaves;
+  const int32_t* pos_of_orig;  // the lists path (k > 32) only
+  int level;                   // start level of the warp kernel; 0 = every query goes to the per-thread kernel
+  float r_first;
+  float vp[3];
+  int* not_dense;              // this set's own flag
+};
+
+// k_knn_warp<true> over queries sorted by set (q[offsets[c] .. offsets[c+1]) belong to set c): each query is searched
+// in its own set's index (one lookup, the same for the whole warp), and each lane's epilogue reads its own set's points,
+// viewpoint and flag.  A set with level 0 hands every finite query to the per-thread kernel.
+__global__ void __launch_bounds__(256)
+k_knn_warp_batch(const NormalsCloud* __restrict__ clouds, const long long* __restrict__ offsets, int n_clouds,
+                 const float4* __restrict__ q, size_t nq, int k, float4* __restrict__ out_n,
+                 unsigned char* __restrict__ redo)
+{
+  constexpr bool NORMALS = true;
+  int32_t* const out_idx = nullptr;
+  float* const out_d2 = nullptr;
+#define PCLB_KNN_WARP_QUERY(qi)                                          \
+  const NormalsCloud& Q = clouds[problem_of(offsets, n_clouds, (long long)(qi))]; \
+  const TreeView T = Q.tree;                                             \
+  const int2* __restrict__ node_leaves = Q.node_leaves;                  \
+  const int b_start = Q.level;                                           \
+  const float r_first = Q.r_first;
+#define PCLB_KNN_WARP_LANE(qi)                                           \
+  const NormalsCloud& L = clouds[problem_of(offsets, n_clouds, (long long)(qi))]; \
+  const TreeView T = L.tree;                                             \
+  const float vpx = L.vp[0], vpy = L.vp[1], vpz = L.vp[2];               \
+  int* const not_dense = L.not_dense;
+#include "knn_warp_body.inc"
+#undef PCLB_KNN_WARP_QUERY
+#undef PCLB_KNN_WARP_LANE
 }
 
 }  // namespace pclb200

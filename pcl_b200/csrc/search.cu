@@ -499,4 +499,70 @@ void launch_normals(Ctx& c, Index& idx, const float4* d_q, size_t nq, int k, con
   PCLB_CUDA(cudaGetLastError());
 }
 
+// launch_normals of every set of a batch in one sequence: each set takes the path its single call would (the lists for
+// k > 32, else the warp kernel where launch_normals runs it, then the per-thread kernel over what is left), so every row
+// is the single call's.  The queries are already sorted by set, and each set's in the order of its own index's frame.
+void launch_normals_batch(Ctx& c, Index* const* idx, int B, const long long* d_offsets, const float4* d_q, size_t nq, int k,
+                          const float* vps, float4* d_out, int* d_flags)
+{
+  cudaStream_t s = c.stream;
+  const unsigned g = grid_for(nq, 128);
+  if (k > 32)
+    for (int b = 0; b < B; ++b)
+      ensure_pos_of_orig(c, *idx[b]);
+  std::vector<NormalsCloud> h(B);
+  bool any_warp = false;
+  for (int b = 0; b < B; ++b) {
+    const Index& I = *idx[b];
+    NormalsCloud& e = h[b];
+    e.tree = tree_view(I);
+    e.node_leaves = I.node_leaves.p;
+    e.pos_of_orig = k > 32 ? I.pos_of_orig.p : nullptr;
+    const WarpKnnStart w =
+        (k <= 32 && I.cell_slots.p && I.node_leaves.p && k >= 12) ? warp_knn_start(I, k) : WarpKnnStart{};
+    const bool warp = w.level >= 1 && (size_t)k <= I.n_valid;
+    e.level = warp ? w.level : 0;
+    e.r_first = warp ? w.r_first : 0.f;
+    for (int d = 0; d < 3; ++d)
+      e.vp[d] = vps[3 * b + d];
+    e.not_dense = d_flags + b;
+    any_warp = any_warp || warp;
+  }
+  DevBuf<NormalsCloud> table;
+  table.alloc(B, s);
+  PCLB_CUDA(cudaMemcpyAsync(table.p, h.data(), B * sizeof(NormalsCloud), cudaMemcpyHostToDevice, s));
+  if (k > 32) {
+    DevBuf<int32_t> li;
+    DevBuf<float> ld;
+    li.alloc(nq * (size_t)k, s);
+    ld.alloc(nq * (size_t)k, s);
+    k_knn_any_batch<<<g, 128, 0, s>>>(table.p, d_offsets, B, d_q, nq, k, __builtin_inff(), li.p, ld.p, c.d_error);
+    k_normals_from_lists_batch<<<g, 128, 0, s>>>(table.p, d_offsets, B, d_q, nq, k, li.p, d_out);
+    c.launches += 2;
+    PCLB_CUDA(cudaGetLastError());
+    return;
+  }
+  DevBuf<unsigned char> redo;
+  const unsigned char* only = nullptr;
+  if (any_warp) {
+    redo.alloc(nq, s);
+    PCLB_CUDA(cudaMemsetAsync(redo.p, 0, nq, s));
+    const unsigned wg = (unsigned)std::min<size_t>((nq + 255) / 256, (size_t)c.sm_count * 8);
+    k_knn_warp_batch<<<wg, 256, 0, s>>>(table.p, d_offsets, B, d_q, nq, k, d_out, redo.p);
+    ++c.launches;
+    only = redo.p;
+  }
+#define PCLB_NRM_CASE(KK) \
+  k_normals_batch<KK><<<g, 128, 0, s>>>(table.p, d_offsets, B, d_q, nq, k, d_out, c.d_error, only)
+  if (k <= 4) PCLB_NRM_CASE(4);
+  else if (k <= 8) PCLB_NRM_CASE(8);
+  else if (k <= 10) PCLB_NRM_CASE(10);
+  else if (k <= 16) PCLB_NRM_CASE(16);
+  else if (k <= 20) PCLB_NRM_CASE(20);
+  else PCLB_NRM_CASE(32);
+#undef PCLB_NRM_CASE
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+}
+
 }  // namespace pclb200

@@ -127,26 +127,7 @@ k_knn_any(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, int
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= nq)
     return;
-  const float4 qq = __ldg(q + i);
-  const size_t slot = (size_t)(unsigned)__float_as_int(qq.w);
-  NearestAny v;
-  v.qx = qq.x; v.qy = qq.y; v.qz = qq.z;
-  v.pts = pts;
-  v.k = k;
-  v.d = out_d2 + slot * k;
-  v.pos = out_idx + slot * k;
-  for (int j = 0; j < k; ++j) {
-    v.d[j] = init_bound;
-    v.pos[j] = -1;
-  }
-  if (isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z) && !traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, kErrStackOverflow);
-  for (int j = 0; j < k; ++j) {
-    int p = v.pos[j];
-    v.pos[j] = p >= 0 ? v.orig(p) : -1;
-    if (p < 0)
-      v.d[j] = __int_as_float(0x7f800000);
-  }
+#include "knn_any_body.inc"
 }
 
 // ---- per-query statistics of the k nearest neighbours (outlier filters) -------------------------------------------
@@ -302,40 +283,7 @@ k_normals(const BvhNode* __restrict__ nodes, const float4* __restrict__ pts, int
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= nq || (only && !only[i]))
     return;
-  const float4 qq = __ldg(q + i);
-  const size_t slot = (size_t)(unsigned)__float_as_int(qq.w);
-  const float qnan = __int_as_float(0x7fc00000);
-  if (!(isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z))) {
-    out[slot] = make_float4(qnan, qnan, qnan, qnan);
-    *not_dense = 1;
-    return;
-  }
-  NearestK<K> v;
-  v.qx = qq.x; v.qy = qq.y; v.qz = qq.z;
-  v.pts = pts;
-  v.init(__int_as_float(0x7f800000));
-  if (!traverse(nodes, pts, root, qq.x, qq.y, qq.z, v))
-    atomicExch(d_error, kErrStackOverflow);
-  int cnt = 0;
-#pragma unroll
-  for (int j = 0; j < K; ++j)
-    if (j < k_req && v.pos[j] >= 0)
-      ++cnt;
-  if (cnt < 3) {
-    out[slot] = make_float4(qnan, qnan, qnan, qnan);
-    *not_dense = 1;
-    return;
-  }
-  float accu[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  float Kx = 0.f, Ky = 0.f, Kz = 0.f;
-#pragma unroll
-  for (int j = 0; j < K; ++j)
-    if (j < cnt) {
-      const float4 p = ldg4(pts + v.pos[j]);
-      if (j == 0) { Kx = p.x; Ky = p.y; Kz = p.z; }
-      moments_add(accu, Kx, Ky, Kz, p);
-    }
-  out[slot] = normal_from_moments(accu, cnt, qq, vpx, vpy, vpz, not_dense);
+#include "normals_body.inc"
 }
 
 // normals from materialised neighbour lists (k > 32): same arithmetic as k_normals, neighbours fetched through
@@ -348,27 +296,7 @@ k_normals_from_lists(const float4* __restrict__ pts, const int32_t* __restrict__
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= nq)
     return;
-  const float4 qq = __ldg(q + i);
-  const size_t slot = (size_t)(unsigned)__float_as_int(qq.w);
-  const int32_t* nn = lists + (slot - slot0) * (size_t)k;
-  const float qnan = __int_as_float(0x7fc00000);
-  int cnt = 0;
-  for (int j = 0; j < k; ++j)
-    if (nn[j] >= 0)
-      ++cnt;
-  if (!(isfinite(qq.x) && isfinite(qq.y) && isfinite(qq.z)) || cnt < 3) {
-    out[slot] = make_float4(qnan, qnan, qnan, qnan);
-    *not_dense = 1;
-    return;
-  }
-  float accu[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  float Kx = 0.f, Ky = 0.f, Kz = 0.f;
-  for (int j = 0; j < cnt; ++j) {
-    const float4 p = ldg4(pts + pos_of_orig[nn[j]]);
-    if (j == 0) { Kx = p.x; Ky = p.y; Kz = p.z; }
-    moments_add(accu, Kx, Ky, Kz, p);
-  }
-  out[slot] = normal_from_moments(accu, cnt, qq, vpx, vpy, vpz, not_dense);
+#include "normals_from_lists_body.inc"
 }
 
 // normals from radius neighbourhoods (setRadiusSearch): rows of a CSR of packed keys (radius_csr), addressed by the
@@ -400,6 +328,60 @@ k_normals_from_csr(const float4* __restrict__ pts, const int32_t* __restrict__ p
     moments_add(accu, Kx, Ky, Kz, p);
   }
   out[slot] = normal_from_moments(accu, (int)(e - b), qq, vpx, vpy, vpz, not_dense);
+}
+
+// ---- batch forms of the k-NN normals kernels (search.cu: launch_normals_batch) -----------------------------------------
+// The queries of every set, sorted by set (q[offsets[c] .. offsets[c+1]) belong to set c, w = the record's row in the
+// whole batch); each thread runs the single kernel's body on its own set's entry of the table (knn_warp.cuh: NormalsCloud).
+template <int K>
+__global__ void __launch_bounds__(128)
+k_normals_batch(const NormalsCloud* __restrict__ clouds, const long long* __restrict__ offsets, int n_clouds,
+                const float4* __restrict__ q, size_t nq, int k_req, float4* __restrict__ out, int* __restrict__ d_error,
+                const unsigned char* __restrict__ only)
+{
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= nq || (only && !only[i]))
+    return;
+  const NormalsCloud& Q = clouds[problem_of(offsets, n_clouds, (long long)i)];
+  const BvhNode* __restrict__ nodes = Q.tree.nodes;
+  const float4* __restrict__ pts = Q.tree.pts;
+  const int root = Q.tree.root;
+  const float vpx = Q.vp[0], vpy = Q.vp[1], vpz = Q.vp[2];
+  int* const not_dense = Q.not_dense;
+#include "normals_body.inc"
+}
+
+// k_knn_any over every set's tree: rows of pitch k by the query's row in the batch
+__global__ void __launch_bounds__(128)
+k_knn_any_batch(const NormalsCloud* __restrict__ clouds, const long long* __restrict__ offsets, int n_clouds,
+                const float4* __restrict__ q, size_t nq, int k, float init_bound, int32_t* out_idx, float* out_d2,
+                int* __restrict__ d_error)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= nq)
+    return;
+  const NormalsCloud& Q = clouds[problem_of(offsets, n_clouds, (long long)i)];
+  const BvhNode* __restrict__ nodes = Q.tree.nodes;
+  const float4* __restrict__ pts = Q.tree.pts;
+  const int root = Q.tree.root;
+#include "knn_any_body.inc"
+}
+
+__global__ void __launch_bounds__(128)
+k_normals_from_lists_batch(const NormalsCloud* __restrict__ clouds, const long long* __restrict__ offsets, int n_clouds,
+                           const float4* __restrict__ q, size_t nq, int k, const int32_t* __restrict__ lists,
+                           float4* __restrict__ out)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= nq)
+    return;
+  const NormalsCloud& Q = clouds[problem_of(offsets, n_clouds, (long long)i)];
+  const float4* __restrict__ pts = Q.tree.pts;
+  const int32_t* __restrict__ pos_of_orig = Q.pos_of_orig;
+  const float vpx = Q.vp[0], vpy = Q.vp[1], vpz = Q.vp[2];
+  int* const not_dense = Q.not_dense;
+  const size_t slot0 = 0;
+#include "normals_from_lists_body.inc"
 }
 
 }  // namespace pclb200
