@@ -19,8 +19,9 @@
  * rejector chain, use_reciprocal, a correspondence_kind other than NEAREST, an active communicator or a sharded target,
  * and the symmetric objective without source normals.
  *
- * The targets of such a batch can themselves be built as one batch (pclb200_index_build_batch), and their normals for
- * point-to-plane or the symmetric objective estimated as one batch (pclb200_normals_knn_batch). */
+ * The clouds of such a batch can themselves be down-sampled as one batch (pclb200_voxelgrid_batch), the targets built as
+ * one batch (pclb200_index_build_batch), and their normals for point-to-plane or the symmetric objective estimated as one
+ * batch (pclb200_normals_knn_batch). */
 #ifndef PCLB200_BATCH_H_
 #define PCLB200_BATCH_H_
 
@@ -99,6 +100,32 @@ PCLB200_API int pclb200_normals_knn_batch(pclb200_ctx* ctx, const pclb200_index*
                                           const void* pts, size_t n, size_t stride, const int64_t* offsets, int k,
                                           const float* viewpoints /* nullable: n_clouds x 3 */, float* out,
                                           int32_t* is_dense_out /* nullable: n_clouds */);
+
+/* VoxelGrid of a batch of clouds in one call: cloud c = records [offsets[c], offsets[c+1]) of pts, down-sampled with one
+ * leaf and one minimum for every cloud.  Cloud c's rows are rows [out_offsets[c], out_offsets[c+1]) of out_xyz1, packed
+ * in cloud order; they and their count are bit for bit what pclb200_voxelgrid(ctx, its first record, its record count,
+ * stride, NULL, 0, 1, leaf, min_points_per_voxel, out, &m) gives, and with normals the same rows of out_normal_curv are
+ * what pclb200_voxelgrid_normals gives.  No row past out_offsets[n_clouds] is written, so out_xyz1 and out_offsets go
+ * straight to pclb200_index_build_batch and pclb200_icp_set_source_batch.  A cloud with no finite point, or whose voxels
+ * all hold fewer than min_points_per_voxel points, gets an empty range, as the single call returns 0 for it; the caller
+ * drops such a cloud before pclb200_index_build_batch, which refuses it.
+ *
+ * pts, normals, out_xyz1 and out_normal_curv: host or device, with the stride rules of pclb200_voxelgrid and
+ * pclb200_voxelgrid_normals; normals and out_normal_curv are both given or both NULL.  out_xyz1 (and out_normal_curv):
+ * capacity n rows.  offsets: host, n_clouds + 1 entries.  out_offsets: host, n_clouds + 1 entries.  Each stage is one
+ * launch (or one sort or select) for the whole batch, and the call synchronises the context's stream as often as one
+ * pclb200_voxelgrid does.  PCLB200_ERR_INVALID for n_clouds outside 1 to 65536, a NULL pts, offsets, leaf, out_xyz1 or
+ * out_offsets, offsets[0] != 0, a cloud with no records, offsets[n_clouds] != n, n >= 2^31 - 1, a bad stride, a normal
+ * stride below 20 or not a multiple of 4, a leaf that is not positive, and only one of normals and out_normal_curv;
+ * PCLB200_ERR_LEAF_TOO_SMALL when the grid of some cloud trips pclb200_voxelgrid's integer guard (pclb200_last_error
+ * names the first such cloud), with no result for any cloud.  Every refusal leaves the outputs and out_offsets
+ * untouched. */
+PCLB200_API int pclb200_voxelgrid_batch(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride,
+                                        const int64_t* offsets, int32_t n_clouds, const float leaf[3],
+                                        unsigned min_points_per_voxel,
+                                        const void* normals /* nullable */, size_t stride_n,
+                                        float* out_xyz1, float* out_normal_curv /* nullable */,
+                                        int64_t* out_offsets /* host, n_clouds + 1 */);
 
 #ifdef __cplusplus
 }

@@ -87,7 +87,7 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
 # every symbol include/pclb200_batch.h declares (a batch of ICP problems in one session; tests/test_icp_batch_symbols.py)
 BATCH_SYMBOLS = ["pclb200_icp_set_target_batch", "pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch",
-                 "pclb200_index_build_batch", "pclb200_normals_knn_batch"]
+                 "pclb200_index_build_batch", "pclb200_normals_knn_batch", "pclb200_voxelgrid_batch"]
 
 _lib = None
 
@@ -188,6 +188,7 @@ def lib():
     L.pclb200_icp_get_correspondences_batch.argtypes = [vp, vp, vp]
     L.pclb200_index_build_batch.argtypes = [vp, vp, sz, sz, vp, C.c_int32, vp]
     L.pclb200_normals_knn_batch.argtypes = [vp, vp, C.c_int32, vp, sz, sz, vp, C.c_int, fp, vp, vp]
+    L.pclb200_voxelgrid_batch.argtypes = [vp, vp, sz, sz, vp, C.c_int32, fp, C.c_uint, vp, sz, vp, vp, vp]
     for s in SYMBOLS + SHARDED_SYMBOLS + BATCH_SYMBOLS:
         getattr(L, s)  # AttributeError here == header and library disagree
     _lib = L
@@ -337,6 +338,35 @@ class Context:
                                                int(k), None if vp is None else vp.ctypes.data_as(C.POINTER(C.c_float)),
                                                ob.ptr, C.c_void_p(dense.ctypes.data)))
         return out, dense[:B].astype(bool)
+
+    def voxelgrid_batch(self, cloud, offsets, leaf, min_points_per_voxel=0, normal_offset=None, out=None, out_normals=None):
+        """VoxelGrid of B clouds in one call: cloud c = the records [offsets[c], offsets[c+1]) of `cloud` (numpy, or a torch
+        tensor on the host or the device).  Returns (rows, out_offsets), or (rows, normal_rows, out_offsets) when
+        normal_offset is given (pcl::PointNormal: 4): cloud c's rows are rows[out_offsets[c]:out_offsets[c+1]], bit for bit
+        voxelgrid (voxelgrid_normals) of that cloud alone; rows and out_offsets go straight to index_build_batch once the
+        empty ranges are dropped.  out / out_normals: caller buffers of (n, 4) / (n, 8) float32, returned as views; by
+        default the rows come back as trimmed host copies."""
+        b = _Buf(cloud)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        B = max(off.size - 1, 0)
+        leaf = (C.c_float * 3)(*[float(x) for x in np.broadcast_to(np.asarray(leaf, dtype=np.float32), (3,))])
+        with_normals = normal_offset is not None
+        nb = _Buf(Field(cloud, normal_offset) if with_normals else None)
+        host_out, host_nout = out is None, out_normals is None
+        if host_out:
+            out = np.empty((max(b.rows, 1), 4), dtype=np.float32)
+        if with_normals and host_nout:
+            out_normals = np.empty((max(b.rows, 1), 8), dtype=np.float32)
+        ob, onb = _Buf(out), _Buf(out_normals if with_normals else None)
+        out_off = np.zeros(B + 1, dtype=np.int64)
+        _check(lib().pclb200_voxelgrid_batch(self.h, b.ptr, b.rows, b.stride, C.c_void_p(off.ctypes.data), B, leaf,
+                                             int(min_points_per_voxel), nb.ptr, nb.stride, ob.ptr, onb.ptr,
+                                             C.c_void_p(out_off.ctypes.data)))
+        m = int(out_off[B])
+        rows = out[:m].copy() if host_out else out[:m]
+        if not with_normals:
+            return rows, out_off
+        return rows, (out_normals[:m].copy() if host_nout else out_normals[:m]), out_off
 
     def comm_init(self, rank, nranks, unique_id_bytes):
         buf = C.create_string_buffer(bytes(unique_id_bytes), 128)

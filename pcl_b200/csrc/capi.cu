@@ -73,6 +73,9 @@ unsigned long long ranks_min(Ctx& c, unsigned long long word);
 size_t voxelgrid(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* indices, size_t n_idx, int is_dense,
                  const float leaf[3], unsigned min_pts, float* out_xyz1, const void* normals, size_t stride_n,
                  float* out_normal_curv, const float* grid_bounds = nullptr);
+size_t voxelgrid_batch(Ctx& c, const void* pts, size_t n, size_t stride, const int64_t* offsets, int n_clouds,
+                       const float leaf[3], unsigned min_pts, const void* normals, size_t stride_n, float* out_xyz1,
+                       float* out_normal_curv, int64_t* out_offsets);
 // shard_voxel.cu
 size_t voxelgrid_sharded(Ctx& c, const void* pts, size_t n, size_t stride, const int32_t* ids, const void* normals,
                          size_t stride_n, const float leaf[3], unsigned min_pts, float* out_xyz1, float* out_normal_curv,
@@ -1314,6 +1317,17 @@ int pclb200_voxelgrid_normals(pclb200_ctx* ctx, const void* pts, size_t n, size_
     ProfScope ps(c, "voxelgrid");
     *n_out = voxelgrid(c, pts, n, stride, indices, n_idx, is_dense, leaf, min_points_per_voxel, out_xyz1, normals,
                        stride_n, out_normal_curv);
+  });
+}
+
+int pclb200_voxelgrid_batch(pclb200_ctx* ctx, const void* pts, size_t n, size_t stride, const int64_t* offsets,
+                            int32_t n_clouds, const float leaf[3], unsigned min_points_per_voxel, const void* normals,
+                            size_t stride_n, float* out_xyz1, float* out_normal_curv, int64_t* out_offsets)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    ProfScope ps(c, "voxelgrid_batch");
+    voxelgrid_batch(c, pts, n, stride, offsets, n_clouds, leaf, min_points_per_voxel, normals, stride_n, out_xyz1,
+                    out_normal_curv, out_offsets);
   });
 }
 

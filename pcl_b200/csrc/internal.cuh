@@ -394,6 +394,11 @@ void vg_load_normals(Ctx& c, const void* normals, size_t n, size_t stride_n, con
 void vg_runs(Ctx& c, const unsigned* starts, size_t n_runs, size_t n_valid, RunRef* runs);
 void vg_reduce(Ctx& c, const float4* pts, const float4* nc, const int32_t* vals, const RunRef* runs, size_t n_runs,
                float4* out, float4* out_nc);
+// The box and finite count of every cloud k = records [offsets[k], offsets[k + 1]) of the dense d_pts (offsets: host,
+// n_clouds + 1 entries) into out[k] (host), in one launch of the batch build's k_bbox_batch (lbvh.cu) over tiles that never
+// straddle a cloud; synchronised.  Its accumulator encodes the box as k_vg_minmax's does, so out[k] is what vg_minmax
+// gives of cloud k alone, up to the sign of a zero, which no voxel key depends on.
+void cloud_boxes(Ctx& c, const float4* d_pts, const int64_t* offsets, int n_clouds, MinMaxAcc* out);
 
 // connected components of the d2 < tolerance^2 graph over the indexed points (cluster.cu)
 void cluster_labels(Ctx& c, const Index& idx, double tolerance, int32_t* d_labels /* idx.n_cloud */);

@@ -24,6 +24,7 @@
 #include "internal.cuh"
 #include "traverse.cuh"
 #include "lbvh_kernels.cuh"
+#include "voxel_grid.cuh"
 
 namespace pclb200 {
 
@@ -505,6 +506,48 @@ std::vector<std::unique_ptr<Index>> build_index_batch(Ctx& c, const void* pts, s
   PCLB_CUDA(cudaGetLastError());
   PCLB_CUDA(cudaStreamSynchronize(s));  // temporaries are released stream-ordered; surface build errors here
   return out;
+}
+
+// the boxes of a batch of clouds (every cloud holds a record), as build_index_batch's step 1 reduces them
+// (voxel.cu: voxelgrid_batch)
+void cloud_boxes(Ctx& c, const float4* d_pts, const int64_t* offsets, int n_clouds, MinMaxAcc* out)
+{
+  cudaStream_t s = c.stream;
+  const int B = n_clouds;
+  std::vector<long long> tiles(B + 1, 0);
+  std::vector<BuildCloud> cl(B);
+  std::vector<BBoxAcc> acc(B);
+  for (int k = 0; k < B; ++k) {
+    cl[k].first = offsets[k];
+    cl[k].n = offsets[k + 1] - offsets[k];
+    tiles[k + 1] = tiles[k] + (cl[k].n + kBatchTile - 1) / kBatchTile;
+    for (int d = 0; d < 3; ++d) {
+      acc[k].lo[d] = 0x7fffffff;
+      acc[k].hi[d] = (int)0x80000000;
+    }
+    acc[k].count = 0;
+  }
+  DevBuf<long long> d_tiles;
+  DevBuf<BuildCloud> d_cl;
+  DevBuf<BBoxAcc> d_acc;
+  d_tiles.alloc(B + 1, s);
+  d_cl.alloc(B, s);
+  d_acc.alloc(B, s);
+  PCLB_CUDA(cudaMemcpyAsync(d_tiles.p, tiles.data(), (B + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+  PCLB_CUDA(cudaMemcpyAsync(d_cl.p, cl.data(), B * sizeof(BuildCloud), cudaMemcpyHostToDevice, s));
+  PCLB_CUDA(cudaMemcpyAsync(d_acc.p, acc.data(), B * sizeof(BBoxAcc), cudaMemcpyHostToDevice, s));
+  k_bbox_batch<<<(unsigned)tiles[B], 256, 0, s>>>(d_pts, d_cl.p, d_tiles.p, B, d_acc.p);
+  ++c.launches;
+  PCLB_CUDA(cudaGetLastError());
+  PCLB_CUDA(cudaMemcpyAsync(acc.data(), d_acc.p, B * sizeof(BBoxAcc), cudaMemcpyDeviceToHost, s));
+  PCLB_CUDA(cudaStreamSynchronize(s));
+  for (int k = 0; k < B; ++k) {
+    for (int d = 0; d < 3; ++d) {
+      out[k].lo[d] = acc[k].lo[d];
+      out[k].hi[d] = acc[k].hi[d];
+    }
+    out[k].count = acc[k].count;
+  }
 }
 
 // ---- labelled index: one tile of a map, its points carrying the caller's ids -------------------------------------

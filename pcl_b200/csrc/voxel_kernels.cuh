@@ -136,4 +136,55 @@ __global__ void k_vg_normals(const float4* __restrict__ nc, const int32_t* __res
   out[2 * m + 1] = make_float4(__fdiv_rn(cv, (float)(r.end - r.begin)), 0.f, 0.f, 0.f);
 }
 
+// ---- a batch of clouds in one call (voxelgrid_batch) ------------------------------------------------------------------
+// Cloud c is the records [offsets[c], offsets[c + 1]) of one dense array.  Record i's key is (c << 32) | its voxel's linear
+// index in cloud c's own grid, or B << 32 when it is not finite.  One stable sort by key then puts every cloud's voxels in
+// its single call's order, one cloud after another, with each voxel's records in ascending record order, and every
+// non-finite record at the tail; no run crosses a cloud.  The runs, the minimum-points filter and the reductions are the
+// single call's kernels over the whole batch.
+__global__ void k_vg_keys_batch(const float4* __restrict__ p, size_t n, const long long* __restrict__ offsets, int n_clouds,
+                                const VgParams* __restrict__ grids, unsigned long long* __restrict__ keys,
+                                int32_t* __restrict__ vals)
+{
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const float4 v = __ldg(p + i);
+  unsigned long long key = (unsigned long long)n_clouds << 32;
+  if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
+    const int c = problem_of(offsets, n_clouds, (long long)i);
+    const VgParams g = grids[c];
+    key = ((unsigned long long)c << 32) |
+          vg_linear(vg_ijk(v.x, g.inv[0], g.min_b[0]), vg_ijk(v.y, g.inv[1], g.min_b[1]), vg_ijk(v.z, g.inv[2], g.min_b[2]), g);
+  }
+  keys[i] = key;
+  vals[i] = (int32_t)i;
+}
+
+__global__ void k_vg_heads_batch(const unsigned long long* __restrict__ keys, size_t n, unsigned char* __restrict__ head)
+{
+  size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (j < n)
+    head[j] = (j == 0 || keys[j] != keys[j - 1]) ? 1 : 0;
+}
+
+// out[c], c = 0..B: the first of the *n_runs runs whose cloud is >= c, so that cloud c's rows are [out[c], out[c + 1]).
+// Run m starts at sorted position begins[m * step]: step 1 over the run heads, step 2 over RunRef {begin, end}.
+__global__ void k_vg_offsets_batch(const unsigned long long* __restrict__ keys, const unsigned* __restrict__ begins,
+                                   size_t step, const size_t* __restrict__ n_runs, int n_clouds, long long* __restrict__ out)
+{
+  const int c = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  if (c > n_clouds)
+    return;
+  size_t lo = 0, hi = *n_runs;
+  while (lo < hi) {
+    const size_t mid = (lo + hi) >> 1;
+    if ((keys[begins[mid * step]] >> 32) < (unsigned long long)c)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  out[c] = (long long)lo;
+}
+
 }  // namespace pclb200
