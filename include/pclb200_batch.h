@@ -20,8 +20,9 @@
  * and the symmetric objective without source normals.
  *
  * The clouds of such a batch can themselves be down-sampled as one batch (pclb200_voxelgrid_batch), the targets built as
- * one batch (pclb200_index_build_batch), and their normals for point-to-plane or the symmetric objective estimated as one
- * batch (pclb200_normals_knn_batch). */
+ * one batch (pclb200_index_build_batch), their normals for point-to-plane or the symmetric objective estimated as one
+ * batch (pclb200_normals_knn_batch), and the aligned pairs scored as one batch (pclb200_icp_fitness_score_batch,
+ * pclb200_fitness_score_batch, pclb200_validate_transformation_batch). */
 #ifndef PCLB200_BATCH_H_
 #define PCLB200_BATCH_H_
 
@@ -67,6 +68,41 @@ PCLB200_API int pclb200_icp_iterate_batch(pclb200_icp* icp, int max_steps, pclb2
  * is what its own session's pclb200_icp_get_correspondences returns: index_query relative to the problem's first
  * record).  out: host or device, capacity n (the batch's records); counts: host, B entries. */
 PCLB200_API int pclb200_icp_get_correspondences_batch(pclb200_icp* icp, pclb200_corr* out, int64_t* counts);
+
+/* getFitnessScore(max_range) of every problem of a batch session: problem p's own records under its current
+ * final_transformation, against its own target (or the session's one target).  scores (host, B entries): scores[p] is bit
+ * for bit pclb200_fitness_score_batch on the session's source, offsets, targets and stats[p].final_transformation with
+ * the session's scalar_is_double, in any state, before the first pclb200_icp_iterate_batch (the guess) included.  The
+ * call works on scratch of its own: the loop state, the correspondences and the moved source stay as they were, so the
+ * next pclb200_icp_iterate_batch continues as if it had not run.  PCLB200_ERR_INVALID, with scores untouched, for a NULL
+ * scores and a session without a batch source. */
+PCLB200_API int pclb200_icp_fitness_score_batch(pclb200_icp* icp, double max_range, double* scores);
+
+/* Registration::getFitnessScore of a batch of problems in one call: problem p = records [offsets[p], offsets[p+1]) of
+ * src, moved by transforms[16p..16p+16) (row-major) and scored against targets[p].  scores[p] is bit for bit what
+ * pclb200_fitness_score(ctx, targets[p], its first record, its record count, stride, NULL, 0, 1, T_p, scalar_is_double,
+ * max_range, &s) gives: the mean squared distance of the nearest-neighbour pairs with d2 <= max_range, or DBL_MAX for a
+ * problem with no finite point or no such pair.  A handle may repeat; every handle pclb200_fitness_score accepts is
+ * accepted, from single builds or from pclb200_index_build_batch.  There is no per-problem index subset, and max_range is
+ * one value for every problem.
+ *
+ * src: host or device, with the stride rules of pclb200_fitness_score.  targets, offsets (n_problems + 1 entries),
+ * transforms (16 n_problems) and scores (n_problems): host.  Each stage is one launch for the whole batch, whatever
+ * n_problems is, and the call reads the sums back and synchronises the context's stream once.  PCLB200_ERR_INVALID, with
+ * scores untouched, for n_problems outside 1 to 65536, a NULL array or NULL handle, offsets[0] != 0, a problem with no
+ * records, offsets[n_problems] != n, n >= 2^31 - 1, a bad stride and a handle on another device than the context. */
+PCLB200_API int pclb200_fitness_score_batch(pclb200_ctx* ctx, const pclb200_index* const* targets, int32_t n_problems,
+                                            const void* src, size_t n, size_t stride, const int64_t* offsets,
+                                            const double* transforms, int scalar_is_double, double max_range,
+                                            double* scores);
+
+/* The same for TransformationValidationEuclidean::validateTransformation: scores[p] is bit for bit
+ * pclb200_validate_transformation(ctx, targets[p], its first record, its record count, stride, T_p, scalar_is_double,
+ * max_range, &s).  Arguments and refusals as pclb200_fitness_score_batch. */
+PCLB200_API int pclb200_validate_transformation_batch(pclb200_ctx* ctx, const pclb200_index* const* targets,
+                                                      int32_t n_problems, const void* src, size_t n, size_t stride,
+                                                      const int64_t* offsets, const double* transforms,
+                                                      int scalar_is_double, double max_range, double* scores);
 
 /* A batch of independent indices in one build: cloud c = records [offsets[c], offsets[c+1]) of pts.  out[c] is bit for
  * bit the handle pclb200_index_build(ctx, its first record, its record count, stride, NULL, 0, &h) would give.  Its result

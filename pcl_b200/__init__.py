@@ -87,7 +87,8 @@ SHARDED_SYMBOLS = ["pclb200_index_build_ids", "pclb200_icp_set_target_sharded", 
                    "pclb200_radius_into_sharded", "pclb200_gicp_covariances_sharded"]
 # every symbol include/pclb200_batch.h declares (a batch of ICP problems in one session; tests/test_icp_batch_symbols.py)
 BATCH_SYMBOLS = ["pclb200_icp_set_target_batch", "pclb200_icp_set_source_batch", "pclb200_icp_iterate_batch", "pclb200_icp_get_correspondences_batch",
-                 "pclb200_index_build_batch", "pclb200_normals_knn_batch", "pclb200_voxelgrid_batch"]
+                 "pclb200_index_build_batch", "pclb200_normals_knn_batch", "pclb200_voxelgrid_batch",
+                 "pclb200_icp_fitness_score_batch", "pclb200_fitness_score_batch", "pclb200_validate_transformation_batch"]
 
 _lib = None
 
@@ -189,6 +190,9 @@ def lib():
     L.pclb200_index_build_batch.argtypes = [vp, vp, sz, sz, vp, C.c_int32, vp]
     L.pclb200_normals_knn_batch.argtypes = [vp, vp, C.c_int32, vp, sz, sz, vp, C.c_int, fp, vp, vp]
     L.pclb200_voxelgrid_batch.argtypes = [vp, vp, sz, sz, vp, C.c_int32, fp, C.c_uint, vp, sz, vp, vp, vp]
+    L.pclb200_icp_fitness_score_batch.argtypes = [vp, C.c_double, dp]
+    L.pclb200_fitness_score_batch.argtypes = [vp, vp, C.c_int32, vp, sz, sz, vp, dp, C.c_int, C.c_double, dp]
+    L.pclb200_validate_transformation_batch.argtypes = L.pclb200_fitness_score_batch.argtypes
     for s in SYMBOLS + SHARDED_SYMBOLS + BATCH_SYMBOLS:
         getattr(L, s)  # AttributeError here == header and library disagree
     _lib = L
@@ -367,6 +371,36 @@ class Context:
         if not with_normals:
             return rows, out_off
         return rows, (out_normals[:m].copy() if host_nout else out_normals[:m]), out_off
+
+    def fitness_score_batch(self, indices, cloud, offsets, transforms, max_range=np.finfo(np.float64).max,
+                            scalar_is_double=False):
+        """getFitnessScore of B problems in one call: problem p = the records [offsets[p], offsets[p+1]) of `cloud` (numpy,
+        or a torch tensor on the host or the device) moved by transforms[p] ((B, 4, 4) or (B, 16)) and scored against
+        indices[p].  Returns B float64 scores, each bit for bit indices[p].fitness_score(its records, transforms[p],
+        max_range, scalar_is_double)."""
+        return self._score_batch(lib().pclb200_fitness_score_batch, indices, cloud, offsets, transforms, max_range,
+                                 scalar_is_double)
+
+    def validate_transformation_batch(self, indices, cloud, offsets, transforms, max_range=np.finfo(np.float64).max,
+                                      scalar_is_double=False):
+        """TransformationValidationEuclidean of B problems in one call: as fitness_score_batch, each score bit for bit
+        indices[p].validate_transformation(its records, transforms[p], max_range, scalar_is_double)."""
+        return self._score_batch(lib().pclb200_validate_transformation_batch, indices, cloud, offsets, transforms,
+                                 max_range, scalar_is_double)
+
+    def _score_batch(self, fn, indices, cloud, offsets, transforms, max_range, scalar_is_double):
+        b = _Buf(cloud)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        B = max(off.size - 1, 0)
+        handles = (C.c_void_p * max(B, 1))(*[None if i is None else i.h for i in indices])
+        T = np.ascontiguousarray(transforms, dtype=np.float64).reshape(-1, 16)
+        if T.shape[0] != B:
+            raise ValueError("one 4x4 transform per problem")
+        scores = np.empty(max(B, 1), dtype=np.float64)
+        _check(fn(self.h, handles, B, b.ptr, b.rows, b.stride, C.c_void_p(off.ctypes.data),
+                  T.ctypes.data_as(C.POINTER(C.c_double)), int(scalar_is_double), float(max_range),
+                  scores.ctypes.data_as(C.POINTER(C.c_double))))
+        return scores[:B]
 
     def comm_init(self, rank, nranks, unique_id_bytes):
         buf = C.create_string_buffer(bytes(unique_id_bytes), 128)
@@ -1067,6 +1101,15 @@ class Icp:
                                                            C.c_void_p(counts.ctypes.data)))
         ends = np.cumsum(counts)
         return [out[e - c:e].copy() for c, e in zip(counts, ends)]
+
+    def fitness_score_batch(self, max_range=np.finfo(np.float64).max):
+        """getFitnessScore(max_range) of every problem under its current final transformation: B float64 scores, each bit
+        for bit Context.fitness_score_batch of the session's source, offsets, targets and final transformations.  The
+        session's loop state is left as it was."""
+        scores = np.empty(max(getattr(self, "n_problems", 0), 1), dtype=np.float64)
+        _check(lib().pclb200_icp_fitness_score_batch(self.h, float(max_range),
+                                                     scores.ctypes.data_as(C.POINTER(C.c_double))))
+        return scores[:getattr(self, "n_problems", 0)]
 
     def get_cloud(self, out=None, stride_floats=4, normals=None):
         if out is None:

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 SO = os.path.join(HERE, "libpclb200.so")
 SOURCES = ["alloc.cu", "lbvh.cu", "search.cu", "icp.cu", "voxel.cu", "reject.cu", "normals_corr.cu", "cluster.cu", "comm.cu", "shard_normals.cu", "shard_cluster.cu", "shard_filter.cu", "shard_voxel.cu", "capi.cu"]
-HEADERS = ["internal.cuh", "traverse.cuh", "knn_warp.cuh", "search_kernels.cuh", "lbvh_kernels.cuh", "voxel_grid.cuh", "voxel_kernels.cuh", "reject_kernels.cuh", "reject_sharded_kernels.cuh", "normals_corr_kernels.cuh", "cluster_kernels.cuh", "union_find.cuh", "icp_kernels.cuh", "grid_sum.cuh", "shard_target_kernels.cuh", "shard_normals_kernels.cuh", "shard_cluster_kernels.cuh", "shard_filter_kernels.cuh", "shard_voxel_kernels.cuh", "corr_select.cuh", "solve_body.inc", "assemble_body.inc", "karras_points_body.inc", "mark_cells_body.inc", "link_cells_body.inc", "knn_warp_body.inc", "normals_body.inc", "knn_any_body.inc", "normals_from_lists_body.inc", "peer_exchange.cuh", "peer_tables.cuh", os.path.join("..", "..", "include", "pclb200.h"), os.path.join("..", "..", "include", "pclb200_sharded.h"), os.path.join("..", "..", "include", "pclb200_batch.h")]
+HEADERS = ["internal.cuh", "traverse.cuh", "knn_warp.cuh", "search_kernels.cuh", "lbvh_kernels.cuh", "voxel_grid.cuh", "voxel_kernels.cuh", "reject_kernels.cuh", "reject_sharded_kernels.cuh", "normals_corr_kernels.cuh", "cluster_kernels.cuh", "union_find.cuh", "icp_kernels.cuh", "grid_sum.cuh", "shard_target_kernels.cuh", "shard_normals_kernels.cuh", "shard_cluster_kernels.cuh", "shard_filter_kernels.cuh", "shard_voxel_kernels.cuh", "corr_select.cuh", "solve_body.inc", "assemble_body.inc", "karras_points_body.inc", "mark_cells_body.inc", "link_cells_body.inc", "knn_warp_body.inc", "normals_body.inc", "knn_any_body.inc", "normals_from_lists_body.inc", "fitness_body.inc", "peer_exchange.cuh", "peer_tables.cuh", os.path.join("..", "..", "include", "pclb200.h"), os.path.join("..", "..", "include", "pclb200_sharded.h"), os.path.join("..", "..", "include", "pclb200_batch.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-fmad=false",

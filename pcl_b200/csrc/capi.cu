@@ -39,6 +39,9 @@ size_t correspondences(Ctx& c, const Index& tgt, const Index* src_index, const v
                        const double* pre_T = nullptr, int pre_mode = kApplyIcp, const float* gate_override = nullptr);
 double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t stride, const int32_t* indices,
                      size_t n_idx, const double* T, int scalar_is_double, double max_range, int mode_override = -1);
+void fitness_score_batch(Ctx& c, const Index* const* tgt, int B, const void* src, size_t n, size_t stride,
+                         const int64_t* offsets, const double* transforms, int mode, double max_range, double* scores);
+void icp_fitness_score_batch(Icp& s, double max_range, double* scores);
 double fitness_score_sharded(Ctx& c, const Index* tile, const void* src, size_t n, size_t stride, const int32_t* indices,
                              size_t n_idx, const double* T, int scalar_is_double, double max_range, int mode_override = -1,
                              const char* fault = nullptr);
@@ -777,6 +780,14 @@ int pclb200_icp_get_correspondences_batch(pclb200_icp* icp, pclb200_corr* out, i
   });
 }
 
+int pclb200_icp_fitness_score_batch(pclb200_icp* icp, double max_range, double* scores)
+{
+  return on_ctx(icp, [&](Icp& s) {
+    PCLB_REQUIRE(scores, PCLB200_ERR_INVALID, "NULL argument");
+    icp_fitness_score_batch(s, max_range, scores);
+  });
+}
+
 int pclb200_icp_get_cloud(pclb200_icp* icp, void* out_pts, size_t stride_out, void* out_normals, size_t stride_n)
 {
   return on_ctx(icp, [&](Icp& s) {
@@ -941,6 +952,54 @@ int pclb200_validate_transformation(pclb200_ctx* ctx, const pclb200_index* idx_t
     // transformation_validation_euclidean.hpp:62-75: T(0,0)*x + T(0,1)*y + T(0,2)*z + T(0,3) in Scalar, cast to float
     *score = fitness_score(c, *idx_tgt->idx, src, n, stride, nullptr, 0, T, scalar_is_double, max_range,
                            scalar_is_double ? kApplyValidationDouble : kApplyIcp);
+  });
+}
+
+// Shared body of pclb200_fitness_score_batch / pclb200_validate_transformation_batch: the refusals of
+// include/pclb200_batch.h, all checked before anything runs, then the batch in the single call's operation order `mode`
+static void fitness_batch_call(Ctx& c, const char* name, const pclb200_index* const* targets, int32_t n_problems,
+                               const void* src, size_t n, size_t stride, const int64_t* offsets, const double* transforms,
+                               int mode, double max_range, double* scores)
+{
+  const std::string who(name);
+  PCLB_REQUIRE(n_problems >= 1 && n_problems <= 65536, PCLB200_ERR_INVALID, who + ": a batch holds 1 to 65536 problems");
+  PCLB_REQUIRE(targets && src && offsets && transforms && scores, PCLB200_ERR_INVALID, "NULL argument");
+  const int B = n_problems;
+  std::vector<const Index*> idx(B);
+  for (int p = 0; p < B; ++p) {
+    PCLB_REQUIRE(targets[p] && targets[p]->idx, PCLB200_ERR_INVALID, who + ": a NULL handle");
+    PCLB_REQUIRE(targets[p]->idx->device == c.device, PCLB200_ERR_INVALID,
+                 who + ": an index lives on another device than the context");
+    idx[p] = targets[p]->idx;
+  }
+  PCLB_REQUIRE(offsets[0] == 0 && offsets[B] == (int64_t)n, PCLB200_ERR_INVALID, who + ": offsets must run from 0 to n");
+  for (int p = 0; p < B; ++p)
+    PCLB_REQUIRE(offsets[p + 1] > offsets[p], PCLB200_ERR_INVALID,
+                 who + ": offsets must increase strictly (every problem holds a record)");
+  PCLB_REQUIRE(n < (size_t)0x7fffffff, PCLB200_ERR_INVALID, who + ": a batch holds fewer than 2^31 - 1 records");
+  PCLB_REQUIRE(stride >= 12 && stride % 4 == 0, PCLB200_ERR_INVALID, "stride must be a multiple of 4 and >= 12");
+  ProfScope ps(c, "fitness_score_batch");
+  fitness_score_batch(c, idx.data(), B, src, n, stride, offsets, transforms, mode, max_range, scores);
+}
+
+int pclb200_fitness_score_batch(pclb200_ctx* ctx, const pclb200_index* const* targets, int32_t n_problems, const void* src,
+                                size_t n, size_t stride, const int64_t* offsets, const double* transforms,
+                                int scalar_is_double, double max_range, double* scores)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    fitness_batch_call(c, "fitness_score_batch", targets, n_problems, src, n, stride, offsets, transforms,
+                       scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat, max_range, scores);
+  });
+}
+
+int pclb200_validate_transformation_batch(pclb200_ctx* ctx, const pclb200_index* const* targets, int32_t n_problems,
+                                          const void* src, size_t n, size_t stride, const int64_t* offsets,
+                                          const double* transforms, int scalar_is_double, double max_range,
+                                          double* scores)
+{
+  return on_ctx(ctx, [&](Ctx& c) {
+    fitness_batch_call(c, "validate_transformation_batch", targets, n_problems, src, n, stride, offsets, transforms,
+                       scalar_is_double ? kApplyValidationDouble : kApplyIcp, max_range, scores);
   });
 }
 

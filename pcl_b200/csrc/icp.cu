@@ -37,24 +37,7 @@ bool comm_peer_view(Ctx& c, PeerView* view, unsigned long long* seq);
 bool comm_peer_fused(const Ctx& c);  // the per-iteration exchange happens inside the accumulate kernel
 int comm_nranks(const Ctx& c);
 
-// ---- misc streaming kernels ------------------------------------------------------------------------------
-__device__ __forceinline__ void transform_one(const Pending& P, float4* __restrict__ pts, size_t i,
-                                              float4* __restrict__ normals /* nullable */)
-{
-  float4 p = pts[i];
-  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z)))
-    return;
-  apply_pending(P, p.x, p.y, p.z);
-  pts[i] = p;
-  if (normals) {
-    float4 m = normals[i];
-    if (P.mode == kApplyIcp && !(isfinite(m.x) && isfinite(m.y) && isfinite(m.z)))
-      return;  // icp.hpp:97-98
-    apply_pending_normal(P, m.x, m.y, m.z);
-    normals[i] = m;
-  }
-}
-
+// ---- misc streaming kernels (transform_one and k_transform_batch: icp_kernels.cuh) ---------------------------------
 __device__ __forceinline__ void transform_range(const Pending& P, float4* __restrict__ pts, size_t n,
                                                 float4* __restrict__ normals /* nullable */)
 {
@@ -75,17 +58,6 @@ __global__ void k_apply_pending(float4* __restrict__ pts, size_t n, const Pendin
 __global__ void k_transform(float4* __restrict__ pts, size_t n, const Pending P, float4* __restrict__ normals)
 {
   transform_range(P, pts, n, normals);
-}
-
-// a batch (icp_kernels.cuh: BatchBlock): point i moved by the Pending of its problem, where that one applies
-__global__ void k_transform_batch(float4* __restrict__ pts, size_t n, const long long* __restrict__ offsets,
-                                  int n_problems, const Pending* __restrict__ P, float4* __restrict__ normals)
-{
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const Pending& Q = P[problem_of(offsets, n_problems, (long long)i)];
-    if (Q.apply)
-      transform_one(Q, pts, i, normals);
-  }
 }
 
 __global__ void k_set_pending(Pending* p, const Pending P) { *p = P; }
@@ -1908,6 +1880,104 @@ double fitness_score(Ctx& c, const Index& tgt, const void* src, size_t n, size_t
   PCLB_CUDA(cudaMemcpyAsync(acc, red.accum.p, sizeof(acc), cudaMemcpyDeviceToHost, st));
   check_device_error(c);
   return acc[0] > 0 ? acc[1] / acc[0] : std::numeric_limits<double>::max();
+}
+
+// fitness_score of B problems at once (DESIGN.md §3): problem p = the dense points pts[off[p], off[p+1]) (device; moved
+// in place) under transforms[16p..16p+16) in the operation order `mode`, scored against tgt[p].  gtab: batch_blocks's
+// table of the grid fitness_score launches for each problem alone, `slots` its blocks.  The queries of each problem reach
+// k_fitness_batch in make_query_batch's order for that problem alone and its sums run over its own grid, so scores[p] is
+// fitness_score's value bit for bit.  Every stage is one launch for the whole batch; the sums come back in one copy, and
+// the stream synchronises once.
+static void fitness_batch(Ctx& c, const Index* const* tgt, int B, float4* pts, size_t n, const long long* d_offsets,
+                          const DevBuf<BatchBlock>& gtab, unsigned slots, const double* transforms, int mode,
+                          double max_range, double* scores)
+{
+  cudaStream_t st = c.stream;
+  std::vector<Pending> h(B);
+  std::vector<float4> frames(B);
+  std::vector<TreeView> trees(B);
+  for (int p = 0; p < B; ++p) {
+    h[p] = make_pending(transforms + 16 * (size_t)p, mode, 1);
+    frames[p] = make_float4(tgt[p]->lo[0], tgt[p]->lo[1], tgt[p]->lo[2], tgt[p]->morton_scale);
+    trees[p] = tree_view(*tgt[p]);
+  }
+  DevBuf<Pending> pending;
+  DevBuf<float4> d_frames;
+  DevBuf<TreeView> d_trees;
+  pending.alloc(B, st);
+  d_frames.alloc(B, st);
+  d_trees.alloc(B, st);
+  PCLB_CUDA(cudaMemcpyAsync(pending.p, h.data(), B * sizeof(Pending), cudaMemcpyHostToDevice, st));
+  PCLB_CUDA(cudaMemcpyAsync(d_frames.p, frames.data(), B * sizeof(float4), cudaMemcpyHostToDevice, st));
+  PCLB_CUDA(cudaMemcpyAsync(d_trees.p, trees.data(), B * sizeof(TreeView), cudaMemcpyHostToDevice, st));
+  k_transform_batch<<<persistent_blocks(c, n), 256, 0, st>>>(pts, n, d_offsets, B, pending.p, nullptr);
+  ++c.launches;
+  QueryBatch qb;
+  {
+    ProfScope ps(c, "query_sort");
+    make_query_batch_framed(c, d_frames.p, d_offsets, B, pts, n, qb);
+    sort_by_problem(c, d_offsets, B, qb);
+  }
+  DevBuf<double> partials, accum;
+  DevBuf<unsigned> counter;
+  partials.alloc((size_t)slots * kAccum, st);
+  accum.alloc((size_t)B * kAccum, st);
+  counter.alloc(B, st);
+  PCLB_CUDA(cudaMemsetAsync(counter.p, 0, B * sizeof(unsigned), st));
+  {
+    ProfScope ps(c, "fitness_batch");
+    k_fitness_batch<<<(unsigned)gtab.n, 256, 0, st>>>(gtab.p, d_trees.p, qb.q.p, max_range,
+                                                      GridSum{partials.p, counter.p, accum.p}, c.d_error);
+    ++c.launches;
+  }
+  PCLB_CUDA(cudaGetLastError());
+  std::vector<double> acc(2 * (size_t)B);
+  PCLB_CUDA(cudaMemcpy2DAsync(acc.data(), 2 * sizeof(double), accum.p, kAccum * sizeof(double), 2 * sizeof(double), B,
+                              cudaMemcpyDeviceToHost, st));
+  check_device_error(c);
+  for (int p = 0; p < B; ++p)
+    scores[p] = acc[2 * p] > 0 ? acc[2 * p + 1] / acc[2 * p] : std::numeric_limits<double>::max();
+}
+
+// pclb200_fitness_score_batch / pclb200_validate_transformation_batch (mode: the single call's operation order), after the
+// C boundary has checked the arguments
+void fitness_score_batch(Ctx& c, const Index* const* tgt, int B, const void* src, size_t n, size_t stride,
+                         const int64_t* offsets, const double* transforms, int mode, double max_range, double* scores)
+{
+  cudaStream_t st = c.stream;
+  const std::vector<long long> off(offsets, offsets + B + 1);
+  DevBuf<long long> d_offsets;
+  d_offsets.alloc(B + 1, st);
+  PCLB_CUDA(cudaMemcpyAsync(d_offsets.p, off.data(), (B + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+  DevBuf<BatchBlock> gtab;
+  unsigned slots = 0;
+  batch_table(c, off, [&](size_t m) { return persistent_blocks(c, m); }, gtab, &slots);
+  DevBuf<float4> dense;
+  dense.alloc(n, st);
+  load_xyz_as_float4(c, src, n, stride, nullptr, 0, dense.p, st);
+  fitness_batch(c, tgt, B, dense.p, n, d_offsets.p, gtab, slots, transforms, mode, max_range, scores);
+}
+
+// getFitnessScore(max_range) of every problem of a batch session under its current final transform, on scratch of its
+// own: the loop state, the matches and `cur` stay as they were
+void icp_fitness_score_batch(Icp& s, double max_range, double* scores)
+{
+  Ctx& c = *s.ctx;
+  cudaStream_t st = c.stream;
+  const IcpBatch& b = s.batch;
+  const int B = b.B;
+  PCLB_REQUIRE(B > 0, PCLB200_ERR_INVALID, "icp: fitness_score_batch needs a batch source (set_source_batch)");
+  std::vector<const Index*> tgt(B, s.tgt);
+  if (s.targets.B)
+    tgt = s.targets.idx;
+  std::vector<double> T(16 * (size_t)B);
+  for (int p = 0; p < B; ++p)
+    std::copy(b.loop[p].final_T, b.loop[p].final_T + 16, T.begin() + 16 * (size_t)p);
+  DevBuf<float4> pts;
+  pts.alloc(s.n_all, st);
+  PCLB_CUDA(cudaMemcpyAsync(pts.p, s.src_all.p, s.n_all * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+  fitness_batch(c, tgt.data(), B, pts.p, s.n_all, b.d_offsets.p, b.gtab, b.g_blocks, T.data(),
+                s.P.scalar_is_double ? kApplyTransformsDouble : kApplyTransformsFloat, max_range, scores);
 }
 
 // Collective getFitnessScore over a map sharded across ranks (every rank passes its tile and the same source): the

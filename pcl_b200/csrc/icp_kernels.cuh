@@ -115,6 +115,34 @@ __device__ __forceinline__ void apply_pending_normal(const Pending& P, float& x,
   }
 }
 
+__device__ __forceinline__ void transform_one(const Pending& P, float4* __restrict__ pts, size_t i,
+                                              float4* __restrict__ normals /* nullable */)
+{
+  float4 p = pts[i];
+  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z)))
+    return;
+  apply_pending(P, p.x, p.y, p.z);
+  pts[i] = p;
+  if (normals) {
+    float4 m = normals[i];
+    if (P.mode == kApplyIcp && !(isfinite(m.x) && isfinite(m.y) && isfinite(m.z)))
+      return;  // icp.hpp:97-98
+    apply_pending_normal(P, m.x, m.y, m.z);
+    normals[i] = m;
+  }
+}
+
+// a batch (BatchBlock below): point i moved by the Pending of its problem, where that one applies
+__global__ void k_transform_batch(float4* __restrict__ pts, size_t n, const long long* __restrict__ offsets,
+                                  int n_problems, const Pending* __restrict__ P, float4* __restrict__ normals)
+{
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const Pending& Q = P[problem_of(offsets, n_problems, (long long)i)];
+    if (Q.apply)
+      transform_one(Q, pts, i, normals);
+  }
+}
+
 struct IterArgs {
   const BvhNode* nodes;
   const float4* pts;
@@ -1149,21 +1177,35 @@ k_fitness(const TreeView T, const float4* __restrict__ q, size_t nq, double max_
   double acc[2] = {0.0, 0.0};
   bool overflow = false;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nq; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 p = __ldg(q + i);
-    if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z)))
-      continue;
-    Nearest1 v{p.x, p.y, p.z, __int_as_float(0x7f800000), kSentinelIndex, -1};
-    WalkStats ws{};
-    if (!nearest1<false>(T, p.x, p.y, p.z, v, -1, 1.00001f, ws))
-      overflow = true;
-    if (v.best_pos >= 0 && (double)v.best <= max_range) {
-      acc[0] += 1.0;
-      acc[1] += (double)v.best;
-    }
+#include "fitness_body.inc"
   }
   if (overflow)
     atomicExch(d_error, kErrStackOverflow);
   block_reduce_and_publish<2>(acc, sum);
+}
+
+// k_fitness of a batch of problems in one launch (icp.cu: fitness_batch): block b of the table (batch_blocks) runs as block
+// b.vblock of the grid of b.vgrid blocks that k_fitness would be launched with over problem b.problem's queries
+// q[b.begin, b.begin + b.n) alone, searching that problem's tree trees[b.problem].  Its sums go through the problem's own
+// partials (from slot b.part), counter and accumulator (kAccum doubles per problem) in the problem's own block order: the
+// single call's sums, bit for bit.
+__global__ void __launch_bounds__(256)
+k_fitness_batch(const BatchBlock* __restrict__ blocks, const TreeView* __restrict__ trees, const float4* __restrict__ q_all,
+                double max_range, GridSum sum, int* d_error)
+{
+  const BatchBlock b = blocks[blockIdx.x];
+  const TreeView T = trees[b.problem];
+  const float4* __restrict__ q = q_all + b.begin;
+  const size_t nq = b.n;
+  double acc[2] = {0.0, 0.0};
+  bool overflow = false;
+  for (size_t i = b.vblock * (size_t)blockDim.x + threadIdx.x; i < nq; i += (size_t)b.vgrid * blockDim.x) {
+#include "fitness_body.inc"
+  }
+  if (overflow)
+    atomicExch(d_error, kErrStackOverflow);
+  const GridSum mine{sum.partials + (size_t)b.part * kAccum, sum.counter + b.problem, sum.accum + (size_t)b.problem * kAccum};
+  block_reduce_and_publish<2>(acc, mine, VirtualGrid{b.vblock, b.vgrid});
 }
 
 // GeneralizedIterativeClosestPoint::computeCovariances, one thread per point over exact k-NN rows (driver: gicp_covariances)
