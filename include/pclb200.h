@@ -302,7 +302,13 @@ PCLB200_API void pclb200_icp_default_params(pclb200_icp_params* p);
  *               tgt_normals (nullable) = first nx of the target normals, device copy kept for LLS.
  * set_source  : Registration::setInputSource + align()'s prologue (registration.hpp:172-216,
  *               icp.hpp:120-161): uploads the (indexed) source, applies `guess` (NULL = identity),
- *               resets the iteration state.
+ *               resets the iteration state.  The convergence criteria's previous MSE is the one thing it
+ *               keeps: as in the reference, whose DefaultConvergenceCriteria lives as long as the
+ *               IterativeClosestPoint object (icp.h:155), the first iteration after set_source is compared
+ *               with the last MSE the criteria recorded in this session (DBL_MAX in a new session).  So a
+ *               tracking loop that aligns again from its last result can stop at iteration 1 on the MSE
+ *               tests.  pclb200_icp_align and every problem of pclb200_icp_set_source_batch start from a
+ *               new criteria object (DBL_MAX).
  * iterate     : runs up to max_steps iterations of the do-while at icp.hpp:164-241, stopping early
  *               when the convergence criteria fire; *stats is refreshed after every call.
  * get_cloud   : output = *input_ transformed by final_transformation_ (icp.hpp:265-267), written
@@ -332,7 +338,8 @@ PCLB200_API int pclb200_icp_get_cloud(pclb200_icp* icp, void* out_pts, size_t st
  * loop that stopped with NO_CORRESPONDENCES returns the list (fewer than 3 pairs) that stopped it. */
 PCLB200_API int pclb200_icp_get_correspondences(pclb200_icp* icp, pclb200_corr* out, size_t* n_out);
 
-/* one-call form: Registration::align(output, guess) (registration.hpp:172-221) */
+/* one-call form: Registration::align(output, guess) (registration.hpp:172-221) of a new IterativeClosestPoint object,
+ * so its criteria start with a previous MSE of DBL_MAX */
 PCLB200_API int pclb200_icp_align(pclb200_ctx* ctx, const pclb200_icp_params* params,
                                   const void* src, size_t n, size_t stride, const void* src_normals,
                                   size_t stride_sn, const int32_t* src_indices, size_t n_idx,

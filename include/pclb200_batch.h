@@ -11,7 +11,9 @@
  *
  * Problem p is bit for bit what a fresh session with the same parameters, target and target normals would do after
  * pclb200_icp_set_source(its records, its guess) and the same sequence of max_steps: every pclb200_icp_stats field
- * (total_skipped_walks included), every iteration's correspondences and the aligned records.
+ * (total_skipped_walks included), every iteration's correspondences and the aligned records.  Every problem starts
+ * with a new criteria state, previous MSE DBL_MAX: unlike pclb200_icp_set_source, set_source_batch carries nothing
+ * over from the session's earlier aligns.
  *
  * A batch takes nearest-neighbour correspondences; SVD (Umeyama or not), point-to-plane LLS or the symmetric objective;
  * float or double Scalar; with_normals_transform; is_dense = 0; every convergence criterion; tracking OFF / ON / AUTO

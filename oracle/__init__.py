@@ -87,6 +87,7 @@ def lib():
         L.orc_reject_chain.argtypes = [C.POINTER(Rejector), C.c_int, C.POINTER(Corr), sz, C.POINTER(Corr), dp]
         L.orc_icp_align_full.argtypes = [C.POINTER(IcpParams), vp, C.POINTER(Rejector), C.c_int, vp, fp, sz, sz, i32p, sz,
                                          fp, sz, sz, dp, C.POINTER(IcpResult), fp, C.POINTER(Corr), C.POINTER(sz)]
+        L.orc_icp_align_carry.argtypes = L.orc_icp_align_full.argtypes + [dp]
         L.orc_fitness_score.restype = C.c_double
         L.orc_fitness_score.argtypes = [vp, fp, sz, sz, i32p, sz, C.c_int, dp, C.c_int, C.c_double, C.c_int]
         L.orc_voxelgrid.restype = C.c_longlong
@@ -440,6 +441,40 @@ def icp_align_rejectors(src, tgt, rejectors, **kw):
                              C.byref(R), None, corr.ctypes.data_as(C.POINTER(Corr)), C.byref(nc))
     return dict(final=np.array(R.final_transformation).reshape(4, 4), converged=bool(R.converged), state=int(R.state),
                 iterations=int(R.iterations), n_correspondences=int(R.n_correspondences), mse=float(R.mse),
+                correspondences=corr[:nc.value].copy())
+
+
+class IcpExt(C.Structure):
+    _fields_ = [("failure_after_max_iter", C.c_int32), ("max_iterations_similar_transforms", C.c_int32),
+                ("svd_no_umeyama", C.c_int32), ("enforce_same_direction_normals", C.c_int32),
+                ("mse_threshold_absolute", C.c_double)]
+
+
+def icp_align_criteria(src, tgt, max_iterations=10, max_correspondence_distance=np.sqrt(np.finfo(np.float64).max),
+                       transformation_epsilon=0.0, transformation_rotation_epsilon=0.0,
+                       euclidean_fitness_epsilon=-np.finfo(np.float64).max, mse_threshold_absolute=1e-12,
+                       failure_after_max_iter=False, max_iterations_similar_transforms=0, estimator=0,
+                       svd_no_umeyama=False, scalar_is_double=False, guess=None, prev_mse=None, nthreads=1):
+    """One align with every DefaultConvergenceCriteria knob.  src / tgt: (n, 8) records, xyz 1 | normal 0 (the normals
+    feed point-to-plane and the symmetric objective).  prev_mse: the criteria's previous MSE when the align starts (None
+    = a new criteria object, DBL_MAX); the result's "prev_mse" is where the align leaves it."""
+    src, tgt = as_cloud(src), as_cloud(tgt)
+    P = IcpParams(max_iterations, 0, estimator, int(scalar_is_double), int(estimator != 0), int(estimator != 0), 1,
+                  nthreads, float(max_correspondence_distance), float(transformation_epsilon),
+                  float(transformation_rotation_epsilon), float(euclidean_fitness_epsilon), 0, 10)
+    pm = C.c_double(np.finfo(np.float64).max if prev_mse is None else float(prev_mse))
+    X = IcpExt(int(failure_after_max_iter), int(max_iterations_similar_transforms), int(svd_no_umeyama), 1,
+               float(mse_threshold_absolute))
+    R = IcpResult()
+    g = None if guess is None else np.ascontiguousarray(guess, dtype=np.float64)
+    corr = np.empty(max(src.shape[0], 1), dtype=CORR_DTYPE)
+    nc = C.c_size_t(0)
+    lib().orc_icp_align_carry(C.byref(P), C.byref(X), None, 0, None, _f(src), src.shape[0], src.shape[1], None, 0,
+                              _f(tgt), tgt.shape[0], tgt.shape[1], _d(g), C.byref(R), None,
+                              corr.ctypes.data_as(C.POINTER(Corr)), C.byref(nc), C.byref(pm))
+    return dict(final=np.array(R.final_transformation).reshape(4, 4), last=np.array(R.last_transformation).reshape(4, 4),
+                converged=bool(R.converged), state=int(R.state), iterations=int(R.iterations),
+                n_correspondences=int(R.n_correspondences), mse=float(R.mse), prev_mse=float(pm.value),
                 correspondences=corr[:nc.value].copy())
 
 

@@ -1663,7 +1663,7 @@ static void icp_run(const orc_icp_params& P, const float* src, size_t n_s, size_
                     const int32_t* indices, size_t n_idx, const float* tgt, size_t n_t, size_t ts,
                     const double* guess, orc_icp_result& R, float* out_cloud, void* prebuilt_tree = nullptr,
                     const orc_rejector* rejectors = nullptr, int n_rejectors = 0, const orc_icp_ext* X = nullptr,
-                    orc_corr* last_corr = nullptr, size_t* n_last_corr = nullptr)
+                    orc_corr* last_corr = nullptr, size_t* n_last_corr = nullptr, double* prev_mse = nullptr)
 {
   // Registration::align (registration/.../impl/registration.hpp:172-221) +
   // IterativeClosestPoint::computeTransformation (impl/icp.hpp:113-268)
@@ -1696,6 +1696,8 @@ static void icp_run(const orc_icp_params& P, const float* src, size_t n_s, size_
     conv.max_iterations_similar_transforms = X->max_iterations_similar_transforms;
     conv.mse_threshold_absolute = X->mse_threshold_absolute;
   }
+  if (prev_mse)
+    conv.prev_mse = *prev_mse;
   std::vector<orc_corr> corr(indices ? n_idx : n_s);
   int iterations = 0;
   bool converged = false;
@@ -1756,6 +1758,8 @@ static void icp_run(const orc_icp_params& P, const float* src, size_t n_s, size_
     R.final_transformation[i] = final_T[i];
     R.last_transformation[i] = T[i];
   }
+  if (prev_mse)
+    *prev_mse = conv.prev_mse;
   R.converged = converged ? 1 : 0;
   R.state = conv.state;
   R.iterations = iterations;
@@ -1808,6 +1812,22 @@ ORC_API void orc_icp_align_full(const orc_icp_params* P, const orc_icp_ext* X, c
   else
     icp_run<float>(*P, src, n_s, sstride, indices, n_idx, tgt, n_t, tstride, guess, *R, out_cloud, h_tgt, rej, n_rej, X,
                    last_corr, n_last_corr);
+}
+
+// orc_icp_align_full on a criteria object that outlives one align (icp.h:155): *prev_mse is its
+// correspondences_prev_mse_ (default_convergence_criteria.h:283) when the align starts, and is where the align leaves it.
+ORC_API void orc_icp_align_carry(const orc_icp_params* P, const orc_icp_ext* X, const orc_rejector* rej, int n_rej,
+                                 void* h_tgt, const float* src, size_t n_s, size_t sstride, const int32_t* indices,
+                                 size_t n_idx, const float* tgt, size_t n_t, size_t tstride, const double* guess,
+                                 orc_icp_result* R, float* out_cloud, orc_corr* last_corr, size_t* n_last_corr,
+                                 double* prev_mse)
+{
+  if (P->scalar_is_double)
+    icp_run<double>(*P, src, n_s, sstride, indices, n_idx, tgt, n_t, tstride, guess, *R, out_cloud, h_tgt, rej, n_rej, X,
+                    last_corr, n_last_corr, prev_mse);
+  else
+    icp_run<float>(*P, src, n_s, sstride, indices, n_idx, tgt, n_t, tstride, guess, *R, out_cloud, h_tgt, rej, n_rej, X,
+                   last_corr, n_last_corr, prev_mse);
 }
 
 // Registration::getFitnessScore — registration/.../impl/registration.hpp:134-168

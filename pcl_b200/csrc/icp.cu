@@ -346,12 +346,17 @@ static void transform_on_device(Ctx& c, const double* T, int mode, float4* pts, 
   ++c.launches;
 }
 
+// Everything an align() starts afresh (icp.hpp:120-136).  The previous MSE is DefaultConvergenceCriteria's member, and
+// that object lives as long as the IterativeClosestPoint (icp.h:155): it starts at DBL_MAX when the session is created
+// (default_convergence_criteria.h:283) and is written only by the criteria (…criteria.hpp:137), so the first iteration
+// of the next align is compared with the last MSE the previous one recorded.
 void icp_reset_state(Icp& s, const double* guess)
 {
   LoopCtrl& L = s.loop;
+  const double prev_mse = L.prev_mse;
   memset(&L, 0, sizeof(L));
   L.state = PCLB200_CONV_NOT_CONVERGED;
-  L.prev_mse = std::numeric_limits<double>::max();
+  L.prev_mse = prev_mse;
   set_identity(L.last_T);
   if (guess) {
     for (int i = 0; i < 16; ++i)
@@ -373,6 +378,7 @@ Icp* icp_create(Ctx& c, const pclb200_icp_params& P)
   s->ctrl.alloc(1, c.stream);
   s->skip_count.alloc(1, c.stream);
   s->red.init(c, (unsigned)c.sm_count * 16);
+  s->loop.prev_mse = std::numeric_limits<double>::max();
   icp_reset_state(*s, nullptr);
   set_pending(c, s->pending.p, make_pending(s->loop.final_T, transform_mode(P), 0));
   return s.release();
@@ -1443,9 +1449,12 @@ void icp_set_source_batch(Icp& s, const void* src, size_t n, size_t stride, cons
   PCLB_CUDA(cudaMemsetAsync(b.counter.p, 0, B * sizeof(unsigned), st));
   PCLB_CUDA(cudaMemsetAsync(b.accum.p, 0, (size_t)B * kAccum * sizeof(double), st));
   b.host.reserve(B * (sizeof(LoopCtrl) + sizeof(unsigned long long)) + sizeof(int));
-  // every problem's loop state as icp_set_source leaves it; a guess that is not the identity moves its queries once
+  // every problem's loop state as icp_set_source of a new session leaves it (its own criteria, previous MSE DBL_MAX);
+  // a guess that is not the identity moves its queries once
   icp_reset_state(s, nullptr);
   b.loop.assign(B, s.loop);
+  for (LoopCtrl& L : b.loop)
+    L.prev_mse = std::numeric_limits<double>::max();
   b.total_skipped.assign(B, 0);
   const int mode = transform_mode(s.P);
   std::vector<Pending> h(B);

@@ -65,6 +65,10 @@ public:
   double rotation_threshold_ = 0.99999;
   double translation_threshold_ = 3e-4 * 3e-4;
   double mse_threshold_relative_ = 0.00001;
+  // correspondences_prev_mse_ (default_convergence_criteria.h:283): written only when no criterion fired, never reset,
+  // so it carries from one align() of the owning object to the next.  The staged loop keeps it here; the device loop
+  // keeps its own in the pclb200_icp session, which carries it the same way.
+  double prev_mse_ = std::numeric_limits<double>::max();
 };
 }  // namespace registration
 
@@ -352,7 +356,7 @@ protected:
     if (!(guess == Matrix4::Identity())) transformCloudHost(*this->input_, moved, guess);  // impl/icp.hpp:125-134
     this->transformation_ = Matrix4::Identity();
     State state = ConvergenceCriteria::CONVERGENCE_CRITERIA_NOT_CONVERGED;
-    double prev_mse = std::numeric_limits<double>::max();
+    double& prev_mse = convergence_criteria_->prev_mse_;
     int iterations_similar = 0;
     const double max_d2 = this->corr_dist_threshold_ * this->corr_dist_threshold_;
     pcl::Correspondences corr, tmp;

@@ -69,6 +69,10 @@ size_t orc_reject_surface_normal(const orc_corr* in, size_t n, const float* sn, 
 void orc_icp_align_full(const orc_icp_params* P, const orc_icp_ext* X, const orc_rejector* rej, int n_rej, void* h_tgt, const float* src,
                         size_t n_s, size_t sstride, const int32_t* indices, size_t n_idx, const float* tgt, size_t n_t, size_t tstride,
                         const double* guess, orc_icp_result* R, float* out_cloud, orc_corr* last_corr, size_t* n_last_corr);
+void orc_icp_align_carry(const orc_icp_params* P, const orc_icp_ext* X, const orc_rejector* rej, int n_rej, void* h_tgt, const float* src,
+                         size_t n_s, size_t sstride, const int32_t* indices, size_t n_idx, const float* tgt, size_t n_t, size_t tstride,
+                         const double* guess, orc_icp_result* R, float* out_cloud, orc_corr* last_corr, size_t* n_last_corr,
+                         double* prev_mse);
 double orc_fitness_score(void* h_tgt, const float* src, size_t n_s, size_t sstride, const int32_t* indices, size_t n_idx, int is_dense,
                          const double* final_T, int scalar_is_double, double max_range, int nthreads);
 long long orc_voxelgrid(const float* pts, size_t n, size_t stride, const int32_t* indices, size_t n_idx, int is_dense, const float leaf[3],
@@ -158,6 +162,10 @@ struct pclb200_icp {
   std::vector<orc_corr> full_corr, cur_corr;
   int done = 0;
   bool finished = false;
+  // the criteria's previous MSE, which outlives an align (icp.h:155): where the last iterate left it, and its value
+  // when set_source started the current align (every replay of that align starts from it)
+  double prev_mse = std::numeric_limits<double>::max(), prev_mse_at_source = std::numeric_limits<double>::max();
+  double full_prev_mse = 0;
 };
 
 extern "C" {
@@ -422,13 +430,15 @@ int pclb200_icp_set_source(pclb200_icp* s, const void* src, size_t n, size_t str
   s->indices.assign(indices, indices + (indices ? n_idx : 0));
   s->has_guess = guess != nullptr;
   if (guess) std::memcpy(s->guess, guess, sizeof(s->guess));
+  s->prev_mse_at_source = s->prev_mse;
   s->have_full = false;
   s->done = 0;
   s->finished = false;
   return PCLB200_OK;
 }
 
-static int icp_run(pclb200_icp* s, int max_iterations, orc_icp_result& R, std::vector<float>& cloud, std::vector<orc_corr>& corr)
+static int icp_run(pclb200_icp* s, int max_iterations, orc_icp_result& R, std::vector<float>& cloud, std::vector<orc_corr>& corr,
+                   double* prev_mse)
 {
   const pclb200_icp_params& P = s->P;
   const bool need_tn = P.estimator != PCLB200_EST_SVD || P.correspondence_kind == PCLB200_CORR_BACK_PROJECTION;
@@ -451,12 +461,13 @@ static int icp_run(pclb200_icp* s, int max_iterations, orc_icp_result& R, std::v
   O.correspondence_kind = P.correspondence_kind;
   O.correspondence_k = P.correspondence_k;
   orc_icp_ext X{P.failure_after_max_iter, P.max_iterations_similar_transforms, P.svd_no_umeyama, P.enforce_same_direction_normals, P.mse_threshold_absolute};
+  *prev_mse = s->prev_mse_at_source;
   cloud.assign(s->src_rec.size(), 0.f);
   corr.assign(std::max<size_t>(s->has_indices ? s->indices.size() : s->n_src, 1), orc_corr{});
   size_t nc = 0;
-  orc_icp_align_full(&O, &X, s->chain.empty() ? nullptr : s->chain.data(), (int)s->chain.size(), s->tgt->tree, s->src_rec.data(), s->n_src, 8,
-                     s->has_indices ? s->indices.data() : nullptr, s->has_indices ? s->indices.size() : 0, s->tgt_rec.data(), s->tgt->n, 8,
-                     s->has_guess ? s->guess : nullptr, &R, cloud.data(), corr.data(), &nc);
+  orc_icp_align_carry(&O, &X, s->chain.empty() ? nullptr : s->chain.data(), (int)s->chain.size(), s->tgt->tree, s->src_rec.data(), s->n_src, 8,
+                      s->has_indices ? s->indices.data() : nullptr, s->has_indices ? s->indices.size() : 0, s->tgt_rec.data(), s->tgt->n, 8,
+                      s->has_guess ? s->guess : nullptr, &R, cloud.data(), corr.data(), &nc, prev_mse);
   corr.resize(nc);
   return PCLB200_OK;
 }
@@ -467,7 +478,7 @@ int pclb200_icp_iterate(pclb200_icp* s, int max_steps, pclb200_icp_stats* st)
   if (!s->tgt || s->src_rec.empty()) return fail(PCLB200_ERR_INVALID, "icp: target and source must be set");
   if (max_steps < 0) return fail(PCLB200_ERR_INVALID, "max_steps < 0");
   if (!s->have_full) {
-    int rc = icp_run(s, s->P.max_iterations, s->full, s->full_cloud, s->full_corr);
+    int rc = icp_run(s, s->P.max_iterations, s->full, s->full_cloud, s->full_corr, &s->full_prev_mse);
     if (rc != PCLB200_OK) return rc;
     s->have_full = true;
   }
@@ -479,13 +490,17 @@ int pclb200_icp_iterate(pclb200_icp* s, int max_steps, pclb200_icp_stats* st)
       s->cur = s->full; s->cur_cloud = s->full_cloud; s->cur_corr = s->full_corr;
       s->done = s->full.iterations;
       s->finished = true;
+      s->prev_mse = s->full_prev_mse;
     }
     else {
-      int rc = icp_run(s, (int)want, s->cur, s->cur_cloud, s->cur_corr);
+      double replay_prev_mse;
+      int rc = icp_run(s, (int)want, s->cur, s->cur_cloud, s->cur_corr, &replay_prev_mse);
       if (rc != PCLB200_OK) return rc;
       s->cur.state = PCLB200_CONV_NOT_CONVERGED;
       s->cur.converged = 0;
       s->done = (int)want;
+      // the replay stopped on its iteration cap before its criteria recorded iteration `want`; the session's did
+      s->prev_mse = s->cur.mse;
     }
   }
   std::memset(st, 0, sizeof(*st));

@@ -82,6 +82,16 @@ def test_extra_facade_program(double, golden, tmp_path):
     assert int(r.stdout.split(" checks")[0].split()[-1]) > 400   # the golden block ran
 
 
+def test_criteria_carry_over_program(double, golden, tmp_path):
+    """pcl_compat/tests/test_facade_loop.cpp: one IterativeClosestPoint aligned twice keeps its criteria's previous MSE,
+    so the second align stops at iteration 1 where a new object stops at 2, on the fused loop (here the double's
+    session) and on the staged loop."""
+    _, _, program = double
+    b0, b4 = _clouds(golden, tmp_path)
+    r = subprocess.run([program("tests/test_facade_loop.cpp"), b0, b4], capture_output=True, text=True)
+    assert r.returncode == 0 and "PASSED" in r.stdout, r.stdout[-3000:] + r.stderr[-1500:]
+
+
 def test_icp_command_line_program(double, golden, tmp_path):
     """pcl_compat/examples/iterative_closest_point.cpp (the flow of the reference's tools/iterative_closest_point.cpp):
     blob PCD in, ICP<PointNormal, double> with injected estimators and a one-to-one rejector, concatenateFields, PCD out."""

@@ -25,6 +25,20 @@ def test_facade_extra_api(golden, tmp_path):
 
 
 @pytest.mark.gpu
+def test_facade_criteria_carry_over(golden, tmp_path):
+    """pcl_b200/pcl_compat/tests/test_facade_loop.cpp on the device: a second align() of one IterativeClosestPoint
+    compares its first iteration with the previous MSE the first align recorded, on the fused device loop and on the
+    staged loop."""
+    subprocess.check_call(["make", "-C", FACADE, "-s", "tests/test_facade_loop"])
+    _write_ascii_pcd(tmp_path / "bun0.pcd", golden["bun0"])
+    _write_binary_pcd(tmp_path / "bun4.pcd", golden["bun4"])
+    r = subprocess.run([os.path.join(FACADE, "tests", "test_facade_loop"), str(tmp_path / "bun0.pcd"),
+                        str(tmp_path / "bun4.pcd")], capture_output=True, text=True)
+    print(r.stdout[-3000:], r.stderr[-2000:])
+    assert r.returncode == 0 and "PASSED" in r.stdout, r.stdout[-3000:]
+
+
+@pytest.mark.gpu
 def test_icp_command_line_example(golden, tmp_path):
     """pcl_b200/pcl_compat/examples/iterative_closest_point.cpp — the flow of the reference's tools/iterative_closest_point.cpp
     (blob PCD in, PointNormal ICP<double> with injected estimators and a one-to-one rejector, concatenateFields, blob PCD

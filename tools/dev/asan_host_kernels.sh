@@ -12,10 +12,10 @@ DEV='-DPCLB_TEST_DEVICE_BUILD -DPCLB_HOST_EMULATION -DPCLB_HOST_EXTRA_SHIMS=\"wa
 LINK="-L$ROOT/oracle -lpcl_oracle -Wl,-rpath,$ROOT/oracle"
 export ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=0
 bad=0
-for t in lbvh lbvh_batch normals_batch fitness_batch traverse search knn_warp icp icp_batch_targets consumers voxel voxel_batch reject reject_sharded shard_target shard_normals shard_cluster shard_filter shard_voxel shard_corr shard_radius; do
+for t in lbvh lbvh_batch normals_batch fitness_batch loop traverse search knn_warp icp icp_batch_targets consumers voxel voxel_batch reject reject_sharded shard_target shard_normals shard_cluster shard_filter shard_voxel shard_corr shard_radius; do
   case $t in lbvh|voxel|voxel_batch|reject|reject_sharded|shard_*) D="";; *) D=$DEV;; esac
   eval g++ $FL $D "$ROOT/tests/host/${t}_host_test.cpp" -o k_$t $LINK 2> build_$t.log || { echo "BUILD FAILED $t"; tail -5 build_$t.log; bad=1; continue; }
-  case $t in icp|icp_batch_targets|lbvh_batch|normals_batch|fitness_batch|consumers|shard_*) args="";; *) args="1";; esac
+  case $t in icp|icp_batch_targets|lbvh_batch|normals_batch|fitness_batch|loop|consumers|shard_*) args="";; *) args="1";; esac
   ./k_$t $args > run_$t.log 2>&1
   rc=$?
   reports=$(grep -c -i -E "AddressSanitizer|runtime error" run_$t.log)

@@ -7,12 +7,12 @@ OUT=${3:-/tmp/pclb_fuzz}
 mkdir -p "$OUT"
 FLAGS="-O1 -std=c++17 -frounding-math -ffp-contract=off -fno-fast-math -I/usr/local/cuda/include -I$ROOT/include -I$ROOT/tests/host -I$ROOT/pcl_b200/pcl_compat"
 LINK="-L$ROOT/oracle -lpcl_oracle -Wl,-rpath,$ROOT/oracle"
-declare -A ARGS=([traverse]="1" [knn_warp]="1" [search]="1" [lbvh]="1" [voxel]="1" [reject]="1" [reject_sharded]="" [icp]="" [consumers]="" [lbvh_batch]="" [normals_batch]="" [fitness_batch]="" [voxel_batch]=""
+declare -A ARGS=([traverse]="1" [knn_warp]="1" [search]="1" [lbvh]="1" [voxel]="1" [reject]="1" [reject_sharded]="" [icp]="" [consumers]="" [lbvh_batch]="" [normals_batch]="" [fitness_batch]="" [voxel_batch]="" [loop]=""
           [shard_target]="" [shard_normals]="" [shard_cluster]="" [shard_filter]="" [shard_voxel]="" [shard_corr]="" [shard_radius]="")
 for t in "${!ARGS[@]}"; do
   for variant in ref dev; do
     [ $variant = dev ] && D="-DPCLB_TEST_DEVICE_BUILD -DPCLB_HOST_EMULATION -DPCLB_HOST_EXTRA_SHIMS=\"warp_emu.h\"" || D=""
-    case $t in lbvh|voxel|voxel_batch|reject|reject_sharded|shard_*) [ $variant = dev ] && continue;; consumers|lbvh_batch|normals_batch|fitness_batch) [ $variant = ref ] && continue;; esac
+    case $t in lbvh|voxel|voxel_batch|reject|reject_sharded|shard_*) [ $variant = dev ] && continue;; consumers|lbvh_batch|normals_batch|fitness_batch|loop) [ $variant = ref ] && continue;; esac
     g++ $FLAGS $D "$ROOT/tests/host/${t}_host_test.cpp" -o "$OUT/${t}_$variant" $LINK 2> "$OUT/${t}_$variant.build.log" || { echo "BUILD FAILED $t $variant"; exit 1; }
   done
 done
